@@ -206,6 +206,30 @@ MPE_API int mpe_rollout_policy(mpe_handle h, void *agent_pv_dev, const void *lm_
                                float *const *obs_n_dev, float *rew_sum_dev, float *rew_steps_dev,
                                float *const *act_record_n, uint8_t *done_dev, uint32_t flags, void *stream);
 
+/* The same closed-loop rollout with MADDPG's actor (mlp_model): obs_dim_i -> hidden -> ReLU -> hidden -> ReLU -> 5,
+ *     logits_i = W3_i relu(W2_i relu(W1_i obs_i + b1_i) + b2_i) + b3_i,
+ * evaluated on the tensor cores (TF32 mma.sync, fp32 accumulation; every operand -- observations, both hidden layers and
+ * all weights -- rounded to TF32 with round-to-nearest, ties away from zero; biases added in fp32).  Weights in torch
+ * nn.Linear layout: w1_n[i] float [hidden][obs_dim_i], b1_n[i] [hidden], w2_n[i] [hidden][hidden], b2_n[i] [hidden],
+ * w3_n[i] [5][hidden], b3_n[i] [5]; hidden = 32 or 64 (both hidden layers).
+ * explore == 0: agent i acts with softmax(logits_i) (MADDPG's mode()).  explore != 0: with the Gumbel-softmax sample
+ * softmax(logits_i - log(-log u)) (SoftCategoricalPd.sample), u_0..u_4 drawn from Philox4x32-10 with key = explore_seed
+ * and counter = (world_offset + w lo, hi, explore_epoch lo, 0x40000000 | ((t * A + i) * 2 + b)): u_0..u_3 are block
+ * b = 0, u_4 is word 0 of block b = 1, u = ((bits >> 8) + 0.5) * 2^-24 with the sum rounded toward zero in fp32.  The
+ * draw depends on the global world index, not on the batch it runs in.
+ * Records (NULL: not written): act_record_n[i] float [n_steps][n_env][5], the action applied (the sample when
+ * exploring); obs_record_n[i] float [n_steps][n_env][obs_dim_i] (16-byte aligned), the observation agent i acted on at
+ * step t; rew_steps_dev as in mpe_rollout_policy.  Feeding act_record_n to mpe_step reproduces state, observations and
+ * rewards bit for bit.  Same programs as mpe_rollout_policy; otherwise, or for another hidden width, MPE_ERR_UNSUPPORTED. */
+MPE_API int mpe_rollout_policy_mlp(mpe_handle h, void *agent_pv_dev, const void *lm_p_dev, float *comm_dev,
+                                   const int32_t *goal_dev, const float *const *w1_n, const float *const *b1_n,
+                                   const float *const *w2_n, const float *const *b2_n, const float *const *w3_n,
+                                   const float *const *b3_n, int32_t hidden, int32_t n_steps, int32_t explore,
+                                   uint64_t explore_seed, uint64_t explore_epoch, uint64_t world_offset,
+                                   float *const *obs_n_dev, float *rew_sum_dev, float *rew_steps_dev,
+                                   float *const *act_record_n, float *const *obs_record_n, uint8_t *done_dev,
+                                   uint32_t flags, void *stream);
+
 /* Same step for a caller that holds HOST buffers (what the reference's callers hold):
  * act_n_host[i] -> (async H2D into act_n_dev[i]) -> mpe_step -> (async D2H) obs_n_host[i],
  * rew_host, done_host, all ordered on `stream`.  Host buffers should be pinned for the copies

@@ -994,6 +994,341 @@ template <> struct PolicyBuilt<Simple<1, 1>> { static constexpr bool value = tru
 template <> struct PolicyBuilt<Spread<3>> { static constexpr bool value = true; };
 template <> struct PolicyBuilt<Tag<3, 1, 2>> { static constexpr bool value = true; };
 
+
+// ---- K-step closed-loop rollout with MADDPG's two-hidden-layer actor on the tensor cores ---------------------------
+// The persistent structure of mpe_policy_rollout_kernel (state in registers for all T steps, nothing read from HBM per
+// step, the same physics<P> / P::reward / P::observe<I>) with the MADDPG actor (mlp_model)
+//     logits_i = W3_i relu(W2_i relu(W1_i obs_i + b1_i) + b2_i) + b3_i       obs_dim_i -> H -> H -> 5,  H = 32 or 64
+// evaluated by the warp as three TF32 GEMMs with mma.sync.m16n8k8 (fp32 accumulation):
+//     [32 x K1] . [K1 x H] -> ReLU -> [32 x H] . [H x H] -> ReLU -> [32 x H] . [H x 8]
+// One warp = 32 worlds = two m16 tiles.  Each lane writes its observation row into the warp's observation tile (the
+// layout of the fused step's coalesced tile store, ObsTile<obs_dim>); the A fragments are read from it with the columns
+// at and beyond obs_dim read as zero, so K1 = obs_dim rounded up to 8.  The accumulators of one layer are the A fragments
+// of the next without any data movement: within a k-tile a lane holds hidden units 2q and 2q+1 of rows g and g+8 and
+// the next layer's B fragments are staged with the same permutation of k.  Layers 2 and 3 are interleaved per 8-unit
+// tile of h2, so h2 never exists as a whole.  The 5 logits (padded to 8) go back to their lane through a small
+// shared-memory tile; that lane does the softmax (or the Gumbel-softmax sample), the _set_action decode and the step.
+// Rounding: every tensor-core operand -- observations, h1, h2 and all weights -- is converted with cvt.rna.tf32.f32
+// (round to nearest, ties away from zero, to 10 mantissa bits); the weights once, while they are staged.  Biases are
+// the accumulators' fp32 initial values.
+// Exploration (explore != 0): agent i at step t acts with softmax(logits - log(-log u)) (SoftCategoricalPd.sample), in
+// fp32 with logf.  u_0..u_4 come from Philox4x32-10 with key = explore_seed and counter = (global world index lo, hi,
+// low 32 bits of explore_epoch, kExploreTag | ((t * A + i) * 2 + b)): u_0..u_3 are the four words of block b = 0, u_4
+// word 0 of block b = 1; u = ((bits >> 8) + 0.5) * 2^-24 with the sum rounded toward zero in fp32 (exact below 2^23,
+// the half is dropped above), so u lies in [2^-25, 1 - 2^-24].  The tag bit keeps this stream apart from reset_kernel's
+// counters, so an exploration seed equal to the env seed does not correlate the noise with initial positions; the
+// global world index (world_offset + w) makes the noise independent of sharding.
+constexpr uint32_t kExploreTag = 0x40000000u;
+// Warps per block at most: one copy of the weights serves all of them, and with 75-90 KB of weights one block is what
+// fits an SM, so this is also the residency.  16 warps leave 128 registers per thread; tag 3+1 at H = 64 (four agents'
+// state next to the 64 registers of h1) needs more than that, and gets 12-warp blocks and up to 168 registers instead.
+template <class P, int H>
+__host__ __device__ constexpr int mlp_block_warps() { return (H == 64 && P::A >= 4) ? 12 : 16; }
+
+struct MlpPolicyArgs {
+    StepArgs s;
+    int32_t T;
+    int32_t explore;
+    uint64_t seed, epoch, world_offset;
+    float *rew_steps;               // [T][A][n] or null
+    float *act_rec[kMaxA];          // [T][n][5] per agent, or null: the action applied (sampled when exploring)
+    float *obs_rec[kMaxA];          // [T][n][obs_dim_i] per agent, or null: the observation the actor saw at step t
+    const float *w1[kMaxA], *b1[kMaxA];   // torch nn.Linear layout: [H][obs_dim_i], [H]
+    const float *w2[kMaxA], *b2[kMaxA];   // [H][H], [H]
+    const float *w3[kMaxA], *b3[kMaxA];   // [5][H], [5]
+};
+static_assert(sizeof(MlpPolicyArgs) <= 4096, "kernel parameter space");
+
+template <class P, int H>
+struct MlpShape {
+    static constexpr int NT = H / 8;                                   // n-tiles of a hidden layer (= its k-tiles)
+    __host__ __device__ static constexpr int kt1(int i) { return (P::obs_dim(i) + 7) / 8; }
+    // per agent, in floats: B fragments [k-tile][n-tile][lane][2] of W1, W2, W3, then b1 [H], b2 [H], b3 [8]
+    __host__ __device__ static constexpr int w2_off(int i) { return 64 * kt1(i) * NT; }
+    __host__ __device__ static constexpr int w3_off(int i) { return w2_off(i) + 64 * NT * NT; }
+    __host__ __device__ static constexpr int b1_off(int i) { return w3_off(i) + 64 * NT; }
+    __host__ __device__ static constexpr int b2_off(int i) { return b1_off(i) + H; }
+    __host__ __device__ static constexpr int b3_off(int i) { return b2_off(i) + H; }
+    __host__ __device__ static constexpr int agent_floats(int i) { return b3_off(i) + 8; }
+    __host__ __device__ static constexpr int agent_off(int i) { int s = 0; for (int j = 0; j < i; ++j) s += agent_floats(j); return s; }
+    static constexpr int kWeightFloats = agent_off(P::A);
+    // per warp: [observation tile][logit tile 32 x 9]; the final observations are written through the same tile
+    __host__ __device__ static constexpr int obs_tile_floats() { int m = 0; for (int i = 0; i < P::A; ++i) m = 32 * Shape<P>::obs_pitch(i) > m ? 32 * Shape<P>::obs_pitch(i) : m; return (m + 3) & ~3; }
+    static constexpr int kLogitPitch = 9;
+    static constexpr int kLogitOff = obs_tile_floats();
+    static constexpr int kWarpFloats = (kLogitOff + 32 * kLogitPitch + 3) & ~3;
+    static_assert(MPE_COMPACT_OBS, "write_observations must use one shared observation slot");
+    static_assert(Shape<P>::kWarpFloats - Shape<P>::obs_base() <= kLogitOff, "final observations fit the tile");
+};
+
+__device__ __forceinline__ uint32_t to_tf32(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return r;
+}
+// d += a . b, one m16n8k8 TF32 tile (A row-major 16 x 8, B column-major 8 x 8, fp32 accumulators)
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], float2 b) {
+    asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(__float_as_uint(b.x)), "r"(__float_as_uint(b.y)));
+}
+
+// W ([NV][KV], torch Linear layout, global) -> TF32 B fragments in shared memory, [KT][NTT][lane][2], zero outside
+// [NV][KV].  Fragment element j of lane l in tile (kt, nt) is B[k][n] = W[n][k] with n = nt*8 + l/4 and
+// k = kt*8 + l%4 + 4j (PERM = false: A comes from the observation tile) or k = kt*8 + 2(l%4) + j (PERM = true: A is the
+// previous layer's accumulator fragment).  Consecutive lanes read consecutive float2: conflict-free LDS.64.
+template <int KT, int NTT, bool PERM>
+__device__ __forceinline__ void stage_fragments(float *dst, const float *__restrict__ W, int NV, int KV) {
+    for (int q = threadIdx.x; q < KT * NTT * 64; q += blockDim.x) {
+        const int j = q & 1, l = (q >> 1) & 31, tile = q >> 6;
+        const int nt = tile % NTT, kt = tile / NTT;
+        const int nn = nt * 8 + (l >> 2);
+        const int k = kt * 8 + (PERM ? 2 * (l & 3) + j : (l & 3) + 4 * j);
+        dst[q] = __uint_as_float(to_tf32((nn < NV && k < KV) ? W[nn * KV + k] : 0.0f));
+    }
+}
+
+// accumulator fragment -> ReLU -> TF32 A fragment of the next layer (k order permuted as in stage_fragments)
+__device__ __forceinline__ void relu_tf32_frag(uint32_t (&a)[4], const float (&c)[4]) {
+    a[0] = to_tf32(fmaxf(c[0], 0.0f));   // row g,   k = 2q
+    a[1] = to_tf32(fmaxf(c[2], 0.0f));   // row g+8, k = 2q
+    a[2] = to_tf32(fmaxf(c[1], 0.0f));   // row g,   k = 2q+1
+    a[3] = to_tf32(fmaxf(c[3], 0.0f));   // row g+8, k = 2q+1
+}
+
+// one agent of the tensor-core actor for the warp's 32 worlds: observation -> tile -> 3 GEMMs -> this lane's logits ->
+// (Gumbel-)softmax -> decoded (u.x, u.y).  Called by all 32 lanes (mma.sync is warp-collective).
+template <class P, int H, int I>
+__device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typename P::W &w, const float *__restrict__ Wsm,
+                                            float *s_warp, int lane, int t, int rows, bool active, int64_t w0, int64_t wi) {
+    using S = MlpShape<P, H>;
+    constexpr int OD = P::obs_dim(I), KT1 = S::kt1(I), NT = S::NT, PITCH = ObsTile<OD>::kPitch;
+    const DevDesc &d = pa.s.d;
+    const int64_t n = pa.s.n;
+    float *tile = s_warp;
+    float *lgs = s_warp + S::kLogitOff;
+    {
+        TileWriter<OD> o(tile, lane);
+        P::template observe<I>(d, w, o);                   // scenario.observation(agent I) -> this lane's tile row
+    }
+    __syncwarp();
+    if (pa.obs_rec[I] != nullptr) {                        // the observation the actor sees at step t
+        float *g = pa.obs_rec[I] + (static_cast<int64_t>(t) * n + w0) * OD;
+        if (rows == 32 && (reinterpret_cast<uintptr_t>(g) & 15u) == 0) {
+            obs_tile_store<OD>(g, tile, lane);             // LDS.128 -> STG.128, as the fused step's observations
+        } else if (active) {
+#pragma unroll
+            for (int k = 0; k < OD; ++k) g[lane * OD + k] = tile[lane * PITCH + k];
+        }
+    }
+    const int gq = lane >> 2, tq = lane & 3;
+    // ---- layer 1: [32 x K1] . [K1 x H] + b1 ----
+    float h[2][NT][4];
+    const float *B1 = Wsm + S::b1_off(I);
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+        const float2 b = *reinterpret_cast<const float2 *>(B1 + nt * 8 + 2 * tq);
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) { h[mt][nt][0] = b.x; h[mt][nt][1] = b.y; h[mt][nt][2] = b.x; h[mt][nt][3] = b.y; }
+    }
+#pragma unroll
+    for (int kt = 0; kt < KT1; ++kt) {
+        uint32_t a[2][4];
+        const int c0 = kt * 8 + tq, c1 = c0 + 4;
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+            const float *r0 = tile + (mt * 16 + gq) * PITCH, *r1 = r0 + 8 * PITCH;
+            if (kt * 8 + 8 <= OD) {
+                a[mt][0] = to_tf32(r0[c0]); a[mt][1] = to_tf32(r1[c0]);
+                a[mt][2] = to_tf32(r0[c1]); a[mt][3] = to_tf32(r1[c1]);
+            } else {                                       // columns >= obs_dim are the zero padding of K1
+                a[mt][0] = to_tf32(c0 < OD ? r0[c0] : 0.0f); a[mt][1] = to_tf32(c0 < OD ? r1[c0] : 0.0f);
+                a[mt][2] = to_tf32(c1 < OD ? r0[c1] : 0.0f); a[mt][3] = to_tf32(c1 < OD ? r1[c1] : 0.0f);
+            }
+        }
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) {
+            const float2 b = *reinterpret_cast<const float2 *>(Wsm + ((kt * NT + nt) * 32 + lane) * 2);
+            mma_tf32(h[0][nt], a[0], b);
+            mma_tf32(h[1][nt], a[1], b);
+        }
+    }
+    uint32_t x1[2][NT][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) relu_tf32_frag(x1[mt][nt], h[mt][nt]);
+    // ---- layers 2 and 3, one 8-unit tile of h2 at a time: logits += relu(x1 . W2^T[:, tile] + b2[tile]) . W3^T[tile, :]
+    const float *W2 = Wsm + S::w2_off(I), *W3 = Wsm + S::w3_off(I), *B2 = Wsm + S::b2_off(I), *B3 = Wsm + S::b3_off(I);
+    float lg[2][4];
+    {
+        const float2 b = *reinterpret_cast<const float2 *>(B3 + 2 * tq);
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) { lg[mt][0] = b.x; lg[mt][1] = b.y; lg[mt][2] = b.x; lg[mt][3] = b.y; }
+    }
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+        float c[2][4];
+        const float2 bb = *reinterpret_cast<const float2 *>(B2 + nt * 8 + 2 * tq);
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) { c[mt][0] = bb.x; c[mt][1] = bb.y; c[mt][2] = bb.x; c[mt][3] = bb.y; }
+#pragma unroll
+        for (int kt = 0; kt < NT; ++kt) {
+            const float2 b = *reinterpret_cast<const float2 *>(W2 + ((kt * NT + nt) * 32 + lane) * 2);
+            mma_tf32(c[0], x1[0][kt], b);
+            mma_tf32(c[1], x1[1][kt], b);
+        }
+        const float2 b3 = *reinterpret_cast<const float2 *>(W3 + (nt * 32 + lane) * 2);
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+            uint32_t x2[4];
+            relu_tf32_frag(x2, c[mt]);
+            mma_tf32(lg[mt], x2, b3);
+        }
+    }
+    // ---- logits back to their lane (row r = world w0 + r) ----
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt) {
+        float *r0 = lgs + (mt * 16 + gq) * S::kLogitPitch + 2 * tq, *r1 = r0 + 8 * S::kLogitPitch;
+        r0[0] = lg[mt][0]; r0[1] = lg[mt][1];
+        r1[0] = lg[mt][2]; r1[1] = lg[mt][3];
+    }
+    __syncwarp();
+    float z[5];
+#pragma unroll
+    for (int c = 0; c < 5; ++c) z[c] = lgs[lane * S::kLogitPitch + c];
+    if (pa.explore) {                                      // Gumbel-softmax sample (see the definition above)
+        const uint64_t gw = pa.world_offset + static_cast<uint64_t>(wi);
+        const uint2 key = make_uint2(static_cast<uint32_t>(pa.seed), static_cast<uint32_t>(pa.seed >> 32));
+        const uint32_t c3 = kExploreTag | (static_cast<uint32_t>(t * P::A + I) * 2u);
+        const uint4 ctr = make_uint4(static_cast<uint32_t>(gw), static_cast<uint32_t>(gw >> 32), static_cast<uint32_t>(pa.epoch), c3);
+        const uint4 r0 = philox4x32_10(ctr, key);
+        const uint4 r1 = philox4x32_10(make_uint4(ctr.x, ctr.y, ctr.z, c3 | 1u), key);
+        const uint32_t bits[5] = {r0.x, r0.y, r0.z, r0.w, r1.x};
+#pragma unroll
+        for (int c = 0; c < 5; ++c) {
+            const float u = __fmul_rn(__fadd_rz(static_cast<float>(bits[c] >> 8), 0.5f), 0x1p-24f);
+            z[c] = __fsub_rn(z[c], logf(-logf(u)));
+        }
+    }
+    const float m = fmaxf(fmaxf(fmaxf(z[0], z[1]), fmaxf(z[2], z[3])), z[4]);
+    float e[5], sum = 0.0f;
+#pragma unroll
+    for (int c = 0; c < 5; ++c) { e[c] = expf(__fsub_rn(z[c], m)); sum = __fadd_rn(sum, e[c]); }
+    float pr[5];
+#pragma unroll
+    for (int c = 0; c < 5; ++c) pr[c] = __fdiv_rn(e[c], sum);
+    if (pa.act_rec[I] != nullptr && active) {
+        float *rec = pa.act_rec[I] + (static_cast<int64_t>(t) * n + wi) * 5;
+#pragma unroll
+        for (int c = 0; c < 5; ++c) rec[c] = pr[c];
+    }
+    // _set_action (environment.py:173-181), the arithmetic of decode_rows
+    float x = 0.0f, y = 0.0f;
+    x += pr[1] - pr[2];
+    y += pr[3] - pr[4];
+    return make_float2(__fmul_rn(x, d.a_sens[I]), __fmul_rn(y, d.a_sens[I]));
+}
+
+template <class P, int H>
+__global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_rollout_kernel(const __grid_constant__ MlpPolicyArgs pa) {
+    static_assert(P::NS == 0 && (H == 32 || H == 64), "MLP policy rollout: silent agents, hidden width 32 or 64");
+    constexpr int A = P::A, L = P::L;
+    using S = MlpShape<P, H>;
+    const StepArgs &a = pa.s;
+    extern __shared__ __align__(16) float smem[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    // ---- all agents' weights -> TF32 B fragments in shared memory, once per block ----
+    static_for<A>([&](auto ic) {
+        constexpr int i = decltype(ic)::value;
+        constexpr int OD = P::obs_dim(i);
+        float *base = smem + S::agent_off(i);
+        stage_fragments<S::kt1(i), S::NT, false>(base, pa.w1[i], H, OD);
+        stage_fragments<S::NT, S::NT, true>(base + S::w2_off(i), pa.w2[i], H, H);
+        stage_fragments<S::NT, 1, true>(base + S::w3_off(i), pa.w3[i], 5, H);
+        for (int q = threadIdx.x; q < H; q += blockDim.x) {
+            base[S::b1_off(i) + q] = pa.b1[i][q];
+            base[S::b2_off(i) + q] = pa.b2[i][q];
+        }
+        for (int q = threadIdx.x; q < 8; q += blockDim.x) base[S::b3_off(i) + q] = q < 5 ? pa.b3[i][q] : 0.0f;
+    });
+    __syncthreads();
+
+    const int64_t n = a.n;
+    const int64_t end = a.begin + a.count;
+    const int64_t w0 = a.begin + (static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + warp) * 32;
+    if (w0 >= end) return;
+    const int rows = (end - w0) < 32 ? static_cast<int>(end - w0) : 32;
+    const bool active = lane < rows;
+    const int64_t wi = w0 + (active ? lane : 0);   // idle lanes of a partial tile replay world w0: every tile row is finite
+    float *s_warp = smem + S::kWeightFloats + warp * S::kWarpFloats;
+    const DevDesc &d = a.d;
+
+    typename P::W w;
+#pragma unroll
+    for (int i = 0; i < A; ++i) {
+        const float4 v = state_load(a.pv + i * n + wi);
+        w.px[i] = v.x; w.py[i] = v.y; w.vx[i] = v.z; w.vy[i] = v.w;
+    }
+#pragma unroll
+    for (int l = 0; l < L; ++l) {
+        const float2 v = state_load(a.lm + l * n + wi);
+        w.lx[l] = v.x; w.ly[l] = v.y;
+    }
+    if constexpr (P::G > 0) {
+#pragma unroll
+        for (int q = 0; q < P::G; ++q) w.g[q] = a.goal[q * n + wi];
+    }
+
+    float rsum[A];
+#pragma unroll
+    for (int i = 0; i < A; ++i) rsum[i] = 0.0f;
+#pragma unroll 1
+    for (int t = 0; t < pa.T; ++t) {
+        float ux[A], uy[A];
+        P::prepare(d, w);
+        static_for<A>([&](auto ic) {
+            constexpr int i = decltype(ic)::value;
+            const float2 u = mlp_agent<P, H, i>(pa, w, smem + S::agent_off(i), s_warp, lane, t, rows, active, w0, wi);
+            ux[i] = u.x;
+            uy[i] = u.y;
+        });
+        physics<P>(d, w, ux, uy);
+        float rew[A];
+        P::reward(d, w, rew, nullptr);
+        if (a.flags & MPE_FLAG_SHARED_REWARD) {
+            float sum = 0.0f;
+#pragma unroll
+            for (int i = 0; i < A; ++i) sum += rew[i];
+#pragma unroll
+            for (int i = 0; i < A; ++i) rew[i] = sum;
+        }
+#pragma unroll
+        for (int i = 0; i < A; ++i) rsum[i] = __fadd_rn(rsum[i], rew[i]);
+        if (pa.rew_steps != nullptr && active) {
+#pragma unroll
+            for (int i = 0; i < A; ++i) pa.rew_steps[(static_cast<int64_t>(t) * A + i) * n + wi] = rew[i];
+        }
+    }
+    if (active) {
+#pragma unroll
+        for (int i = 0; i < A; ++i)
+            if (P::movable(i)) a.pv[i * n + wi] = make_float4(w.px[i], w.py[i], w.vx[i], w.vy[i]);
+    }
+    P::prepare(d, w);
+    __syncwarp();                  // every lane has read its logits before the tile is reused
+    // write_observations addresses the observation slot at Shape<P>::obs_off(i) == obs_base(): shift the base so that
+    // the slot is this warp's observation tile
+    write_observations<P>(a, d, w, s_warp - Shape<P>::obs_base(), lane, rows, active, w0, wi, -1);
+    if (active) {
+#pragma unroll
+        for (int i = 0; i < A; ++i) {
+            a.rew[i * n + wi] = rsum[i];
+            a.done[i * n + wi] = 0;
+        }
+    }
+}
+
 // ---- generic program for user scenarios (MPE_SCN_CUSTOM) ------------------------------------------
 // Any entity table, flags read at run time; same arithmetic primitives and the same (a, b) pair order as
 // the compiled programs, so for a table that matches a built-in scenario the state is bit-identical.
@@ -1198,6 +1533,8 @@ struct Program {
     int pipe_smem;      // dynamic shared memory per WARP of the pipelined kernel
     void (*policy_fn[2])(PolicyArgs);  // K-step closed-loop rollout, hidden width 32 / 64 (null: not built for this program)
     int policy_weight_floats[2];
+    void (*mlp_fn[2])(MlpPolicyArgs);  // the same with the two-hidden-layer actor on the tensor cores, H = 32 / 64
+    int mlp_weight_floats[2], mlp_warp_floats[2], mlp_warps[2];
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
     int rollout_smem;   // dynamic shared memory per WARP of the rollout kernel
     KernelFn lanes_fn;  // lane-per-agent fused step (simple_spread only), else null
@@ -1234,6 +1571,14 @@ static Program make_program() {
         p.policy_fn[1] = mpe_policy_rollout_kernel<P, 64>;
         p.policy_weight_floats[0] = PolicyShape<P, 32>::kWeightFloats;
         p.policy_weight_floats[1] = PolicyShape<P, 64>::kWeightFloats;
+        p.mlp_fn[0] = mpe_policy_mlp_rollout_kernel<P, 32>;
+        p.mlp_fn[1] = mpe_policy_mlp_rollout_kernel<P, 64>;
+        p.mlp_weight_floats[0] = MlpShape<P, 32>::kWeightFloats;
+        p.mlp_weight_floats[1] = MlpShape<P, 64>::kWeightFloats;
+        p.mlp_warp_floats[0] = MlpShape<P, 32>::kWarpFloats;
+        p.mlp_warp_floats[1] = MlpShape<P, 64>::kWarpFloats;
+        p.mlp_warps[0] = mlp_block_warps<P, 32>();
+        p.mlp_warps[1] = mlp_block_warps<P, 64>();
     }
     p.smem_bytes = Shape<P>::kWarpBytes;  // per warp
     p.A = P::A; p.L = P::L; p.NS = P::NS; p.DIMC = P::DIMC; p.INFO = P::INFO; p.G = P::G;
@@ -1379,6 +1724,10 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
             if (prog->policy_fn[k])
                 CUDA_TRY(cudaFuncSetAttribute(prog->policy_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               prog->policy_weight_floats[k] * 4 + prog->smem_bytes * 4));
+        for (int k = 0; k < 2; ++k)
+            if (prog->mlp_fn[k])
+                CUDA_TRY(cudaFuncSetAttribute(prog->mlp_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp_warps[k]) * 4));
         if (prog->rollout_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->rollout_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->rollout_smem * max_warps_per_block(prog->rollout_smem)));
@@ -1826,6 +2175,69 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
                                      dim3(32 * wpb), params, smem, static_cast<cudaStream_t>(stream));
     if (prev != h->device) cudaSetDevice(prev);
     if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchKernel(rollout_policy)");
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    return MPE_OK;
+}
+
+extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
+                                      const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
+                                      const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
+                                      int32_t hidden, int32_t n_steps, int32_t explore, uint64_t explore_seed,
+                                      uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n, float *rew_sum,
+                                      float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
+                                      uint8_t *done, uint32_t flags, void *stream) {
+    if (!h || n_steps < 0 || !w1_n || !b1_n || !w2_n || !b2_n || !w3_n || !b3_n) return MPE_ERR_BAD_ARG;
+    if (h->device < 0) return MPE_ERR_NO_DEVICE;
+    const int k = hidden == 32 ? 0 : (hidden == 64 ? 1 : -1);
+    if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || h->prog->mlp_fn[k] == nullptr) return MPE_ERR_UNSUPPORTED;
+    if (flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
+    if (rew_steps != nullptr && !ok4(rew_steps)) return MPE_ERR_BAD_ARG;
+    // the Philox counter word holds (t * A + i) * 2 + b below the tag bit
+    if (explore && static_cast<int64_t>(n_steps) * h->prog->A * 2 > static_cast<int64_t>(kExploreTag)) return MPE_ERR_BAD_ARG;
+    NvtxRange range("mpe_rollout_policy_mlp");
+    MlpPolicyArgs pa{};
+    StepArgs &a = pa.s;
+    int r = fill_state(h, a, pv, lm, comm, goal);
+    if (r) return r;
+    r = fill_outputs(h, a, obs_n, rew_sum, done, nullptr);
+    if (r) return r;
+    for (int i = 0; i < h->prog->A; ++i) {
+        if (!ok4(w1_n[i]) || !ok4(b1_n[i]) || !ok4(w2_n[i]) || !ok4(b2_n[i]) || !ok4(w3_n[i]) || !ok4(b3_n[i]))
+            return MPE_ERR_BAD_ARG;
+        pa.w1[i] = w1_n[i]; pa.b1[i] = b1_n[i]; pa.w2[i] = w2_n[i]; pa.b2[i] = b2_n[i]; pa.w3[i] = w3_n[i]; pa.b3[i] = b3_n[i];
+        pa.act_rec[i] = act_record_n ? act_record_n[i] : nullptr;
+        if (pa.act_rec[i] != nullptr && !ok4(pa.act_rec[i])) return MPE_ERR_BAD_ARG;
+        pa.obs_rec[i] = obs_record_n ? obs_record_n[i] : nullptr;
+        if (pa.obs_rec[i] != nullptr && !ok16(pa.obs_rec[i])) return MPE_ERR_BAD_ARG;   // 16-byte tile stores
+    }
+    a.info = nullptr;
+    a.flags = flags;
+    a.d = h->dev;
+    a.n = h->n;
+    a.begin = 0;
+    a.count = h->n;
+    pa.T = n_steps;
+    pa.explore = explore ? 1 : 0;
+    pa.seed = explore_seed;
+    pa.epoch = explore_epoch;
+    pa.world_offset = world_offset;
+    pa.rew_steps = rew_steps;
+    // every block stages all agents' weights once, so blocks are as large as possible while every SM still gets work
+    const int64_t warps = (h->n + 31) / 32;
+    int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
+    if (wpb < 1) wpb = 1;
+    if (wpb > h->prog->mlp_warps[k]) wpb = h->prog->mlp_warps[k];
+    const int64_t blocks = (warps + wpb - 1) / wpb;
+    if (blocks > 0x7fffffffLL) return MPE_ERR_BAD_ARG;
+    int prev = 0;
+    CUDA_TRY(cudaGetDevice(&prev));
+    if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
+    void *params[] = {&pa};
+    const size_t smem = (static_cast<size_t>(h->prog->mlp_weight_floats[k]) + static_cast<size_t>(h->prog->mlp_warp_floats[k]) * wpb) * 4;
+    cudaError_t e = cudaLaunchKernel(reinterpret_cast<const void *>(h->prog->mlp_fn[k]), dim3(static_cast<unsigned>(blocks)),
+                                     dim3(static_cast<unsigned>(32 * wpb)), params, smem, static_cast<cudaStream_t>(stream));
+    if (prev != h->device) cudaSetDevice(prev);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchKernel(rollout_policy_mlp)");
     __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     return MPE_OK;
 }

@@ -54,6 +54,9 @@ class MultiAgentEnv(_Env):
         #: next step).  Host callers: results are views of two flip-flopped pinned slabs (valid until the
         #: next-but-one step).  Default False = the reference's ownership: every step returns fresh arrays.
         self.reuse_buffers = False
+        #: exploration epoch of rollout_policy(..., explore_seed=s): part of the noise counter, advanced by one per
+        #: exploring call, so consecutive calls draw fresh noise and a new env with the same seed replays the sequence
+        self.explore_epoch = 0
 
         self._custom = (getattr(world, "native_program", None) == "custom")
         if self._custom and not world.batched:
@@ -240,15 +243,27 @@ class MultiAgentEnv(_Env):
             return obs_n, reward_n, done_n, info_n, rew_steps
         return obs_n, reward_n, done_n, info_n
 
-    def rollout_policy(self, policies, n_steps, record_actions=False, per_step_rewards=False):
-        """T closed-loop steps in ONE kernel launch with the actors inside the kernel (mpe_rollout_policy): agent i acts
-        with softmax(W2_i relu(W1_i obs_i + b1_i) + b2_i).  policies[i] is a `torch.nn.Sequential(Linear(obs_dim_i, H),
-        ReLU(), Linear(H, 5))` or the tuple (W1 [H, obs_dim_i], b1 [H], W2 [5, H], b2 [5]) in torch's Linear layout, H = 32
-        or 64.  Returns (obs_n, reward_sum_n, done_n, info_n, extras) for the state after the last step; extras["actions"]
+    def rollout_policy(self, policies, n_steps, record_actions=False, per_step_rewards=False, record_observations=False,
+                       explore_seed=None):
+        """T closed-loop steps in ONE kernel launch with the actors inside the kernel.
+
+        One hidden layer (mpe_rollout_policy, fp32): agent i acts with softmax(W2_i relu(W1_i obs_i + b1_i) + b2_i).
+        policies[i] is a `torch.nn.Sequential(Linear(obs_dim_i, H), ReLU(), Linear(H, 5))` or the tuple (W1 [H, obs_dim_i],
+        b1 [H], W2 [5, H], b2 [5]) in torch's Linear layout, H = 32 or 64.
+
+        Two hidden layers, MADDPG's actor (mpe_rollout_policy_mlp, TF32 tensor cores): policies[i] is a
+        `torch.nn.Sequential(Linear(obs_dim_i, H), ReLU(), Linear(H, H), ReLU(), Linear(H, 5))` or the tuple (W1, b1, W2,
+        b2, W3, b3), H = 32 or 64.  explore_seed (an int) makes every agent act with the Gumbel-softmax sample
+        softmax(logits - log(-log u)) instead of softmax(logits); the noise is keyed by (explore_seed, self.explore_epoch,
+        global world index, step, agent) and self.explore_epoch advances by one per exploring call.
+        record_observations=True returns extras["observations"], a list of [T, N, obs_dim_i] tensors: the observation
+        agent i acted on at each step.  Both options need the two-hidden-layer actor.
+
+        Returns (obs_n, reward_sum_n, done_n, info_n, extras) for the state after the last step; extras["actions"]
         (record_actions) is a list of [T, N, 5] tensors with the actions taken, extras["rewards"] (per_step_rewards) a
-        [T, n, N] tensor.  World state lives in registers for all T steps and no observation is written in between.
-        Batched CUDA mode; scenarios whose agents all move and are silent and whose program was built with the policy
-        kernel (simple, simple_spread N=3, simple_tag 3+1) -- anything else raises."""
+        [T, n, N] tensor.  World state lives in registers for all T steps.  Batched CUDA mode; scenarios whose agents all
+        move and are silent and whose program was built with the policy kernels (simple, simple_spread N=3, simple_tag
+        3+1) -- anything else raises."""
         import torch
         world = self.world
         if not world.batched:
@@ -257,6 +272,12 @@ class MultiAgentEnv(_Env):
             raise NotImplementedError("rollout_policy: compiled scenarios with plain action vectors only")
         if len(policies) != self.n:
             raise ValueError("expected %d policies, got %d" % (self.n, len(policies)))
+        if any(_has_two_hidden_layers(p) for p in policies):
+            return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
+                                            explore_seed)
+        if record_observations or explore_seed is not None:
+            raise NotImplementedError("rollout_policy: observation records and exploration need the two-hidden-layer "
+                                      "actor (Linear -> ReLU -> Linear -> ReLU -> Linear)")
         nw = world.bind()
         N, T = nw.n_env, int(n_steps)
         keep, hidden = [], None
@@ -288,6 +309,32 @@ class MultiAgentEnv(_Env):
         world._obs_valid = False
         info_n = {'n': [{} for _ in range(self.n)]}
         return list(out.obs), list(out.rew_list), list(out.done_list), info_n, {"actions": actions, "rewards": rew_steps}
+
+    def _rollout_policy_mlp(self, policies, n_steps, record_actions, per_step_rewards, record_observations, explore_seed):
+        import torch
+        world = self.world
+        nw = world.bind()
+        N, T = nw.n_env, int(n_steps)
+        params, hidden = mlp_actor_params(policies, nw.obs_dims)
+        keep = [[t.detach().to(device=nw.device, dtype=torch.float32).contiguous() for t in p] for p in params]
+        w_ptrs = [_lib.ptr_array([keep[i][j].data_ptr() for i in range(self.n)]) for j in range(6)]
+        out = nw.out if self.reuse_buffers else nw.new_outputs()
+        dev = dict(dtype=torch.float32, device=nw.device)
+        rew_steps = torch.empty((T, self.n, N), **dev) if per_step_rewards else None
+        actions = [torch.empty((T, N, 5), **dev) for _ in range(self.n)] if record_actions else None
+        observations = [torch.empty((T, N, od), **dev) for od in nw.obs_dims] if record_observations else None
+        seed = None if explore_seed is None else int(explore_seed) & 0xFFFFFFFFFFFFFFFF
+        nw.rollout_policy_mlp(w_ptrs, hidden, T, out, self._flags(), rew_steps,
+                              _lib.ptr_array([a.data_ptr() for a in actions]) if actions is not None else None,
+                              _lib.ptr_array([o.data_ptr() for o in observations]) if observations is not None else None,
+                              explore_seed=seed, explore_epoch=self.explore_epoch)
+        if seed is not None:
+            self.explore_epoch += 1
+        self._last_out = out
+        world._obs_valid = False
+        info_n = {'n': [{} for _ in range(self.n)]}
+        return list(out.obs), list(out.rew_list), list(out.done_list), info_n, \
+            {"actions": actions, "rewards": rew_steps, "observations": observations}
 
     # ---- user scenarios: native _set_action + World.step, callbacks in the user's torch code -------
     def _step_custom(self, action_n, nw, flags):
@@ -544,3 +591,55 @@ class MultiAgentEnv(_Env):
             center = (0.0, 0.0) if self.shared_viewer else tuple(pv[i, 0:2])
             results.append(draw_world(pos, sizes, colors, alphas, center=center))
         return results
+
+
+# ---- the two-hidden-layer actor of rollout_policy (MADDPG's mlp_model) ------------------------------
+_MLP_SHAPE = "nn.Sequential(Linear(obs_dim, H), ReLU(), Linear(H, H), ReLU(), Linear(H, 5)) or a tuple (W1, b1, W2, b2, W3, b3)"
+
+
+def _has_two_hidden_layers(pol):
+    """does this policy ask for the two-hidden-layer actor?  (A 6-tuple, or a module with three Linear layers; whether
+    the module really is Linear -> ReLU -> Linear -> ReLU -> Linear is checked by mlp_actor_params.)"""
+    import torch
+    if isinstance(pol, torch.nn.Module):
+        return sum(isinstance(m, torch.nn.Linear) for m in pol.modules()) == 3
+    return isinstance(pol, (tuple, list)) and len(pol) == 6
+
+
+def mlp_actor_params(policies, obs_dims):
+    """policies -> ([(W1, b1, W2, b2, W3, b3) per agent], H) in torch's Linear layout, or ValueError.  A module must be
+    an nn.Sequential whose layers are exactly Linear, ReLU, Linear, ReLU, Linear (types and order are checked: that
+    order is the one the kernel evaluates); shapes must be W1 [H, obs_dim_i], b1 [H], W2 [H, H], b2 [H], W3 [5, H],
+    b3 [5] with one H for all agents.  No device is needed."""
+    import torch
+    if len(policies) != len(obs_dims):
+        raise ValueError("expected %d policies, got %d" % (len(obs_dims), len(policies)))
+    params, hidden = [], None
+    for i, pol in enumerate(policies):
+        if isinstance(pol, torch.nn.Module):
+            layers = [m for m in pol.modules() if not list(m.children())]
+            names = " -> ".join(type(m).__name__ for m in layers)
+            ok = (isinstance(pol, torch.nn.Sequential) and len(layers) == 5
+                  and all(isinstance(layers[k], torch.nn.Linear) for k in (0, 2, 4))
+                  and all(type(layers[k]) is torch.nn.ReLU for k in (1, 3)))
+            if not ok:
+                raise ValueError("policy %d must be %s; got %s (%s)" % (i, _MLP_SHAPE, type(pol).__name__, names))
+            if any(layers[k].bias is None for k in (0, 2, 4)):
+                raise ValueError("policy %d: every Linear layer needs a bias" % i)
+            pol = (layers[0].weight, layers[0].bias, layers[2].weight, layers[2].bias, layers[4].weight, layers[4].bias)
+        elif not (isinstance(pol, (tuple, list)) and len(pol) == 6):
+            raise ValueError("policy %d must be %s" % (i, _MLP_SHAPE))
+        ts = [t if torch.is_tensor(t) else torch.as_tensor(np.asarray(t, dtype=np.float32)) for t in pol]
+        if ts[0].dim() != 2:
+            raise ValueError("policy %d: W1 must be a matrix [H, %d], got shape %s" % (i, obs_dims[i], tuple(ts[0].shape)))
+        H = int(ts[0].shape[0])
+        if hidden is None:
+            hidden = H
+        want = ((hidden, obs_dims[i]), (hidden,), (hidden, hidden), (hidden,), (5, hidden), (5,))
+        got = tuple(tuple(t.shape) for t in ts)
+        if got != want:
+            raise ValueError("policy %d: expected W1 [%d, %d], b1 [%d], W2 [%d, %d], b2 [%d], W3 [5, %d], b3 [5]; got %s"
+                             % (i, hidden, obs_dims[i], hidden, hidden, hidden, hidden, hidden,
+                                ", ".join(str(list(s)) for s in got)))
+        params.append(tuple(ts))
+    return params, hidden

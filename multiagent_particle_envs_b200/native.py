@@ -273,6 +273,21 @@ class NativeWorld(ShapeHandle):
                                           out.done_ptr, flags, self._stream()), "mpe_rollout_policy")
         return out
 
+    def rollout_policy_mlp(self, w_ptrs, hidden, n_steps, out=None, flags=0, rew_steps=None, act_rec_ptrs=None,
+                           obs_rec_ptrs=None, explore_seed=None, explore_epoch=0):
+        """n_steps fused steps in ONE launch with every agent's two-hidden-layer actor evaluated on the tensor cores
+        (mpe_rollout_policy_mlp); w_ptrs: the six pointer arrays (W1, b1, W2, b2, W3, b3), one device pointer per
+        agent each.  explore_seed (not None) switches the Gumbel-softmax sampling on."""
+        out = out or self.out
+        pv, lm, comm, goal = self._state_ptrs()
+        explore = explore_seed is not None
+        check(self.lib.mpe_rollout_policy_mlp(self.handle, pv, lm, comm, goal, *w_ptrs, int(hidden), int(n_steps),
+                                              int(explore), int(explore_seed) if explore else 0, int(explore_epoch),
+                                              self.world_offset, out.obs_ptrs, out.rew_ptr,
+                                              rew_steps.data_ptr() if rew_steps is not None else None, act_rec_ptrs,
+                                              obs_rec_ptrs, out.done_ptr, flags, self._stream()), "mpe_rollout_policy_mlp")
+        return out
+
     # ---- host callers (what the reference's callers hold: NumPy arrays) -----------------------
     def host_staging(self):
         if self._host is None:

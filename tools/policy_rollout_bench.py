@@ -1,15 +1,36 @@
 #!/usr/bin/env python
-"""Closed-loop rollouts: T steps of obs -> per-agent actor (Linear-ReLU-Linear-softmax) -> env.step, as
-  (a) ONE launch of mpe_rollout_policy (actors evaluated inside the kernel, state and observations in registers),
+"""Closed-loop rollouts: T steps of obs -> per-agent actor -> env.step, as
+  (a) ONE launch of the in-kernel rollout (actors evaluated inside the kernel, state and observations in registers):
+      --layers 2: Linear-ReLU-Linear-softmax in fp32 (mpe_rollout_policy);
+      --layers 3: MADDPG's Linear-ReLU-Linear-ReLU-Linear on the tensor cores in TF32 (mpe_rollout_policy_mlp),
+      --explore: with the Gumbel-softmax sample instead of softmax (--layers 3 only);
   (b) the same actors as torch modules + env.step, all captured in one CUDA graph (rollout.GraphedRollout).
-Device time per 65 536-world step of each."""
+Device time per step of each.  With --layers 3 also the actor's FLOPs per step, computed from the padded shapes the
+kernel multiplies (2 (K1 H + H H + 8 H) per agent and world, K1 = obs_dim rounded up to 8), the in-kernel rollout's
+achieved TFLOP/s (actor FLOPs over the whole step's time: physics, observations and rewards are in that time too),
+torch's float32 matmul precision for the graphed loop, and the card's name and power limit read in the same run."""
 import argparse
 import json
 import os
+import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+
+
+def actor_flops_per_step(obs_dims, H, n):
+    return sum(2 * (((od + 7) // 8 * 8) * H + H * H + 8 * H) for od in obs_dims) * n
+
+
+def card_info():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        name, power, clock = [x.strip() for x in out[0].split(",")]
+        return {"name": name, "power_limit": power, "max_sm_clock": clock}
+    except Exception as e:  # noqa: BLE001  (the number still stands; say what is missing)
+        return {"error": "nvidia-smi: %s" % e}
 
 
 def main():
@@ -19,7 +40,11 @@ def main():
     ap.add_argument("--steps", type=int, default=25)
     ap.add_argument("--hidden", type=int, default=64)
     ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--layers", type=int, choices=(2, 3), default=2, help="Linear layers of the actor")
+    ap.add_argument("--explore", action="store_true", help="Gumbel-softmax exploration (--layers 3)")
     args = ap.parse_args()
+    if args.explore and args.layers != 3:
+        ap.error("--explore needs --layers 3")
     import torch
     import __graft_entry__ as g
     g.build(quiet=True)
@@ -32,25 +57,38 @@ def main():
     env.reset()
     nw = env.world.native
     torch.manual_seed(0)
-    mods = [torch.nn.Sequential(torch.nn.Linear(od, H), torch.nn.ReLU(), torch.nn.Linear(H, 5)).to(dev) for od in nw.obs_dims]
+    if args.layers == 2:
+        mods = [torch.nn.Sequential(torch.nn.Linear(od, H), torch.nn.ReLU(), torch.nn.Linear(H, 5)).to(dev) for od in nw.obs_dims]
+    else:
+        mods = [torch.nn.Sequential(torch.nn.Linear(od, H), torch.nn.ReLU(), torch.nn.Linear(H, H), torch.nn.ReLU(),
+                                    torch.nn.Linear(H, 5)).to(dev) for od in nw.obs_dims]
     res = {"config": {"scenario": args.scenario, "n_env": n, "T": T, "hidden": H}}
+    if args.layers == 3:
+        res["config"].update(layers=3, explore=args.explore, torch_float32_matmul_precision=torch.get_float32_matmul_precision())
+    kw = {"explore_seed": 1} if args.explore else {}
     # (a) in-kernel actors
     for _ in range(2):
-        env.rollout_policy(mods, T)
+        env.rollout_policy(mods, T, **kw)
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.reps):
-        env.rollout_policy(mods, T)
+        env.rollout_policy(mods, T, **kw)
     e1.record()
     torch.cuda.synchronize()
     sec = e0.elapsed_time(e1) / 1e3 / (args.reps * T)
     res["in_kernel"] = {"us_per_step": 1e6 * sec, "env_steps_per_sec": n / sec}
+    if args.layers == 3:
+        flops = actor_flops_per_step(nw.obs_dims, H, n)
+        res["in_kernel"].update(actor_flop_per_step=flops, actor_tflops=flops / sec / 1e12)
     # (b) torch actors + env.step in one CUDA graph
     env2 = make_env(args.scenario, num_envs=n, device=dev)
     env2.reset()
 
     def policy(obs_n):
+        if args.explore:   # the same Gumbel-softmax sample, noise from torch's generator
+            return [torch.softmax(m(o) - torch.log(-torch.log(torch.rand(o.shape[0], 5, device=dev))), -1)
+                    for m, o in zip(mods, obs_n)]
         return [torch.softmax(m(o), -1) for m, o in zip(mods, obs_n)]
 
     ro = GraphedRollout(env2, policy, steps=T)
@@ -67,6 +105,8 @@ def main():
     sec2 = e0.elapsed_time(e1) / 1e3 / (args.reps * T)
     res["graphed_torch"] = {"us_per_step": 1e6 * sec2, "env_steps_per_sec": n / sec2}
     res["speedup"] = sec2 / sec
+    if args.layers == 3:
+        res["card"] = card_info()
     print(json.dumps(res))
 
 
