@@ -101,12 +101,113 @@ def random_actions(act_dims, n, rng, temperature=2.0, movable=None):
     return np.concatenate(parts, axis=1)
 
 
+# ---- launch shapes: which block size the library picks for a batch ----------------------------------
+# Mirrors of the launch-shape rules in multiagent_particle_envs_b200/csrc/mpe_kernels.cu (sms = the device's SM count):
+#   "step"   launch() -> launch_grid (~l.1954): the fused step runs whole 32-world tiles on the HOT kernel -- 1 warp per
+#            block up to 16*sms tiles, 2 up to 64*sms, else 4 -- and the ragged tail (< 32 worlds) on the general kernel
+#            at begin = whole tiles, in one 1-warp block (~l.1982-1993).  Above 16*sms tiles the programs with a
+#            hot_dense_fn take that 80-register build instead of hot_fn (~l.1987); make_program (~l.1563) builds it
+#            where kLowRegVariant holds: tag with 3 to 6 agents and spread N=4 (csrc/mpe_scenarios.cuh ~l.96, ~l.173).
+#   "rollout" mpe_rollout (~l.2116): 1 warp per block up to 4*sms warps, 2 up to 64*sms, else 4
+#   "policy"  mpe_rollout_policy (~l.2166): 1 up to 16*sms warps, 2 up to 64*sms, else 4
+#   "mlp"     mpe_rollout_policy_mlp (~l.2227-2229): ceil(warps / sms) warps per block, capped at mlp_block_warps
+#            (~l.1026: 12 for H = 64 with four or more agents, else 16)
+# The shared-memory caps (max_warps_per_block, ~l.1647) never bind for the built-in scenarios at 4 warps per block.
+STEP_DENSE_TAGS = ("simple_tag", "simple_tag_2v1", "simple_tag_4v2")    # the test tags with a hot_dense_fn
+
+
+def device_sms():
+    import torch
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def mlp_block_cap(H, n_agents):
+    return 12 if (H == 64 and n_agents >= 4) else 16
+
+
+def launch_shape(kernel, n, sms, cap=16):
+    """(warps per block, #blocks, last block partial, worlds in the last warp) the library picks for n worlds.  For
+    "step" this describes the HOT launch over the whole tiles; the tail is n % 32 worlds on the general kernel."""
+    warps = n // 32 if kernel == "step" else (n + 31) // 32
+    if kernel == "step":
+        wpb = 1 if warps <= 16 * sms else (2 if warps <= 64 * sms else 4)
+    elif kernel == "rollout":
+        wpb = 1 if warps <= 4 * sms else (2 if warps <= 64 * sms else 4)
+    elif kernel == "policy":
+        wpb = 1 if warps <= 16 * sms else (2 if warps <= 64 * sms else 4)
+    elif kernel == "mlp":
+        wpb = max(1, min(cap, -(-warps // sms)))
+    else:
+        raise ValueError(kernel)
+    blocks = -(-warps // wpb)
+    last_rows = n % 32 if kernel == "step" else (n - 32 * (warps - 1))
+    return wpb, blocks, warps % wpb != 0, last_rows if last_rows else 32
+
+
+def step_uses_dense(tag, n, sms):
+    return tag in STEP_DENSE_TAGS and n // 32 > 16 * sms
+
+
+def regime_size(kernel, sms, wpb, cap=16, base=None):
+    """A batch size for which `kernel` launches blocks of `wpb` warps with a partial last block (when wpb > 1) and a
+    ragged last warp (17 worlds).  `base` (worlds) asks for a size just above it in that regime, e.g. 65 536 worlds
+    plus a ragged tail."""
+    if kernel == "mlp":
+        lo = (wpb - 1) * sms + 1                 # ceil(warps / sms) == wpb from here on (up to wpb * sms, or the cap)
+    else:
+        lo = {1: 1, 2: {"rollout": 4, "policy": 16, "step": 16}[kernel] * sms + 1, 4: 64 * sms + 1}[wpb]
+    warps = max(lo, base // 32 + 1 if base else lo)   # "step": whole tiles; otherwise warps including the ragged one
+    while wpb > 1 and warps % wpb == 0:
+        warps += 1
+    n = warps * 32 + 17 if kernel == "step" else (warps - 1) * 32 + 17
+    shape = launch_shape(kernel, n, sms, cap)
+    assert shape[0] == wpb and shape[2] == (wpb > 1) and shape[3] == 17, (kernel, sms, wpb, n, shape)
+    return n
+
+
 def split_cols(a, dims):
     out, c = [], 0
     for d in dims:
         out.append(a[..., c:c + d])
         c += d
     return out
+
+
+# ---- conditioning of the post-step velocity ---------------------------------------------------------
+# integrate_state (core.py:158-169) makes each velocity component the sum v (1 - damping) + (u + sum of contact forces)
+# dt / m.  In a squeezed world those forces are large and cancel, so the result can be small next to its terms; any
+# fp32 evaluation then errs by a few ulps of the TERMS, which the per-element rtol of the small result does not cover.
+VELOCITY_TERM_ULPS = 8
+
+
+def velocity_term_scale(desc, pv0, lm, act, act_dims):
+    """[n, A, 2]: per velocity component, the sum of |terms| of that sum (fp64, from the pre-step state and actions)"""
+    A, L = desc.n_agents, desc.n_landmarks
+    pos = np.concatenate([np.asarray(pv0, np.float64)[:, :, 0:2], np.asarray(lm, np.float64).reshape(len(pv0), L, 2)], 1)
+    size = [desc.agent_size[i] for i in range(A)] + [desc.landmark_size[l] for l in range(L)]
+    collide = [bool(desc.agent_collide[i]) for i in range(A)] + [bool(desc.landmark_collide[l]) for l in range(L)]
+    F = np.zeros((len(pv0), A, 2))
+    off = 0
+    for i in range(A):
+        if desc.agent_movable[i]:                                   # |u| (environment.py:174-181)
+            a = np.asarray(act[:, off:off + 5], np.float64)
+            F[:, i, 0] += np.abs(a[:, 1] - a[:, 2]) * desc.agent_sens[i]
+            F[:, i, 1] += np.abs(a[:, 3] - a[:, 4]) * desc.agent_sens[i]
+        off += act_dims[i]
+    k = desc.contact_margin
+    for a in range(A + L):                                          # |collision forces| (core.py:181-193)
+        for b in range(a + 1, A + L):
+            if not (collide[a] and collide[b]) or (a >= A and b >= A):
+                continue
+            delta = pos[:, a] - pos[:, b]
+            dist = np.sqrt((delta ** 2).sum(-1, keepdims=True))
+            pen = np.logaddexp(0, -(dist - size[a] - size[b]) / k) * k
+            f = np.abs(desc.contact_force * delta / np.maximum(dist, 1e-30) * pen)
+            for e in (a, b):
+                if e < A:
+                    F[:, e] += f
+    mass = np.array([desc.agent_mass[i] for i in range(A)])[None, :, None]
+    return np.abs(np.asarray(pv0, np.float64)[:, :, 2:4]) * (1 - desc.damping) + F / mass * desc.dt
 
 
 # ---- accounting for contact-indicator mismatches between fp32 and fp64 ---------------------------------

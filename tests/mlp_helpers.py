@@ -1,6 +1,8 @@
 """NumPy models of the two-hidden-layer in-kernel actor (env.rollout_policy with a Linear-ReLU-Linear-ReLU-Linear
 policy): TF32 rounding as cvt.rna.tf32.f32 does it, Philox4x32-10, the Gumbel noise stream, and a float64 evaluation
-of the actor with or without the kernel's operand rounding."""
+of the actor with or without the kernel's operand rounding, and the accounting for its TF32 rounding flips."""
+import itertools
+
 import numpy as np
 
 EXPLORE_TAG = 0x40000000
@@ -14,6 +16,20 @@ def tf32_rna(x):
     r = ((b.astype(np.uint64) + 0x1000) & 0xFFFFE000).astype(np.uint32)
     special = (b & 0x7F800000) == 0x7F800000
     return np.where(special, b, r).view(np.float32)
+
+
+def tf32_rne(x):
+    """fp32 -> TF32 rounded to nearest, ties to EVEN (what cvt.rna is not), as float32; finite inputs"""
+    b = np.asarray(x, dtype=np.float32).view(np.uint32).astype(np.uint64)
+    return (((b + 0xFFF + ((b >> 13) & 1)) & 0xFFFFE000).astype(np.uint32)).view(np.float32)
+
+
+def tf32_tie(x, every=1):
+    """x (float32) with every `every`-th entry (flat index) moved onto a TF32 rounding tie: the 13 bits below TF32 set
+    to exactly half a unit, where ties-away and ties-to-even rounding part"""
+    b = np.array(x, dtype=np.float32).view(np.uint32)
+    pick = (np.arange(b.size) % every == 0).reshape(b.shape)
+    return np.where(pick, (b & np.uint32(0xFFFFE000)) | np.uint32(0x1000), b).view(np.float32)
 
 
 def philox4x32_10(ctr, key):
@@ -68,3 +84,117 @@ def actor_logits(obs, W1, b1, W2, b2, W3, b3, tf32=True):
 def softmax(z):
     e = np.exp(z - z.max(-1, keepdims=True))
     return e / e.sum(-1, keepdims=True)
+
+
+# ---- accounting for TF32 rounding flips between the kernel and the float64 actor -------------------------------------
+# actor_logits(tf32=True) rounds every tensor-core operand exactly as the kernel does, so the two can only differ through
+# fp32 accumulation: in the logits by ~1e-7, and in a hidden layer where a unit's fp32 sum and the float64 sum fall on
+# different sides of a TF32 rounding boundary -- h1 / h2 then round to neighbouring TF32 values, 2^-10 relative apart,
+# and the row moves by up to a few 1e-4.  Every row beyond atol must be explained that way.
+#
+# Accumulation-error bound of one unit, sum_k a_k b_k + bias over K products (tf32_accumulation_bound): the operands
+# have 11 significant bits, so every product is exact in fp32 and only the additions err.  The tensor cores add a whole
+# k-tile of 8 products to the accumulator at once (aligned to the largest term, not sequential round-to-nearest), so
+# the textbook K u S bound of a sequential fp32 sum (u = 2^-24, S = sum_k |a_k b_k| + |bias|, no partial sum exceeds S)
+# does not apply as such.  tools/tf32_mma_error.cu measures the error of the kernel's exact mma.sync chain against the
+# exact sum on actor-like operands: at most 2.0, 2.9, 3.3 and 4.1 u S for K = 8, 16, 32 and 64 (H100 SXM, 400 W, 2^19
+# sums per K).  We allow 2 u S per k-tile plus 4 u S: (K/4 + 4) u S, i.e. 6, 8, 12 and 20 u S for those K -- 3 to 5
+# times the measured worst case.
+#
+# Per row, a unit is ambiguous when relu(pre-activation) lies within the bound of a TF32 rounding boundary (units
+# within the bound of zero are not: relu clips them to [0, bound], far below atol downstream).  Combinations of
+# ambiguous units are enumerated layer by layer, in order of their number of flips: every choice of h1 flips, then h2
+# recomputed -- and its ambiguity with it, so that an h1 flip too small to matter by itself can still carry an h2 unit
+# across a boundary -- and every choice of h2 flips.
+#
+# How strict this is: at H = 64 most rows hold an ambiguous unit (a few per row, mostly small ones), so "has an
+# ambiguous unit" alone rules out little there.  What does is the re-evaluation: a flip moves a row along one of a few
+# fixed directions, so a change of the row in any other direction -- a wrong logit, a wrong lane, a row that no longer
+# sums to one -- is not explained unless it happens to lie within atol of one of those directions.  A wrong logit that
+# moves the row by 3e-5 can still pass in a sizeable fraction of rows at H = 64; by 3e-4 almost never.  A systematic
+# defect moves many rows and is caught.
+TF32_MAX_COMBOS = 2 ** 6
+
+
+def tf32_accumulation_bound(a, b, bias):
+    """per-unit bound on |fp32 tensor-core sum - exact sum| for rows a [m, K] (TF32 values) times weights b [N, K]"""
+    K = a.shape[-1]
+    return (K / 4.0 + 4.0) * 2.0 ** -24 * (np.abs(a) @ np.abs(b).T + np.abs(bias))
+
+
+def tf32_flip_choices(pre, bound):
+    """(relu(pre) rounded to TF32 as the model does, the other TF32 value a sum within `bound` of pre may round to --
+    NaN where the unit is not ambiguous)"""
+    f32 = np.float32
+    r = tf32_rna(np.maximum(pre, 0.0).astype(f32)).astype(np.float64)
+    lo = tf32_rna(np.maximum(pre - bound, 0.0).astype(f32)).astype(np.float64)
+    hi = tf32_rna((pre + bound).astype(f32)).astype(np.float64)
+    alt = np.where(lo != r, lo, np.where(hi != r, hi, np.nan))
+    alt[pre <= bound] = np.nan
+    return r, alt
+
+
+def explain_tf32_mismatches(actions, obs, params, noise=0.0, atol=1e-5):
+    """Assert that every row of the kernel's `actions` [n, 5] that differs from softmax(actor_logits(obs, *params,
+    tf32=True) + noise) by more than atol is a TF32 rounding flip (see above): it has an ambiguous h1 or h2 unit, and
+    rounding some combination of them the other way brings it within atol.  At most TF32_MAX_COMBOS combinations per
+    row; a row that needs more fails.  Returns the number of explained rows."""
+    f64 = np.float64
+    W1, b1, W2, b2, W3, b3 = [np.asarray(p, dtype=np.float32) for p in params]
+    H = W1.shape[0]
+    t1, t2, t3 = (tf32_rna(W).astype(f64) for W in (W1, W2, W3))
+    b1, b2, b3 = (np.asarray(b, f64) for b in (b1, b2, b3))
+    got = np.asarray(actions, f64)
+    noise = np.broadcast_to(np.asarray(noise, f64), got.shape)
+    x0 = tf32_rna(obs).astype(f64)
+    p1 = x0 @ t1.T + b1
+    h1 = tf32_rna(np.maximum(p1, 0.0).astype(np.float32)).astype(f64)
+    h2 = tf32_rna(np.maximum(h1 @ t2.T + b2, 0.0).astype(np.float32)).astype(f64)
+    want = softmax(h2 @ t3.T + b3 + noise)
+    bad = np.where((np.abs(got - want) > atol).any(-1))[0]
+    if bad.size == 0:
+        return 0
+    _, alt1 = tf32_flip_choices(p1[bad], tf32_accumulation_bound(x0[bad], t1, b1))
+    unexplained = []
+    for r, w in enumerate(bad):
+        amb1 = list(np.where(~np.isnan(alt1[r]))[0])
+        h2_of = {}                                   # h1 flip set -> (h2 as the model rounds it, alternatives, ambiguous)
+
+        def layer2(f1):
+            if f1 not in h2_of:
+                h = h1[w].copy()
+                h[list(f1)] = alt1[r, list(f1)]
+                q = h @ t2.T + b2
+                r2, alt2 = tf32_flip_choices(q, tf32_accumulation_bound(h[None], t2, b2)[0])
+                h2_of[f1] = (r2, alt2, list(np.where(~np.isnan(alt2))[0]))
+            return h2_of[f1]
+
+        any_ambiguous = bool(amb1) or bool(layer2(())[2])
+        ok, combos = False, 0
+        for nflips in range(1, len(amb1) + H + 1) if any_ambiguous else ():
+            tried = combos
+            for k1 in range(min(nflips, len(amb1)) + 1):
+                for f1 in itertools.combinations(amb1, k1):
+                    r2, alt2, amb2 = layer2(f1)
+                    for f2 in itertools.combinations(amb2, nflips - k1):
+                        combos += 1
+                        if combos > TF32_MAX_COMBOS:
+                            break
+                        g = r2.copy()
+                        g[list(f2)] = alt2[list(f2)]
+                        ok = bool((np.abs(softmax(g @ t3.T + b3 + noise[w]) - got[w]) <= atol).all())
+                        if ok:
+                            break
+                    if ok or combos > TF32_MAX_COMBOS:
+                        break
+                if ok or combos > TF32_MAX_COMBOS:
+                    break
+            if ok or combos > TF32_MAX_COMBOS or combos == tried:
+                break
+        if not ok:
+            unexplained.append((int(w), any_ambiguous, min(combos, TF32_MAX_COMBOS + 1),
+                                float(np.abs(got[w] - want[w]).max())))
+    assert not unexplained, ("%d of %d rows beyond %g are not TF32 rounding flips (row, has an ambiguous unit, "
+                             "combinations tried, max |difference|): %s" % (len(unexplained), bad.size, atol,
+                                                                            unexplained[:8]))
+    return int(bad.size)

@@ -4,7 +4,8 @@ import numpy as np
 import pytest
 
 from helpers import make_product_env
-from mlp_helpers import philox4x32_10, tf32_rna, uniform_from_bits
+import mlp_helpers
+from mlp_helpers import philox4x32_10, softmax, tf32_rna, tf32_rne, tf32_tie, uniform_from_bits
 
 torch = pytest.importorskip("torch")
 
@@ -104,3 +105,123 @@ def test_malformed_two_hidden_layer_policies_are_refused():
     # one-hidden-layer policies keep their own path
     one = nn.Sequential(nn.Linear(18, 64), nn.ReLU(), nn.Linear(64, 5))
     assert not _has_two_hidden_layers(one) and not _has_two_hidden_layers(tuples[0][:4])
+
+
+# ---- explain_tf32_mismatches on synthetic actors (no GPU) ----------------------------------------------------------
+def _actions(obs, params, rnd=tf32_rna, h1_override=None):
+    """the actor with every operand rounded by `rnd` and exact accumulation; h1_override (row, unit, value) replaces
+    one rounded h1 entry"""
+    f64 = np.float64
+    W1, b1, W2, b2, W3, b3 = params
+    h1 = rnd(np.maximum(rnd(obs).astype(f64) @ rnd(W1).astype(f64).T + b1, 0).astype(np.float32)).astype(f64)
+    if h1_override is not None:
+        h1[h1_override[0], h1_override[1]] = h1_override[2]
+    h2 = rnd(np.maximum(h1 @ rnd(W2).astype(f64).T + b2, 0).astype(np.float32)).astype(f64)
+    return softmax(h2 @ rnd(W3).astype(f64).T + b3)
+
+
+def _dyadic_actor(rng, od=6, H=32, scale=2.0):
+    """weights and observations on a 2^-4 grid: every sum is exact and every h1 / h2 value a short dyadic number, so no
+    unit lies near a TF32 rounding boundary"""
+    q = lambda *s: (np.round(rng.randn(*s) * scale * 16) / 16).astype(np.float32)        # noqa: E731
+    params = (q(H, od) / 4, q(H) / 4, q(H, H) / 16, q(H) / 4, q(5, H) / 4, q(5) / 4)
+    obs = q(32, od)
+    return obs, params
+
+
+def test_accounting_accepts_a_unit_on_a_tf32_midpoint_rounded_the_other_way():
+    rng = np.random.RandomState(1)
+    obs, (W1, b1, W2, b2, W3, b3) = _dyadic_actor(rng)
+    # unit 0 of row 5: pre-activation 1 + 2^-11 exactly (a TF32 tie); the model rounds it up to 1 + 2^-10, the "kernel"
+    # lands a hair below the tie and rounds it down to 1
+    W1 = W1.copy()
+    W1[0] = 0.0
+    b1 = b1.copy()
+    b1[0] = np.float32(1 + 2 ** -11)
+    W2 = W2.copy()
+    W2[:, 0] = 1.0                          # make the flip visible in the actions
+    params = (W1, b1, W2, b2, W3, b3)
+    want = _actions(obs, params)
+    got = _actions(obs, params, h1_override=(5, 0, 1.0))
+    assert np.abs(got - want)[5].max() > 1e-4 and np.abs(got - want)[np.arange(32) != 5].max() == 0
+    assert mlp_helpers.explain_tf32_mismatches(got, obs, params) == 1
+    assert mlp_helpers.explain_tf32_mismatches(want, obs, params) == 0
+
+
+def test_accounting_rejects_a_perturbation_without_an_ambiguous_unit():
+    obs, params = _dyadic_actor(np.random.RandomState(2))
+    got = _actions(obs, params)
+    assert mlp_helpers.explain_tf32_mismatches(got, obs, params) == 0
+    bad = got.copy()
+    bad[7, 2] += 3e-4
+    with pytest.raises(AssertionError, match="not TF32 rounding flips"):
+        mlp_helpers.explain_tf32_mismatches(bad, obs, params)
+    # a wrong logit, renormalised by the softmax as a lane bug would be
+    z = mlp_helpers.actor_logits(obs, *params)
+    z[7, z[7].argmax()] += 2e-3
+    bad = got.copy()
+    bad[7] = softmax(z[7])
+    assert np.abs(bad - got).max() > 1e-4
+    with pytest.raises(AssertionError, match="not TF32 rounding flips"):
+        mlp_helpers.explain_tf32_mismatches(bad, obs, params)
+
+
+def test_accounting_rejects_a_perturbation_in_the_last_row_of_a_tile():
+    """generic weights (ambiguous units everywhere): a change no rounding flip can make -- one entry of the last row of
+    a 32-row tile, so the row no longer sums to one -- is still caught"""
+    rng = np.random.RandomState(3)
+    od, H = 18, 64
+    r = lambda *s: rng.randn(*s).astype(np.float32)                                     # noqa: E731
+    params = (r(H, od) * 1.5 / od ** 0.5, r(H) * 0.3, r(H, H) * 1.5 / H ** 0.5, r(H) * 0.3, r(5, H) * 1.5 / H ** 0.5,
+              r(5) * 0.2)
+    obs = rng.uniform(-1.5, 1.5, (64, od)).astype(np.float32)
+    got = _actions(obs, params)
+    mlp_helpers.explain_tf32_mismatches(got, obs, params)
+    bad = got.copy()
+    bad[31, 4] += 1e-4
+    with pytest.raises(AssertionError, match=r"\(31, "):
+        mlp_helpers.explain_tf32_mismatches(bad, obs, params)
+    z = mlp_helpers.actor_logits(obs, *params)                  # a wrong logit of that row, renormalised
+    z[31, 4] += 4e-3
+    bad = got.copy()
+    bad[31] = softmax(z[31])
+    assert np.abs(bad - got).max() > 3e-4
+    with pytest.raises(AssertionError, match=r"\(31, "):
+        mlp_helpers.explain_tf32_mismatches(bad, obs, params)
+
+
+def test_accounting_rejects_round_to_nearest_even():
+    """weights and observations that are exact TF32 ties: an actor that rounds them to nearest-even is not the kernel"""
+    rng = np.random.RandomState(4)
+    obs, (W1, b1, W2, b2, W3, b3) = _dyadic_actor(rng)
+    params = (tf32_tie(W1 + 0.3), b1, tf32_tie(W2 + 0.1), b2, tf32_tie(W3), b3)
+    obs = tf32_tie(obs + 0.7)
+    assert (tf32_rna(params[0]) != tf32_rne(params[0])).mean() > 0.3
+    want = _actions(obs, params)
+    assert mlp_helpers.explain_tf32_mismatches(want, obs, params) == 0
+    rne = _actions(obs, params, rnd=tf32_rne)
+    assert np.abs(rne - want).max() > 1e-4
+    with pytest.raises(AssertionError, match="not TF32 rounding flips"):
+        mlp_helpers.explain_tf32_mismatches(rne, obs, params)
+
+
+def test_regime_sizes_match_the_launch_rules():
+    """the batch sizes the GPU tests use for each launch-shape regime, for an H100 SXM (132 SMs) and PCIe (114 SMs)"""
+    from helpers import launch_shape, regime_size, step_uses_dense
+    for sms in (132, 114):
+        for kernel, wpbs in (("step", (1, 2, 4)), ("rollout", (1, 2, 4)), ("policy", (1, 2, 4)), ("mlp", (1, 5, 12, 16))):
+            for wpb in wpbs:
+                n = regime_size(kernel, sms, wpb, base=2048 if wpb == 1 else None)
+                got = launch_shape(kernel, n, sms)
+                assert got[0] == wpb and got[2] == (wpb > 1) and got[3] == 17, (sms, kernel, wpb, n, got)
+        n = regime_size("mlp", sms, 12, cap=12, base=65536)
+        assert n > 65536 and launch_shape("mlp", n, sms, cap=12)[0] == 12 and launch_shape("mlp", n, sms)[0] == 16
+        assert step_uses_dense("simple_tag", regime_size("step", sms, 2), sms)
+        assert not step_uses_dense("simple_spread_n6", regime_size("step", sms, 2), sms)
+    # the thresholds themselves, at 132 SMs
+    assert launch_shape("step", 16 * 132 * 32 + 31, 132)[0] == 1 and launch_shape("step", (16 * 132 + 1) * 32, 132)[0] == 2
+    assert launch_shape("rollout", 4 * 132 * 32, 132)[0] == 1 and launch_shape("rollout", 4 * 132 * 32 + 1, 132)[0] == 2
+    assert launch_shape("policy", 64 * 132 * 32, 132)[0] == 2 and launch_shape("policy", 64 * 132 * 32 + 1, 132)[0] == 4
+    assert launch_shape("mlp", 65536, 132) == (16, 128, False, 32)
+    assert launch_shape("mlp", 65536, 132, cap=12) == (12, 171, True, 32)
+    assert launch_shape("mlp", 65536, 114) == (16, 128, False, 32)

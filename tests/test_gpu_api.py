@@ -211,11 +211,16 @@ def test_graphed_rollout_with_resets_draws_fresh_episodes_on_replay():
 
 @pytest.mark.parametrize("tag,n,T", [("simple_spread_n3", 2049, 25), ("simple_tag", 4096, 10), ("simple_world_comm", 1031, 7),
                                      ("simple_reference", 512, 6), ("simple_speaker_listener", 100, 5),
-                                     ("simple_crypto", 333, 4), ("simple_adversary", 64, 9), ("simple", 33, 3)])
+                                     ("simple_crypto", 333, 4), ("simple_adversary", 64, 9), ("simple", 33, 3),
+                                     ("simple_spread_n3", "2warp", 4), ("simple_tag", "4warp", 3)])
 def test_open_loop_rollout_equals_repeated_steps(tag, n, T):
     """env.rollout (mpe_rollout: T steps in one launch, state in registers, next step's actions prefetched) is
     bit-identical to T calls of env.step on the same actions with the rewards summed in step order -- full tiles take
-    the cp.async path, the ragged last tile the scalar one"""
+    the cp.async path, the ragged last tile the scalar one.  "2warp" / "4warp": sizes with 2- / 4-warp blocks
+    (helpers.launch_shape "rollout"), partial last block and ragged last warp"""
+    if isinstance(n, str):
+        from helpers import device_sms, regime_size
+        n = regime_size("rollout", device_sms(), int(n[0]))
     env_a = make_product_env(tag, num_envs=n, seed=5)
     env_b = make_product_env(tag, num_envs=n, seed=5)
     env_a.reset()
@@ -249,14 +254,19 @@ def test_open_loop_rollout_equals_repeated_steps(tag, n, T):
 
 
 @pytest.mark.parametrize("tag,n,T,H", [("simple_spread_n3", 2049, 12, 32), ("simple_spread_n3", 1000, 8, 64),
-                                       ("simple_tag", 1031, 10, 32), ("simple_tag", 512, 5, 64), ("simple", 257, 6, 64)])
+                                       ("simple_tag", 1031, 10, 32), ("simple_tag", 512, 5, 64), ("simple", 257, 6, 64),
+                                       ("simple", 1031, 6, 32), ("simple_spread_n3", "2warp", 3, 64)])
 def test_closed_loop_policy_rollout(tag, n, T, H):
     """env.rollout_policy (mpe_rollout_policy: T steps in one launch, every agent's two-layer actor evaluated inside the
     kernel from observations that never leave the registers):
       (1) the actions it records, fed to T ordinary fused steps of a twin env, reproduce the final state, the final
           observations, every step's rewards and the reward sums BIT FOR BIT (physics / reward / observation parity);
       (2) every recorded action equals softmax(W2 relu(W1 obs + b1) + b2) evaluated in float64 on the twin's observations
-          to 1e-5 (the fp32 perceptron, FMA accumulation in a fixed order)."""
+          to 1e-5 (the fp32 perceptron, FMA accumulation in a fixed order).
+    "2warp": a size with 2-warp blocks (helpers.launch_shape "policy"), partial last block and ragged last warp."""
+    if isinstance(n, str):
+        from helpers import device_sms, regime_size
+        n = regime_size("policy", device_sms(), int(n[0]))
     env_a = make_product_env(tag, num_envs=n, seed=9)
     env_b = make_product_env(tag, num_envs=n, seed=9)
     env_a.reset()

@@ -6,8 +6,8 @@ on the kernels' own stored state.  Run on an H100: pytest -m gpu."""
 import numpy as np
 import pytest
 
-from helpers import (CONFIGS, VARIANTS, explain_flag_mismatches, load_golden, make_product_env, random_actions,
-                     random_goals, random_states, split_cols)
+from helpers import (CONFIGS, VARIANTS, VELOCITY_TERM_ULPS, explain_flag_mismatches, load_golden, make_product_env,
+                     random_actions, random_goals, random_states, scenario_of, split_cols, velocity_term_scale)
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -111,14 +111,35 @@ def test_golden_fixtures_free_running(tag):
     assert np.median(err) < 1e-5 and (err < 1e-3).mean() > 0.97
 
 
+def close_per_element(got, want, slack=0.0):
+    """rtol 1e-5 / atol 1e-6 per element, or within `slack` (per element) where the value is ill-conditioned"""
+    err = np.abs(got - want)
+    bad = err > np.maximum(ATOL + RTOL * np.abs(want), slack)
+    assert not bad.any(), ("%d elements beyond rtol %g / atol %g: first %s, |difference| %s" % (
+        int(bad.sum()), RTOL, ATOL, np.argwhere(bad)[:4].tolist(), err[bad][:4]))
+
+
 @pytest.mark.parametrize("tag,n", [("simple", 4096), ("simple_spread_n3", 8192), ("simple_spread_n6", 4096),
                                    ("simple_tag", 8192), ("simple_world_comm", 4096), ("simple_adversary", 4096),
                                    ("simple_push", 4096), ("simple_speaker_listener", 4096), ("simple_reference", 4096),
                                    ("simple_crypto", 4096), ("simple_tag_1v1", 2048), ("simple_tag_2v1", 2048),
-                                   ("simple_tag_4v2", 2048), ("simple_tag_6v2", 2048), ("simple_adversary_n4", 2048)])
+                                   ("simple_tag_4v2", 2048), ("simple_tag_6v2", 2048), ("simple_adversary_n4", 2048),
+                                   # production sizes (BASELINE.json) and launch shapes of the fused step, see
+                                   # helpers.launch_shape "step": (hot kernel, warps per block) -- resolved on the device
+                                   ("simple_spread_n3", 65536), ("simple_tag", 262144), ("simple_spread_n6", 131072),
+                                   ("simple_world_comm", 32768), ("simple_tag", "dense_4warp_ragged")])
 def test_seeded_worlds_vs_oracle(tag, n):
     from oracle import Oracle
     from multiagent_particle_envs_b200 import _lib
+    from helpers import device_sms, launch_shape, regime_size, step_uses_dense
+    sms = device_sms()
+    if n == "dense_4warp_ragged":     # 4-warp blocks of the 80-register kernel + the general kernel's tail at begin > 0
+        n = regime_size("step", sms, 4)
+        assert step_uses_dense(tag, n, sms) and launch_shape("step", n, sms)[:3:2] == (4, True) and n % 32
+    elif n == 262144:                 # the BASELINE tag size: 80-register kernel, 2-warp blocks on 132 SMs (4 on 114)
+        assert step_uses_dense(tag, n, sms) and launch_shape("step", n, sms)[0] == 2
+    elif n == 131072:                 # the BASELINE spread N=6 size: 2-warp blocks (on 64 SMs or more)
+        assert not step_uses_dense(tag, n, sms) and launch_shape("step", n, sms)[0] == 2
     env = make_product_env(tag, num_envs=n)
     env.reset()
     nw = env.world.native
@@ -136,9 +157,19 @@ def test_seeded_worlds_vs_oracle(tag, n):
     pv, comm = extract(nw)
     # (1) against the reference arithmetic (fp64) on identical fp32 inputs
     rpv, rcomm, robs, rrew, rdone, rinfo = o64.step(pv0, lm, comm0, act, flags, goal=goal)
-    np.testing.assert_allclose(pv, rpv, rtol=RTOL, atol=ATOL)
+    # a velocity that is the small difference of large contact forces (squeezed worlds) may differ by a few fp32 ulps of
+    # those forces (seen: spread N=6 at 131 072 worlds, 1.19e-6 on a velocity of -0.0123 whose terms sum to 9.96 in
+    # magnitude -- 2 ulps of them); the same slack applies to the observation entries that copy the velocity
+    slack = VELOCITY_TERM_ULPS * 2.0 ** -24 * velocity_term_scale(desc, pv0, lm, act, nw.act_dims)
+    pv_slack = np.zeros_like(rpv)
+    pv_slack[:, :, 2:4] = slack
+    obs_slack = np.zeros_like(robs)
+    if scenario_of(tag) in ("simple", "simple_spread", "simple_tag", "simple_world_comm"):   # obs = [own vel, ...]
+        for i, o in enumerate(np.cumsum([0] + list(nw.obs_dims))[:-1]):
+            obs_slack[:, o:o + 2] = slack[:, i]
+    close_per_element(pv, rpv, pv_slack)
     np.testing.assert_allclose(comm, rcomm, rtol=1e-7, atol=0)
-    np.testing.assert_allclose(obs, robs, rtol=RTOL, atol=ATOL)
+    close_per_element(obs, robs, obs_slack)
     assert np.array_equal(done, rdone)
     a_size = [desc.agent_size[i] for i in range(desc.n_agents)]
     l_size = [desc.landmark_size[l] for l in range(desc.n_landmarks)]
@@ -380,6 +411,11 @@ ALT_KERNELS = {
     "low_register_build": {"MPE_B200_DENSE": "1"},                # the 80-register HOT variant (tag family, spread N=4)
     "warp_pair_split": {"MPE_B200_SPLIT": "1"},
     "software_pipelined_persistent": {"MPE_B200_PIPE": "1"},
+    # the default kernels (HOT whole tiles, general-kernel tails) in 3- and 4-warp blocks instead of 1-warp blocks:
+    # per-warp shared-memory offsets and partial last blocks
+    "three_warp_blocks": {"MPE_B200_WPB": "3"},
+    "four_warp_blocks": {"MPE_B200_WPB": "4"},
+    "four_warp_blocks_low_register_build": {"MPE_B200_WPB": "4", "MPE_B200_DENSE": "1"},
 }
 
 
@@ -398,7 +434,7 @@ def test_alternative_step_kernels_are_bit_identical(tmp_path, variant):
     for mode in ("0", "1"):
         path = str(tmp_path / ("alt%s.npz" % mode))
         env = dict(os.environ)
-        for k in ("MPE_B200_SPLIT", "MPE_B200_PIPE", "MPE_B200_HOT", "MPE_B200_DENSE"):
+        for k in ("MPE_B200_SPLIT", "MPE_B200_PIPE", "MPE_B200_HOT", "MPE_B200_DENSE", "MPE_B200_WPB"):
             env.pop(k, None)
         if mode == "1":
             env.update(ALT_KERNELS[variant])
