@@ -206,21 +206,33 @@ MPE_API int mpe_rollout_policy(mpe_handle h, void *agent_pv_dev, const void *lm_
                                float *const *obs_n_dev, float *rew_sum_dev, float *rew_steps_dev,
                                float *const *act_record_n, uint8_t *done_dev, uint32_t flags, void *stream);
 
-/* The same closed-loop rollout with MADDPG's actor (mlp_model): obs_dim_i -> hidden -> ReLU -> hidden -> ReLU -> 5,
+/* The same closed-loop rollout with MADDPG's actor (mlp_model): obs_dim_i -> hidden -> ReLU -> hidden -> ReLU -> act_dim_i,
  *     logits_i = W3_i relu(W2_i relu(W1_i obs_i + b1_i) + b2_i) + b3_i,
  * evaluated on the tensor cores (TF32 mma.sync, fp32 accumulation; every operand -- observations, both hidden layers and
  * all weights -- rounded to TF32 with round-to-nearest, ties away from zero; biases added in fp32).  Weights in torch
  * nn.Linear layout: w1_n[i] float [hidden][obs_dim_i], b1_n[i] [hidden], w2_n[i] [hidden][hidden], b2_n[i] [hidden],
- * w3_n[i] [5][hidden], b3_n[i] [5]; hidden = 32 or 64 (both hidden layers).
- * explore == 0: agent i acts with softmax(logits_i) (MADDPG's mode()).  explore != 0: with the Gumbel-softmax sample
- * softmax(logits_i - log(-log u)) (SoftCategoricalPd.sample), u_0..u_4 drawn from Philox4x32-10 with key = explore_seed
- * and counter = (world_offset + w lo, hi, explore_epoch lo, 0x40000000 | ((t * A + i) * 2 + b)): u_0..u_3 are block
- * b = 0, u_4 is word 0 of block b = 1, u = ((bits >> 8) + 0.5) * 2^-24 with the sum rounded toward zero in fp32.  The
- * draw depends on the global world index, not on the batch it runs in.
- * Records (NULL: not written): act_record_n[i] float [n_steps][n_env][5], the action applied (the sample when
+ * w3_n[i] [act_dim_i][hidden], b3_n[i] [act_dim_i]; hidden = 32 or 64 (both hidden layers).
+ * The act_dim_i logits split into the action vector's sub-spaces (environment.py:40-66): 5 movement logits if agent i
+ * is movable, then dim_c utterance logits if it is not silent.  explore == 0: the action is the concatenation of one
+ * softmax per sub-space (MADDPG's mode()).  explore != 0: of one Gumbel-softmax sample softmax(z - log(-log u)) per
+ * sub-space (SoftCategoricalPd / SoftMultiCategoricalPd.sample).  Logit k uses u_k = word k mod 4 of the Philox4x32-10
+ * block b = k div 4 with key = explore_seed and counter = (world_offset + w lo, hi, explore_epoch lo,
+ * 0x40000000 | ((t * A + i) * S + b)), S = 2 when every act_dim of the scenario is <= 8 and 4 otherwise
+ * (simple_reference); u = ((bits >> 8) + 0.5) * 2^-24 with the sum rounded toward zero in fp32.  The draw depends on the
+ * global world index, not on the batch it runs in.  An exploring call with n_steps * A * S > 2^30 is refused with
+ * MPE_ERR_BAD_ARG before anything runs.
+ * The action is applied as _set_action does: movement (p1 - p2, p3 - p4) * sensitivity for movable agents only (an
+ * immovable agent's state is never written), the utterance becomes action.c; after the physics state.c = action.c and
+ * the rewards are computed from the new state, so an utterance of step t reaches the observations from step t + 1 on.
+ * comm_dev is read at the start and written at the end.
+ * Records (NULL: not written): act_record_n[i] float [n_steps][n_env][act_dim_i], the action applied (the sample when
  * exploring); obs_record_n[i] float [n_steps][n_env][obs_dim_i] (16-byte aligned), the observation agent i acted on at
- * step t; rew_steps_dev as in mpe_rollout_policy.  Feeding act_record_n to mpe_step reproduces state, observations and
- * rewards bit for bit.  Same programs as mpe_rollout_policy; otherwise, or for another hidden width, MPE_ERR_UNSUPPORTED. */
+ * step t; rew_steps_dev as in mpe_rollout_policy.  Feeding act_record_n to mpe_step reproduces state, comm state,
+ * observations and rewards bit for bit.  Built for simple, simple_spread N = 3, simple_tag 3 + 1,
+ * simple_speaker_listener, simple_reference, simple_crypto, simple_adversary (1 + 2 agents) and simple_push (1 + 1);
+ * otherwise, or for another hidden width, MPE_ERR_UNSUPPORTED.  The scenario and hidden width are checked before any
+ * state, weight or output pointer: a call with those null returns MPE_ERR_UNSUPPORTED or MPE_ERR_BAD_ARG and runs
+ * nothing. */
 MPE_API int mpe_rollout_policy_mlp(mpe_handle h, void *agent_pv_dev, const void *lm_p_dev, float *comm_dev,
                                    const int32_t *goal_dev, const float *const *w1_n, const float *const *b1_n,
                                    const float *const *w2_n, const float *const *b2_n, const float *const *w3_n,

@@ -993,37 +993,59 @@ template <class P> struct PolicyBuilt { static constexpr bool value = false; };
 template <> struct PolicyBuilt<Simple<1, 1>> { static constexpr bool value = true; };
 template <> struct PolicyBuilt<Spread<3>> { static constexpr bool value = true; };
 template <> struct PolicyBuilt<Tag<3, 1, 2>> { static constexpr bool value = true; };
+// the two-hidden-layer actor (mpe_policy_mlp_rollout_kernel) is built for those and for the reference's default
+// configurations of the scenarios with speaking or immovable agents
+template <class P> struct MlpBuilt : PolicyBuilt<P> {};
+template <> struct MlpBuilt<SpeakerListener> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Reference> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Crypto> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Adversary<1, 2, 2>> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Push<1, 1, 2>> { static constexpr bool value = true; };
 
 
 // ---- K-step closed-loop rollout with MADDPG's two-hidden-layer actor on the tensor cores ---------------------------
 // The persistent structure of mpe_policy_rollout_kernel (state in registers for all T steps, nothing read from HBM per
 // step, the same physics<P> / P::reward / P::observe<I>) with the MADDPG actor (mlp_model)
-//     logits_i = W3_i relu(W2_i relu(W1_i obs_i + b1_i) + b2_i) + b3_i       obs_dim_i -> H -> H -> 5,  H = 32 or 64
+//     logits_i = W3_i relu(W2_i relu(W1_i obs_i + b1_i) + b2_i) + b3_i       obs_dim_i -> H -> H -> act_dim_i,  H = 32 or 64
 // evaluated by the warp as three TF32 GEMMs with mma.sync.m16n8k8 (fp32 accumulation):
-//     [32 x K1] . [K1 x H] -> ReLU -> [32 x H] . [H x H] -> ReLU -> [32 x H] . [H x 8]
+//     [32 x K1] . [K1 x H] -> ReLU -> [32 x H] . [H x H] -> ReLU -> [32 x H] . [H x NOUT_i],  NOUT_i = act_dim_i rounded up to 8
 // One warp = 32 worlds = two m16 tiles.  Each lane writes its observation row into the warp's observation tile (the
 // layout of the fused step's coalesced tile store, ObsTile<obs_dim>); the A fragments are read from it with the columns
 // at and beyond obs_dim read as zero, so K1 = obs_dim rounded up to 8.  The accumulators of one layer are the A fragments
 // of the next without any data movement: within a k-tile a lane holds hidden units 2q and 2q+1 of rows g and g+8 and
 // the next layer's B fragments are staged with the same permutation of k.  Layers 2 and 3 are interleaved per 8-unit
-// tile of h2, so h2 never exists as a whole.  The 5 logits (padded to 8) go back to their lane through a small
-// shared-memory tile; that lane does the softmax (or the Gumbel-softmax sample), the _set_action decode and the step.
+// tile of h2, so h2 never exists as a whole.  The act_dim_i logits (padded to NOUT_i) go back to their lane through a
+// small shared-memory tile; that lane does the softmax (or the Gumbel-softmax sample), the _set_action decode and the
+// step.
+// Action sub-spaces (environment.py:40-66, MADDPG's SoftMultiCategoricalPd): the logits split, in action-vector order,
+// into 5 movement logits if the agent is movable, then dim_c utterance logits if it speaks; the action is the
+// concatenation of one softmax per sub-space.  Movement is decoded as _set_action does; an utterance becomes the
+// world's comm state after the physics (update_agent_state), as in the fused step, so the other agents observe it from
+// step t + 1 on.  Immovable agents keep their position and velocity.
 // Rounding: every tensor-core operand -- observations, h1, h2 and all weights -- is converted with cvt.rna.tf32.f32
 // (round to nearest, ties away from zero, to 10 mantissa bits); the weights once, while they are staged.  Biases are
 // the accumulators' fp32 initial values.
-// Exploration (explore != 0): agent i at step t acts with softmax(logits - log(-log u)) (SoftCategoricalPd.sample), in
-// fp32 with logf.  u_0..u_4 come from Philox4x32-10 with key = explore_seed and counter = (global world index lo, hi,
-// low 32 bits of explore_epoch, kExploreTag | ((t * A + i) * 2 + b)): u_0..u_3 are the four words of block b = 0, u_4
-// word 0 of block b = 1; u = ((bits >> 8) + 0.5) * 2^-24 with the sum rounded toward zero in fp32 (exact below 2^23,
-// the half is dropped above), so u lies in [2^-25, 1 - 2^-24].  The tag bit keeps this stream apart from reset_kernel's
-// counters, so an exploration seed equal to the env seed does not correlate the noise with initial positions; the
-// global world index (world_offset + w) makes the noise independent of sharding.
+// Exploration (explore != 0): agent i at step t acts with one softmax(z - log(-log u)) per sub-space
+// (SoftCategoricalPd.sample), in fp32 with logf.  Logit k of the action vector uses u_k = word k mod 4 of Philox4x32-10
+// block b = k div 4, with key = explore_seed and counter = (global world index lo, hi, low 32 bits of explore_epoch,
+// kExploreTag | ((t * A + i) * S + b)), S = mlp_explore_stride<P>() blocks per agent and step; u = ((bits >> 8) + 0.5)
+// * 2^-24 with the sum rounded toward zero in fp32 (exact below 2^23, the half is dropped above), so u lies in
+// [2^-25, 1 - 2^-24].  The tag bit keeps this stream apart from reset_kernel's counters, so an exploration seed equal
+// to the env seed does not correlate the noise with initial positions; the global world index (world_offset + w) makes
+// the noise independent of sharding.
 constexpr uint32_t kExploreTag = 0x40000000u;
-// Warps per block at most: one copy of the weights serves all of them, and with 75-90 KB of weights one block is what
-// fits an SM, so this is also the residency.  16 warps leave 128 registers per thread; tag 3+1 at H = 64 (four agents'
-// state next to the 64 registers of h1) needs more than that, and gets 12-warp blocks and up to 168 registers instead.
+// S: 2 blocks (8 uniforms) per agent and step when every action vector has at most 8 entries, else 4 (simple_reference:
+// 15).  S = 2 for the 5-logit programs keeps their stream what it has always been.
+template <class P>
+__host__ __device__ constexpr int mlp_max_act_dim() { int m = 0; for (int i = 0; i < P::A; ++i) m = P::act_dim(i) > m ? P::act_dim(i) : m; return m; }
+template <class P>
+__host__ __device__ constexpr int mlp_explore_stride() { return mlp_max_act_dim<P>() <= 8 ? 2 : 4; }
+// Warps per block at most: one copy of the weights serves all of them, and with 45-90 KB of weights one block is what
+// fits an SM, so this is also the residency.  16 warps leave 128 registers per thread.  Two programs need more at
+// H = 64 and get 12-warp blocks and up to 168 registers instead: tag 3+1 (four agents' state next to the 64 registers
+// of h1) and simple_reference (two 8-column logit tiles and 20 comm floats next to h1; it spills at 128).
 template <class P, int H>
-__host__ __device__ constexpr int mlp_block_warps() { return (H == 64 && P::A >= 4) ? 12 : 16; }
+__host__ __device__ constexpr int mlp_block_warps() { return (H == 64 && (P::A >= 4 || mlp_max_act_dim<P>() > 8)) ? 12 : 16; }
 
 struct MlpPolicyArgs {
     StepArgs s;
@@ -1031,11 +1053,11 @@ struct MlpPolicyArgs {
     int32_t explore;
     uint64_t seed, epoch, world_offset;
     float *rew_steps;               // [T][A][n] or null
-    float *act_rec[kMaxA];          // [T][n][5] per agent, or null: the action applied (sampled when exploring)
+    float *act_rec[kMaxA];          // [T][n][act_dim_i] per agent, or null: the action applied (sampled when exploring)
     float *obs_rec[kMaxA];          // [T][n][obs_dim_i] per agent, or null: the observation the actor saw at step t
     const float *w1[kMaxA], *b1[kMaxA];   // torch nn.Linear layout: [H][obs_dim_i], [H]
     const float *w2[kMaxA], *b2[kMaxA];   // [H][H], [H]
-    const float *w3[kMaxA], *b3[kMaxA];   // [5][H], [5]
+    const float *w3[kMaxA], *b3[kMaxA];   // [act_dim_i][H], [act_dim_i]
 };
 static_assert(sizeof(MlpPolicyArgs) <= 4096, "kernel parameter space");
 
@@ -1043,18 +1065,22 @@ template <class P, int H>
 struct MlpShape {
     static constexpr int NT = H / 8;                                   // n-tiles of a hidden layer (= its k-tiles)
     __host__ __device__ static constexpr int kt1(int i) { return (P::obs_dim(i) + 7) / 8; }
-    // per agent, in floats: B fragments [k-tile][n-tile][lane][2] of W1, W2, W3, then b1 [H], b2 [H], b3 [8]
+    __host__ __device__ static constexpr int nout(int i) { return (P::act_dim(i) + 7) / 8 * 8; }   // layer-3 columns
+    // per agent, in floats: B fragments [k-tile][n-tile][lane][2] of W1, W2, W3, then b1 [H], b2 [H], b3 [NOUT]; the
+    // rows of W3 and b3 at and beyond act_dim are zero
     __host__ __device__ static constexpr int w2_off(int i) { return 64 * kt1(i) * NT; }
     __host__ __device__ static constexpr int w3_off(int i) { return w2_off(i) + 64 * NT * NT; }
-    __host__ __device__ static constexpr int b1_off(int i) { return w3_off(i) + 64 * NT; }
+    __host__ __device__ static constexpr int b1_off(int i) { return w3_off(i) + 64 * NT * (nout(i) / 8); }
     __host__ __device__ static constexpr int b2_off(int i) { return b1_off(i) + H; }
     __host__ __device__ static constexpr int b3_off(int i) { return b2_off(i) + H; }
-    __host__ __device__ static constexpr int agent_floats(int i) { return b3_off(i) + 8; }
+    __host__ __device__ static constexpr int agent_floats(int i) { return b3_off(i) + nout(i); }
     __host__ __device__ static constexpr int agent_off(int i) { int s = 0; for (int j = 0; j < i; ++j) s += agent_floats(j); return s; }
     static constexpr int kWeightFloats = agent_off(P::A);
-    // per warp: [observation tile][logit tile 32 x 9]; the final observations are written through the same tile
+    // per warp: [observation tile][logit tile 32 x (max NOUT + 1)]; the final observations are written through the
+    // same tile.  The odd pitch keeps each lane's row reads conflict-free.
     __host__ __device__ static constexpr int obs_tile_floats() { int m = 0; for (int i = 0; i < P::A; ++i) m = 32 * Shape<P>::obs_pitch(i) > m ? 32 * Shape<P>::obs_pitch(i) : m; return (m + 3) & ~3; }
-    static constexpr int kLogitPitch = 9;
+    __host__ __device__ static constexpr int max_nout() { int m = 0; for (int i = 0; i < P::A; ++i) m = nout(i) > m ? nout(i) : m; return m; }
+    static constexpr int kLogitPitch = max_nout() + 1;
     static constexpr int kLogitOff = obs_tile_floats();
     static constexpr int kWarpFloats = (kLogitOff + 32 * kLogitPitch + 3) & ~3;
     static_assert(MPE_COMPACT_OBS, "write_observations must use one shared observation slot");
@@ -1096,13 +1122,33 @@ __device__ __forceinline__ void relu_tf32_frag(uint32_t (&a)[4], const float (&c
     a[3] = to_tf32(fmaxf(c[3], 0.0f));   // row g+8, k = 2q+1
 }
 
+// pr[B, B + K) = softmax(z[B, B + K)): one action sub-space.  The operation order is the one of every other softmax
+// here (the max is exact in any order; the sum runs from the first entry to the last).
+template <int B, int K, int N>
+__device__ __forceinline__ void softmax_segment(const float (&z)[N], float (&pr)[N]) {
+    static_assert(B + K <= N, "segment inside the action vector");
+    float m = z[B];
+#pragma unroll
+    for (int c = 1; c < K; ++c) m = fmaxf(m, z[B + c]);
+    float e[K], sum = 0.0f;
+#pragma unroll
+    for (int c = 0; c < K; ++c) { e[c] = expf(__fsub_rn(z[B + c], m)); sum = __fadd_rn(sum, e[c]); }
+#pragma unroll
+    for (int c = 0; c < K; ++c) pr[B + c] = __fdiv_rn(e[c], sum);
+}
+
 // one agent of the tensor-core actor for the warp's 32 worlds: observation -> tile -> 3 GEMMs -> this lane's logits ->
-// (Gumbel-)softmax -> decoded (u.x, u.y).  Called by all 32 lanes (mma.sync is warp-collective).
+// (Gumbel-)softmax per sub-space -> decoded (u.x, u.y), and a speaker's utterance into cact[I * dim_c ...].  Called by
+// all 32 lanes (mma.sync is warp-collective).
 template <class P, int H, int I>
 __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typename P::W &w, const float *__restrict__ Wsm,
-                                            float *s_warp, int lane, int t, int rows, bool active, int64_t w0, int64_t wi) {
+                                            float *s_warp, int lane, int t, int rows, bool active, int64_t w0, int64_t wi,
+                                            float *cact) {
     using S = MlpShape<P, H>;
     constexpr int OD = P::obs_dim(I), KT1 = S::kt1(I), NT = S::NT, PITCH = ObsTile<OD>::kPitch;
+    constexpr int AD = P::act_dim(I), NO = S::nout(I) / 8;
+    constexpr int MOVE = P::movable(I) ? 5 : 0, COMM = I < P::NS ? P::DIMC : 0;   // sub-spaces, speakers come first
+    static_assert(MOVE + COMM == AD && AD > 0, "action vector = [movement][utterance]");
     const DevDesc &d = pa.s.d;
     const int64_t n = pa.s.n;
     float *tile = s_warp;
@@ -1160,11 +1206,12 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
         for (int nt = 0; nt < NT; ++nt) relu_tf32_frag(x1[mt][nt], h[mt][nt]);
     // ---- layers 2 and 3, one 8-unit tile of h2 at a time: logits += relu(x1 . W2^T[:, tile] + b2[tile]) . W3^T[tile, :]
     const float *W2 = Wsm + S::w2_off(I), *W3 = Wsm + S::w3_off(I), *B2 = Wsm + S::b2_off(I), *B3 = Wsm + S::b3_off(I);
-    float lg[2][4];
-    {
-        const float2 b = *reinterpret_cast<const float2 *>(B3 + 2 * tq);
+    float lg[2][NO][4];
 #pragma unroll
-        for (int mt = 0; mt < 2; ++mt) { lg[mt][0] = b.x; lg[mt][1] = b.y; lg[mt][2] = b.x; lg[mt][3] = b.y; }
+    for (int ot = 0; ot < NO; ++ot) {
+        const float2 b = *reinterpret_cast<const float2 *>(B3 + ot * 8 + 2 * tq);
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) { lg[mt][ot][0] = b.x; lg[mt][ot][1] = b.y; lg[mt][ot][2] = b.x; lg[mt][ot][3] = b.y; }
     }
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
@@ -1178,62 +1225,74 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
             mma_tf32(c[0], x1[0][kt], b);
             mma_tf32(c[1], x1[1][kt], b);
         }
-        const float2 b3 = *reinterpret_cast<const float2 *>(W3 + (nt * 32 + lane) * 2);
 #pragma unroll
-        for (int mt = 0; mt < 2; ++mt) {
-            uint32_t x2[4];
-            relu_tf32_frag(x2, c[mt]);
-            mma_tf32(lg[mt], x2, b3);
+        for (int ot = 0; ot < NO; ++ot) {
+            const float2 b3 = *reinterpret_cast<const float2 *>(W3 + ((nt * NO + ot) * 32 + lane) * 2);
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt) {
+                uint32_t x2[4];
+                relu_tf32_frag(x2, c[mt]);
+                mma_tf32(lg[mt][ot], x2, b3);
+            }
         }
     }
     // ---- logits back to their lane (row r = world w0 + r) ----
 #pragma unroll
-    for (int mt = 0; mt < 2; ++mt) {
-        float *r0 = lgs + (mt * 16 + gq) * S::kLogitPitch + 2 * tq, *r1 = r0 + 8 * S::kLogitPitch;
-        r0[0] = lg[mt][0]; r0[1] = lg[mt][1];
-        r1[0] = lg[mt][2]; r1[1] = lg[mt][3];
-    }
-    __syncwarp();
-    float z[5];
+    for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-    for (int c = 0; c < 5; ++c) z[c] = lgs[lane * S::kLogitPitch + c];
+        for (int ot = 0; ot < NO; ++ot) {
+            float *r0 = lgs + (mt * 16 + gq) * S::kLogitPitch + ot * 8 + 2 * tq, *r1 = r0 + 8 * S::kLogitPitch;
+            r0[0] = lg[mt][ot][0]; r0[1] = lg[mt][ot][1];
+            r1[0] = lg[mt][ot][2]; r1[1] = lg[mt][ot][3];
+        }
+    __syncwarp();
+    float z[AD];
+#pragma unroll
+    for (int c = 0; c < AD; ++c) z[c] = lgs[lane * S::kLogitPitch + c];
     if (pa.explore) {                                      // Gumbel-softmax sample (see the definition above)
         const uint64_t gw = pa.world_offset + static_cast<uint64_t>(wi);
         const uint2 key = make_uint2(static_cast<uint32_t>(pa.seed), static_cast<uint32_t>(pa.seed >> 32));
-        const uint32_t c3 = kExploreTag | (static_cast<uint32_t>(t * P::A + I) * 2u);
-        const uint4 ctr = make_uint4(static_cast<uint32_t>(gw), static_cast<uint32_t>(gw >> 32), static_cast<uint32_t>(pa.epoch), c3);
-        const uint4 r0 = philox4x32_10(ctr, key);
-        const uint4 r1 = philox4x32_10(make_uint4(ctr.x, ctr.y, ctr.z, c3 | 1u), key);
-        const uint32_t bits[5] = {r0.x, r0.y, r0.z, r0.w, r1.x};
+        const uint32_t c3 = kExploreTag | (static_cast<uint32_t>(t * P::A + I) * static_cast<uint32_t>(mlp_explore_stride<P>()));
+        uint32_t bits[(AD + 3) / 4 * 4];
 #pragma unroll
-        for (int c = 0; c < 5; ++c) {
+        for (int b = 0; b < (AD + 3) / 4; ++b) {
+            const uint4 r = philox4x32_10(make_uint4(static_cast<uint32_t>(gw), static_cast<uint32_t>(gw >> 32),
+                                                     static_cast<uint32_t>(pa.epoch), c3 | static_cast<uint32_t>(b)), key);
+            bits[4 * b] = r.x; bits[4 * b + 1] = r.y; bits[4 * b + 2] = r.z; bits[4 * b + 3] = r.w;
+        }
+#pragma unroll
+        for (int c = 0; c < AD; ++c) {
             const float u = __fmul_rn(__fadd_rz(static_cast<float>(bits[c] >> 8), 0.5f), 0x1p-24f);
             z[c] = __fsub_rn(z[c], logf(-logf(u)));
         }
     }
-    const float m = fmaxf(fmaxf(fmaxf(z[0], z[1]), fmaxf(z[2], z[3])), z[4]);
-    float e[5], sum = 0.0f;
-#pragma unroll
-    for (int c = 0; c < 5; ++c) { e[c] = expf(__fsub_rn(z[c], m)); sum = __fadd_rn(sum, e[c]); }
-    float pr[5];
-#pragma unroll
-    for (int c = 0; c < 5; ++c) pr[c] = __fdiv_rn(e[c], sum);
+    float pr[AD];
+    if constexpr (MOVE > 0) softmax_segment<0, MOVE>(z, pr);
+    if constexpr (COMM > 0) softmax_segment<MOVE, COMM>(z, pr);
     if (pa.act_rec[I] != nullptr && active) {
-        float *rec = pa.act_rec[I] + (static_cast<int64_t>(t) * n + wi) * 5;
+        float *rec = pa.act_rec[I] + (static_cast<int64_t>(t) * n + wi) * AD;
 #pragma unroll
-        for (int c = 0; c < 5; ++c) rec[c] = pr[c];
+        for (int c = 0; c < AD; ++c) rec[c] = pr[c];
     }
-    // _set_action (environment.py:173-181), the arithmetic of decode_rows
-    float x = 0.0f, y = 0.0f;
-    x += pr[1] - pr[2];
-    y += pr[3] - pr[4];
-    return make_float2(__fmul_rn(x, d.a_sens[I]), __fmul_rn(y, d.a_sens[I]));
+    // _set_action (environment.py:173-190), the arithmetic of decode_rows
+    if constexpr (COMM > 0) {
+#pragma unroll
+        for (int q = 0; q < COMM; ++q) cact[I * P::DIMC + q] = pr[MOVE + q];
+    }
+    if constexpr (MOVE > 0) {
+        float x = 0.0f, y = 0.0f;
+        x += pr[1] - pr[2];
+        y += pr[3] - pr[4];
+        return make_float2(__fmul_rn(x, d.a_sens[I]), __fmul_rn(y, d.a_sens[I]));
+    } else {
+        return make_float2(0.0f, 0.0f);                    // immovable: no force, and physics<P> never moves it
+    }
 }
 
 template <class P, int H>
 __global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_rollout_kernel(const __grid_constant__ MlpPolicyArgs pa) {
-    static_assert(P::NS == 0 && (H == 32 || H == 64), "MLP policy rollout: silent agents, hidden width 32 or 64");
-    constexpr int A = P::A, L = P::L;
+    static_assert(H == 32 || H == 64, "MLP policy rollout: hidden width 32 or 64");
+    constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     using S = MlpShape<P, H>;
     const StepArgs &a = pa.s;
     extern __shared__ __align__(16) float smem[];
@@ -1245,12 +1304,12 @@ __global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_r
         float *base = smem + S::agent_off(i);
         stage_fragments<S::kt1(i), S::NT, false>(base, pa.w1[i], H, OD);
         stage_fragments<S::NT, S::NT, true>(base + S::w2_off(i), pa.w2[i], H, H);
-        stage_fragments<S::NT, 1, true>(base + S::w3_off(i), pa.w3[i], 5, H);
+        stage_fragments<S::NT, S::nout(i) / 8, true>(base + S::w3_off(i), pa.w3[i], P::act_dim(i), H);
         for (int q = threadIdx.x; q < H; q += blockDim.x) {
             base[S::b1_off(i) + q] = pa.b1[i][q];
             base[S::b2_off(i) + q] = pa.b2[i][q];
         }
-        for (int q = threadIdx.x; q < 8; q += blockDim.x) base[S::b3_off(i) + q] = q < 5 ? pa.b3[i][q] : 0.0f;
+        for (int q = threadIdx.x; q < S::nout(i); q += blockDim.x) base[S::b3_off(i) + q] = q < P::act_dim(i) ? pa.b3[i][q] : 0.0f;
     });
     __syncthreads();
 
@@ -1279,6 +1338,10 @@ __global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_r
 #pragma unroll
         for (int q = 0; q < P::G; ++q) w.g[q] = a.goal[q * n + wi];
     }
+    if constexpr (NC > 0) {
+#pragma unroll
+        for (int q = 0; q < NC; ++q) w.c[q] = a.comm[q * n + wi];
+    }
 
     float rsum[A];
 #pragma unroll
@@ -1286,14 +1349,17 @@ __global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_r
 #pragma unroll 1
     for (int t = 0; t < pa.T; ++t) {
         float ux[A], uy[A];
+        float cact[NC > 0 ? NC : 1];
         P::prepare(d, w);
         static_for<A>([&](auto ic) {
             constexpr int i = decltype(ic)::value;
-            const float2 u = mlp_agent<P, H, i>(pa, w, smem + S::agent_off(i), s_warp, lane, t, rows, active, w0, wi);
+            const float2 u = mlp_agent<P, H, i>(pa, w, smem + S::agent_off(i), s_warp, lane, t, rows, active, w0, wi, cact);
             ux[i] = u.x;
             uy[i] = u.y;
         });
         physics<P>(d, w, ux, uy);
+#pragma unroll
+        for (int q = 0; q < NC; ++q) w.c[q] = cact[q];      // update_agent_state (core.py:171-177), as the fused step
         float rew[A];
         P::reward(d, w, rew, nullptr);
         if (a.flags & MPE_FLAG_SHARED_REWARD) {
@@ -1314,6 +1380,8 @@ __global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_r
 #pragma unroll
         for (int i = 0; i < A; ++i)
             if (P::movable(i)) a.pv[i * n + wi] = make_float4(w.px[i], w.py[i], w.vx[i], w.vy[i]);
+#pragma unroll
+        for (int q = 0; q < NC; ++q) a.comm[q * n + wi] = w.c[q];
     }
     P::prepare(d, w);
     __syncwarp();                  // every lane has read its logits before the tile is reused
@@ -1535,6 +1603,7 @@ struct Program {
     int policy_weight_floats[2];
     void (*mlp_fn[2])(MlpPolicyArgs);  // the same with the two-hidden-layer actor on the tensor cores, H = 32 / 64
     int mlp_weight_floats[2], mlp_warp_floats[2], mlp_warps[2];
+    int mlp_explore_stride;            // Philox blocks per (step, agent) of its exploration noise
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
     int rollout_smem;   // dynamic shared memory per WARP of the rollout kernel
     KernelFn lanes_fn;  // lane-per-agent fused step (simple_spread only), else null
@@ -1571,6 +1640,8 @@ static Program make_program() {
         p.policy_fn[1] = mpe_policy_rollout_kernel<P, 64>;
         p.policy_weight_floats[0] = PolicyShape<P, 32>::kWeightFloats;
         p.policy_weight_floats[1] = PolicyShape<P, 64>::kWeightFloats;
+    }
+    if constexpr (MlpBuilt<P>::value) {
         p.mlp_fn[0] = mpe_policy_mlp_rollout_kernel<P, 32>;
         p.mlp_fn[1] = mpe_policy_mlp_rollout_kernel<P, 64>;
         p.mlp_weight_floats[0] = MlpShape<P, 32>::kWeightFloats;
@@ -1579,6 +1650,7 @@ static Program make_program() {
         p.mlp_warp_floats[1] = MlpShape<P, 64>::kWarpFloats;
         p.mlp_warps[0] = mlp_block_warps<P, 32>();
         p.mlp_warps[1] = mlp_block_warps<P, 64>();
+        p.mlp_explore_stride = mlp_explore_stride<P>();
     }
     p.smem_bytes = Shape<P>::kWarpBytes;  // per warp
     p.A = P::A; p.L = P::L; p.NS = P::NS; p.DIMC = P::DIMC; p.INFO = P::INFO; p.G = P::G;
@@ -2192,8 +2264,9 @@ extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, fl
     if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || h->prog->mlp_fn[k] == nullptr) return MPE_ERR_UNSUPPORTED;
     if (flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
     if (rew_steps != nullptr && !ok4(rew_steps)) return MPE_ERR_BAD_ARG;
-    // the Philox counter word holds (t * A + i) * 2 + b below the tag bit
-    if (explore && static_cast<int64_t>(n_steps) * h->prog->A * 2 > static_cast<int64_t>(kExploreTag)) return MPE_ERR_BAD_ARG;
+    // the Philox counter word holds (t * A + i) * S + b below the tag bit
+    if (explore && static_cast<int64_t>(n_steps) * h->prog->A * h->prog->mlp_explore_stride > static_cast<int64_t>(kExploreTag))
+        return MPE_ERR_BAD_ARG;
     NvtxRange range("mpe_rollout_policy_mlp");
     MlpPolicyArgs pa{};
     StepArgs &a = pa.s;

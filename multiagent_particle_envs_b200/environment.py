@@ -252,18 +252,23 @@ class MultiAgentEnv(_Env):
         b1 [H], W2 [5, H], b2 [5]) in torch's Linear layout, H = 32 or 64.
 
         Two hidden layers, MADDPG's actor (mpe_rollout_policy_mlp, TF32 tensor cores): policies[i] is a
-        `torch.nn.Sequential(Linear(obs_dim_i, H), ReLU(), Linear(H, H), ReLU(), Linear(H, 5))` or the tuple (W1, b1, W2,
-        b2, W3, b3), H = 32 or 64.  explore_seed (an int) makes every agent act with the Gumbel-softmax sample
-        softmax(logits - log(-log u)) instead of softmax(logits); the noise is keyed by (explore_seed, self.explore_epoch,
-        global world index, step, agent) and self.explore_epoch advances by one per exploring call.
-        record_observations=True returns extras["observations"], a list of [T, N, obs_dim_i] tensors: the observation
-        agent i acted on at each step.  Both options need the two-hidden-layer actor.
+        `torch.nn.Sequential(Linear(obs_dim_i, H), ReLU(), Linear(H, H), ReLU(), Linear(H, act_dim_i))` or the tuple
+        (W1, b1, W2, b2, W3, b3), H = 32 or 64.  The act_dim_i outputs split into the agent's action sub-spaces as the
+        action vector does -- 5 movement logits if it is movable, then dim_c utterance logits if it speaks -- and the
+        action is one softmax per sub-space (MADDPG's SoftMultiCategoricalPd).  An utterance becomes the world's comm
+        state after the step, so the other agents observe it from the next step on.  explore_seed (an int) makes every
+        agent act with the Gumbel-softmax sample softmax(logits - log(-log u)) per sub-space instead; the noise is keyed
+        by (explore_seed, self.explore_epoch, global world index, step, agent) and self.explore_epoch advances by one per
+        exploring call.  record_observations=True returns extras["observations"], a list of [T, N, obs_dim_i] tensors:
+        the observation agent i acted on at each step.  Both options need the two-hidden-layer actor.  Built for simple,
+        simple_spread N=3, simple_tag 3+1, simple_speaker_listener, simple_reference, simple_crypto, simple_adversary
+        (3 agents) and simple_push (2 agents); other programs raise MpeError.
 
         Returns (obs_n, reward_sum_n, done_n, info_n, extras) for the state after the last step; extras["actions"]
-        (record_actions) is a list of [T, N, 5] tensors with the actions taken, extras["rewards"] (per_step_rewards) a
-        [T, n, N] tensor.  World state lives in registers for all T steps.  Batched CUDA mode; scenarios whose agents all
-        move and are silent and whose program was built with the policy kernels (simple, simple_spread N=3, simple_tag
-        3+1) -- anything else raises."""
+        (record_actions) is a list of [T, N, act_dim_i] tensors with the actions taken ([T, N, 5] for the one-hidden-layer
+        actor), extras["rewards"] (per_step_rewards) a [T, n, N] tensor.  World state lives in registers for all T steps.
+        Batched CUDA mode.  The one-hidden-layer actor needs a scenario whose agents all move and are silent and whose
+        program was built with that kernel (simple, simple_spread N=3, simple_tag 3+1) -- anything else raises."""
         import torch
         world = self.world
         if not world.batched:
@@ -315,13 +320,14 @@ class MultiAgentEnv(_Env):
         world = self.world
         nw = world.bind()
         N, T = nw.n_env, int(n_steps)
-        params, hidden = mlp_actor_params(policies, nw.obs_dims)
+        nw.require_mlp_actor()   # a program without the kernel is refused as such, before its heads are checked
+        params, hidden = mlp_actor_params(policies, nw.obs_dims, nw.act_dims)
         keep = [[t.detach().to(device=nw.device, dtype=torch.float32).contiguous() for t in p] for p in params]
         w_ptrs = [_lib.ptr_array([keep[i][j].data_ptr() for i in range(self.n)]) for j in range(6)]
         out = nw.out if self.reuse_buffers else nw.new_outputs()
         dev = dict(dtype=torch.float32, device=nw.device)
         rew_steps = torch.empty((T, self.n, N), **dev) if per_step_rewards else None
-        actions = [torch.empty((T, N, 5), **dev) for _ in range(self.n)] if record_actions else None
+        actions = [torch.empty((T, N, ad), **dev) for ad in nw.act_dims] if record_actions else None
         observations = [torch.empty((T, N, od), **dev) for od in nw.obs_dims] if record_observations else None
         seed = None if explore_seed is None else int(explore_seed) & 0xFFFFFFFFFFFFFFFF
         nw.rollout_policy_mlp(w_ptrs, hidden, T, out, self._flags(), rew_steps,
@@ -594,7 +600,8 @@ class MultiAgentEnv(_Env):
 
 
 # ---- the two-hidden-layer actor of rollout_policy (MADDPG's mlp_model) ------------------------------
-_MLP_SHAPE = "nn.Sequential(Linear(obs_dim, H), ReLU(), Linear(H, H), ReLU(), Linear(H, 5)) or a tuple (W1, b1, W2, b2, W3, b3)"
+_MLP_SHAPE = ("nn.Sequential(Linear(obs_dim, H), ReLU(), Linear(H, H), ReLU(), Linear(H, act_dim)) or a tuple "
+              "(W1, b1, W2, b2, W3, b3)")
 
 
 def _has_two_hidden_layers(pol):
@@ -606,12 +613,15 @@ def _has_two_hidden_layers(pol):
     return isinstance(pol, (tuple, list)) and len(pol) == 6
 
 
-def mlp_actor_params(policies, obs_dims):
+def mlp_actor_params(policies, obs_dims, act_dims=None):
     """policies -> ([(W1, b1, W2, b2, W3, b3) per agent], H) in torch's Linear layout, or ValueError.  A module must be
     an nn.Sequential whose layers are exactly Linear, ReLU, Linear, ReLU, Linear (types and order are checked: that
-    order is the one the kernel evaluates); shapes must be W1 [H, obs_dim_i], b1 [H], W2 [H, H], b2 [H], W3 [5, H],
-    b3 [5] with one H for all agents.  No device is needed."""
+    order is the one the kernel evaluates); shapes must be W1 [H, obs_dim_i], b1 [H], W2 [H, H], b2 [H],
+    W3 [act_dim_i, H], b3 [act_dim_i] with one H for all agents.  act_dims None means 5 (movement only) for every agent.
+    No device is needed."""
     import torch
+    if act_dims is None:
+        act_dims = [5] * len(obs_dims)
     if len(policies) != len(obs_dims):
         raise ValueError("expected %d policies, got %d" % (len(obs_dims), len(policies)))
     params, hidden = [], None
@@ -635,11 +645,12 @@ def mlp_actor_params(policies, obs_dims):
         H = int(ts[0].shape[0])
         if hidden is None:
             hidden = H
-        want = ((hidden, obs_dims[i]), (hidden,), (hidden, hidden), (hidden,), (5, hidden), (5,))
+        ad = act_dims[i]
+        want = ((hidden, obs_dims[i]), (hidden,), (hidden, hidden), (hidden,), (ad, hidden), (ad,))
         got = tuple(tuple(t.shape) for t in ts)
         if got != want:
-            raise ValueError("policy %d: expected W1 [%d, %d], b1 [%d], W2 [%d, %d], b2 [%d], W3 [5, %d], b3 [5]; got %s"
-                             % (i, hidden, obs_dims[i], hidden, hidden, hidden, hidden, hidden,
+            raise ValueError("policy %d: expected W1 [%d, %d], b1 [%d], W2 [%d, %d], b2 [%d], W3 [%d, %d], b3 [%d]; got %s"
+                             % (i, hidden, obs_dims[i], hidden, hidden, hidden, hidden, ad, hidden, ad,
                                 ", ".join(str(list(s)) for s in got)))
         params.append(tuple(ts))
     return params, hidden

@@ -273,6 +273,15 @@ class NativeWorld(ShapeHandle):
                                           out.done_ptr, flags, self._stream()), "mpe_rollout_policy")
         return out
 
+    def require_mlp_actor(self):
+        """MpeError unless the library has the two-hidden-layer actor for this program.  mpe_rollout_policy_mlp checks
+        the program before any pointer, so a call without state or weights answers that and runs nothing."""
+        none = _lib.ptr_array([None] * self.n_agents)
+        rc = self.lib.mpe_rollout_policy_mlp(self.handle, None, None, None, None, none, none, none, none, none, none, 32,
+                                             0, 0, 0, 0, 0, None, None, None, None, None, None, 0, self._stream())
+        if rc == _lib.ERR_UNSUPPORTED:
+            check(rc, "mpe_rollout_policy_mlp")
+
     def rollout_policy_mlp(self, w_ptrs, hidden, n_steps, out=None, flags=0, rew_steps=None, act_rec_ptrs=None,
                            obs_rec_ptrs=None, explore_seed=None, explore_epoch=0):
         """n_steps fused steps in ONE launch with every agent's two-hidden-layer actor evaluated on the tensor cores

@@ -5,8 +5,10 @@
       --layers 3: MADDPG's Linear-ReLU-Linear-ReLU-Linear on the tensor cores in TF32 (mpe_rollout_policy_mlp),
       --explore: with the Gumbel-softmax sample instead of softmax (--layers 3 only);
   (b) the same actors as torch modules + env.step, all captured in one CUDA graph (rollout.GraphedRollout).
-Device time per step of each.  With --layers 3 also the actor's FLOPs per step, computed from the padded shapes the
-kernel multiplies (2 (K1 H + H H + 8 H) per agent and world, K1 = obs_dim rounded up to 8), the in-kernel rollout's
+Device time per step of each.  With --layers 3 the actor of agent i has act_dim_i outputs and its action is one
+(Gumbel-)softmax per action sub-space (5 movement logits if the agent moves, then dim_c utterance logits if it speaks).
+Also the actor's FLOPs per step, computed from the padded shapes the kernel multiplies (2 (K1 H + H H + NOUT H) per
+agent and world, K1 = obs_dim and NOUT = act_dim rounded up to 8), the in-kernel rollout's
 achieved TFLOP/s (actor FLOPs over the whole step's time: physics, observations and rewards are in that time too),
 torch's float32 matmul precision for the graphed loop, and the card's name and power limit read in the same run."""
 import argparse
@@ -19,8 +21,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-def actor_flops_per_step(obs_dims, H, n):
-    return sum(2 * (((od + 7) // 8 * 8) * H + H * H + 8 * H) for od in obs_dims) * n
+def actor_flops_per_step(obs_dims, act_dims, H, n):
+    return sum(2 * (((od + 7) // 8 * 8) * H + H * H + ((ad + 7) // 8 * 8) * H) for od, ad in zip(obs_dims, act_dims)) * n
+
+
+def sub_spaces(world):
+    """per agent, the widths of its action sub-spaces in action-vector order: [5] if movable, then [dim_c] if it speaks"""
+    return [([5] if a.movable else []) + ([world.dim_c] if not a.silent else []) for a in world.agents]
 
 
 def card_info():
@@ -61,7 +68,8 @@ def main():
         mods = [torch.nn.Sequential(torch.nn.Linear(od, H), torch.nn.ReLU(), torch.nn.Linear(H, 5)).to(dev) for od in nw.obs_dims]
     else:
         mods = [torch.nn.Sequential(torch.nn.Linear(od, H), torch.nn.ReLU(), torch.nn.Linear(H, H), torch.nn.ReLU(),
-                                    torch.nn.Linear(H, 5)).to(dev) for od in nw.obs_dims]
+                                    torch.nn.Linear(H, ad)).to(dev) for od, ad in zip(nw.obs_dims, nw.act_dims)]
+    segs = sub_spaces(env.world) if args.layers == 3 else [[5]] * len(nw.obs_dims)
     res = {"config": {"scenario": args.scenario, "n_env": n, "T": T, "hidden": H}}
     if args.layers == 3:
         res["config"].update(layers=3, explore=args.explore, torch_float32_matmul_precision=torch.get_float32_matmul_precision())
@@ -79,17 +87,22 @@ def main():
     sec = e0.elapsed_time(e1) / 1e3 / (args.reps * T)
     res["in_kernel"] = {"us_per_step": 1e6 * sec, "env_steps_per_sec": n / sec}
     if args.layers == 3:
-        flops = actor_flops_per_step(nw.obs_dims, H, n)
+        flops = actor_flops_per_step(nw.obs_dims, nw.act_dims, H, n)
         res["in_kernel"].update(actor_flop_per_step=flops, actor_tflops=flops / sec / 1e12)
     # (b) torch actors + env.step in one CUDA graph
     env2 = make_env(args.scenario, num_envs=n, device=dev)
     env2.reset()
 
+    def act(z, seg):   # one softmax per action sub-space
+        if len(seg) == 1:
+            return torch.softmax(z, -1)
+        return torch.cat([torch.softmax(p, -1) for p in torch.split(z, seg, -1)], -1)
+
     def policy(obs_n):
         if args.explore:   # the same Gumbel-softmax sample, noise from torch's generator
-            return [torch.softmax(m(o) - torch.log(-torch.log(torch.rand(o.shape[0], 5, device=dev))), -1)
-                    for m, o in zip(mods, obs_n)]
-        return [torch.softmax(m(o), -1) for m, o in zip(mods, obs_n)]
+            return [act(m(o) - torch.log(-torch.log(torch.rand(o.shape[0], sum(seg), device=dev))), seg)
+                    for m, o, seg in zip(mods, obs_n, segs)]
+        return [act(m(o), seg) for m, o, seg in zip(mods, obs_n, segs)]
 
     ro = GraphedRollout(env2, policy, steps=T)
     for _ in range(2):
