@@ -23,7 +23,7 @@
  * API-facing per-agent tensors are row-major exactly as a trainer holds them:
  *   act_n[i]  float  [n_env][act_dim_i]  (5 physical one-hot/probabilities, then dim_c comm)
  *   obs_n[i]  float  [n_env][obs_dim_i]    (base pointer 16-byte aligned; act_n[i] may be 4-byte aligned,
- *                                           16-byte alignment enables the TMA path)
+ *                                           16-byte alignment enables the cp.async path)
  *   rew       float  [A][n_env],  done uint8 [A][n_env],  info float [A][info_dim][n_env]
  */
 #ifndef MPE_B200_H

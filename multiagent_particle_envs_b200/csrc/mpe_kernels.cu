@@ -17,7 +17,6 @@
 #include <nvtx3/nvToolsExt.h>   // header-only NVTX v3: ranges cost a few ns unless a profiler is attached
 
 #include "mpe_scenarios.cuh"
-#include "mpe_spread_lanes.cuh"
 
 namespace mpe {
 
@@ -32,55 +31,36 @@ __device__ __forceinline__ void static_for(F &&f) {
 
 template <class P>
 struct Shape {
-    // warp-private staging, in floats: [mbarrier: 4][action tiles of all agents][observation tiles]
-    // Dense observation tiles (exact images of the global rows) each get their own slot, so that the
-    // rows of all agents are written first and then streamed out after ONE __syncwarp; padded tiles
-    // share one slot.
-    static constexpr int kBarFloats = 4;
+    // warp-private staging, in floats: [lead: 4][action tiles of all agents][one observation slot]
+    // Every observation tile of a warp shares the slot (write rows, sync, stream out, sync).  A slot per tile would
+    // make world_comm's staging 22 KB per warp and let shared memory cap residency at 10 warps per SM; shared, it is
+    // 6 KB and registers are the limit (16 warps per SM).
+    // The tiles start 16 bytes into the staging.  At offset 0, world_comm's fused step at 32 768 worlds measured 8-20 %
+    // slower on an H100 SXM (400 W), while spread N=3, tag and the open-loop rollout measured 0.3-8 % faster.
+    static constexpr int kLeadFloats = 4;
     __host__ __device__ static constexpr int act_floats(int i) { return 32 * (P::act_dim(i) | 1); }
-    __host__ __device__ static constexpr int act_off(int i) { int s = kBarFloats; for (int j = 0; j < i; ++j) s += act_floats(j); return s; }
+    __host__ __device__ static constexpr int act_off(int i) { int s = kLeadFloats; for (int j = 0; j < i; ++j) s += act_floats(j); return s; }
     __host__ __device__ static constexpr bool act_dense(int i) { return (P::act_dim(i) | 1) == P::act_dim(i); }
     __host__ __device__ static constexpr bool all_act_dense() { for (int i = 0; i < P::A; ++i) if (!act_dense(i)) return false; return true; }
-    __host__ __device__ static constexpr int act_bytes_total() { int s = 0; for (int i = 0; i < P::A; ++i) s += 32 * P::act_dim(i) * 4; return s; }
     __host__ __device__ static constexpr int obs_pitch(int i) {
         const int od = P::obs_dim(i), unit = (od % 2 == 0) ? 2 : 1;
         return ((od / unit) | 1) * unit;
     }
-    __host__ __device__ static constexpr bool obs_dense(int i) { return obs_pitch(i) == P::obs_dim(i); }
-    // Every observation tile of a warp shares ONE slot (write rows, sync, stream out, sync) -- MPE_COMPACT_OBS=1, the
-    // default.  With a private slot per dense tile (-DMPE_COMPACT_OBS=0: all rows written first, one sync, then
-    // streamed) the staging of world_comm is 22 KB per warp and shared memory caps residency at 10 warps per SM; shared
-    // it is 6 KB (spread N=3: 8.8 -> 4.3 KB) and registers are the limit (16 warps per SM).
-#ifndef MPE_COMPACT_OBS
-#define MPE_COMPACT_OBS 1
-#endif
-    __host__ __device__ static constexpr bool obs_private(int i) { return obs_dense(i) && !MPE_COMPACT_OBS; }
     __host__ __device__ static constexpr int obs_floats(int i) { return (32 * obs_pitch(i) + 3) & ~3; }
     __host__ __device__ static constexpr int obs_base() { return act_off(P::A); }
-    __host__ __device__ static constexpr int shared_obs_floats() { int m = 0; for (int i = 0; i < P::A; ++i) if (!obs_private(i)) m = obs_floats(i) > m ? obs_floats(i) : m; return m; }
-    __host__ __device__ static constexpr int obs_off(int i) {
-        if (!obs_private(i)) return obs_base();
-        int s = obs_base() + shared_obs_floats();
-        for (int j = 0; j < i; ++j) if (obs_private(j)) s += obs_floats(j);
-        return s;
-    }
     __host__ __device__ static constexpr int warp_floats() {
-        int s = obs_base() + shared_obs_floats();
-        for (int j = 0; j < P::A; ++j) if (obs_private(j)) s += obs_floats(j);
-        return (s + 3) & ~3;
+        int m = 0;
+        for (int i = 0; i < P::A; ++i) m = obs_floats(i) > m ? obs_floats(i) : m;
+        return (obs_base() + m + 3) & ~3;
     }
+    // cp.async destinations and the LDS.128 of the tile streams need every tile on a 16-byte boundary
+    __host__ __device__ static constexpr bool tiles_aligned() { for (int i = 0; i <= P::A; ++i) if (act_off(i) % 4) return false; return true; }
+    static_assert(tiles_aligned(), "every staging tile starts at a multiple of 4 floats");
     static constexpr int kWarpFloats = warp_floats();
     static constexpr int kWarpBytes = kWarpFloats * 4;
     // K-step rollout: a second set of action tiles behind the regular staging (step t+1 is prefetched while step t runs)
     static constexpr int kRolloutWarpFloats = kWarpFloats + ((obs_base() + 3) & ~3);
     static constexpr int kRolloutWarpBytes = kRolloutWarpFloats * 4;
-    // software-pipelined persistent step (mpe_pipe_kernel): per warp [regular staging incl. obs tiles][second action
-    // region][2 x state image: pv float4 [A][32], lm float2 [L][32], goal int [G][32]]
-    static constexpr int kStateFloats = (4 * P::A + 2 * P::L + P::G) * 32;
-    static constexpr int kPipeAct1 = kWarpFloats;
-    static constexpr int kPipeState0 = kPipeAct1 + ((obs_base() + 3) & ~3);
-    static constexpr int kPipeWarpFloats = kPipeState0 + 2 * kStateFloats;
-    static constexpr int kPipeWarpBytes = kPipeWarpFloats * 4;
     static constexpr int kNC = P::NS * P::DIMC;
 };
 
@@ -125,88 +105,6 @@ __device__ __forceinline__ void physics(const DevDesc &d, typename P::W &w, cons
 }
 
 
-// ---- warp-pair physics (SPLIT) ------------------------------------------------------------------------------------
-// The active (colliding) pairs of apply_environment_force, numbered in the reference's (a, b) order.
-template <class P>
-__host__ __device__ constexpr bool pair_active(int a, int b) {
-    return b > a && P::agent_collides(a) && (b < P::A ? P::agent_collides(b) : P::landmark_collides(b - P::A));
-}
-template <class P>
-__host__ __device__ constexpr int pair_index(int a, int b) {   // number of active pairs before (a, b)
-    int k = 0;
-    for (int aa = 0; aa < P::A; ++aa)
-        for (int bb = aa + 1; bb < P::A + P::L; ++bb) {
-            if (aa == a && bb == b) return k;
-            if (pair_active<P>(aa, bb)) ++k;
-        }
-    return k;
-}
-template <class P>
-__host__ __device__ constexpr int pair_count() { return pair_index<P>(P::A, P::A + P::L); }
-
-__device__ __forceinline__ void pair_sync(int id) { asm volatile("bar.sync %0, 64;" ::"r"(id) : "memory"); }
-
-// Same result as physics<P>, bit for bit, computed by TWO warps that hold the same 32 worlds: warp `half` evaluates the
-// contact forces of the pairs with index % 2 == half (the MUFU-heavy part) and publishes them in the pair's exchange
-// buffer `ex` ([pair][lane] float2); after the pair barrier both warps read ALL pair forces back and accumulate them in
-// the reference's order, then integrate.  The barrier also orders the partner's state loads before the in-place store.
-template <class P>
-__device__ __forceinline__ void physics_split(const DevDesc &d, typename P::W &w, const float (&ux)[P::A],
-                                              const float (&uy)[P::A], int half, float2 *ex, int lane, int bar_id) {
-    constexpr int A = P::A, L = P::L;
-    const float k = d.contact_margin, cf = d.contact_force;
-    static_for<A>([&](auto ac) {
-        static_for<A + L>([&](auto bc) {
-            constexpr int a = decltype(ac)::value, b = decltype(bc)::value;
-            if constexpr (pair_active<P>(a, b)) {
-                constexpr int idx = pair_index<P>(a, b);
-                if ((idx & 1) == half) {   // warp-uniform
-                    constexpr bool b_agent = b < A;
-                    constexpr int bi = b_agent ? b : 0, bl = b_agent ? 0 : b - A;
-                    const float bx = b_agent ? w.px[bi] : w.lx[bl];
-                    const float by = b_agent ? w.py[bi] : w.ly[bl];
-                    const float sb = b_agent ? d.a_size[bi] : d.l_size[bl];
-                    const float2 dl = sub2(make_float2(w.px[a], w.py[a]), make_float2(bx, by));
-                    ex[idx * 32 + lane] = pair_force(dl.x, dl.y, __fadd_rn(d.a_size[a], sb), cf, k, d.inv_margin);
-                }
-            }
-        });
-    });
-    pair_sync(bar_id);
-    float fx[A], fy[A];
-#pragma unroll
-    for (int i = 0; i < A; ++i) {  // apply_action_force (core.py:134-140)
-        fx[i] = ux[i];
-        fy[i] = uy[i];
-    }
-    static_for<A>([&](auto ac) {
-        static_for<A + L>([&](auto bc) {
-            constexpr int a = decltype(ac)::value, b = decltype(bc)::value;
-            if constexpr (pair_active<P>(a, b)) {
-                constexpr int idx = pair_index<P>(a, b);
-                const float2 f = ex[idx * 32 + lane];
-                if (P::movable(a)) {
-                    fx[a] = __fadd_rn(fx[a], f.x);
-                    fy[a] = __fadd_rn(fy[a], f.y);
-                }
-                if constexpr (b < A) {
-                    if (P::movable(b)) {
-                        fx[b] = __fsub_rn(fx[b], f.x);
-                        fy[b] = __fsub_rn(fy[b], f.y);
-                    }
-                }
-            }
-        });
-    });
-#pragma unroll
-    for (int i = 0; i < A; ++i) {
-        if (!P::movable(i)) continue;
-        const float4 r = integrate_entity<P::kSpeedLimit>(w.px[i], w.py[i], w.vx[i], w.vy[i], fx[i], fy[i], d.keep,
-                                                          d.a_dt_over_mass[i], d.dt, d.a_max_speed[i]);
-        w.px[i] = r.x; w.py[i] = r.y; w.vx[i] = r.z; w.vy[i] = r.w;
-    }
-}
-
 // MultiAgentEnv._set_action (environment.py:144-192) for this lane's world, from the warp's staged action tiles
 // (s_act = the warp's staging base; tile i starts at Shape<P>::act_off(i))
 template <class P, bool ALLOW_FORCE_DISCRETE = true>
@@ -248,69 +146,38 @@ __device__ __forceinline__ void decode_rows(const float *s_act, int lane, const 
     });
 }
 
-// observation rows of one 32-world tile: full warps write through the warp-private tiles and stream them out as
-// coalesced 16-byte stores; the batch's last, partial warp writes its rows straight to global memory.
-// `half` < 0: every agent; 0: agents [0, split_point); 1: agents [split_point, A) (warp pairs; the second warp also
-// computes the rewards, so it gets the smaller share: split_point = ceil(2A/3)).
-template <class P>
-__host__ __device__ constexpr int split_point() { return (2 * P::A + 2) / 3; }
-template <class P>
-__host__ __device__ constexpr int agent_half(int i) { return i < split_point<P>() ? 0 : 1; }
+// observation rows of one 32-world tile: full warps write each agent's rows into the warp's observation slot and
+// stream them out as coalesced 16-byte stores (not a TMA bulk store: the warp would have to stay resident until the
+// copy engine has read its shared memory); the batch's last, partial warp writes its rows straight to global memory.
 template <class P>
 __device__ __forceinline__ void write_observations(const StepArgs &a, const DevDesc &d, const typename P::W &w, float *s_warp,
-                                                   int lane, int rows, bool active, int64_t w0, int64_t wi, int half) {
+                                                   int lane, int rows, bool active, int64_t w0, int64_t wi) {
     constexpr int A = P::A;
+    float *slot = s_warp + Shape<P>::obs_base();
     if (rows == 32) {
-        // Tiles are private per agent (dense ones), so no barrier is needed between agents: all rows are
-        // written, one __syncwarp, then the warp streams every tile out as 16-byte stores and retires.
-        // (Not a TMA bulk store: the warp would have to stay resident until the copy engine has read its
-        // shared memory.)
         static_for<A>([&](auto ic) {
             constexpr int i = decltype(ic)::value;
             constexpr int OD = P::obs_dim(i);
-            if (half >= 0 && agent_half<P>(i) != half) return;     // warp-uniform: the partner warp writes this agent
-            TileWriter<OD> o(s_warp + Shape<P>::obs_off(i), lane);
+            TileWriter<OD> o(slot, lane);
             P::template observe<i>(d, w, o);
-            if constexpr (!Shape<P>::obs_private(i)) {  // tiles without a slot of their own share one
-                __syncwarp();
-                obs_tile_store<OD>(a.obs[i] + w0 * OD, s_warp + Shape<P>::obs_off(i), lane);
-                __syncwarp();
-            }
-        });
-        __syncwarp();
-        static_for<A>([&](auto ic) {
-            constexpr int i = decltype(ic)::value;
-            constexpr int OD = P::obs_dim(i);
-            if (half >= 0 && agent_half<P>(i) != half) return;
-            if constexpr (Shape<P>::obs_private(i)) obs_tile_store<OD>(a.obs[i] + w0 * OD, s_warp + Shape<P>::obs_off(i), lane);
+            __syncwarp();
+            obs_tile_store<OD>(a.obs[i] + w0 * OD, slot, lane);
+            __syncwarp();
         });
     } else if (active) {  // the batch's last, partial warp: rows go straight to global memory
         static_for<A>([&](auto ic) {
             constexpr int i = decltype(ic)::value;
-            if (half >= 0 && agent_half<P>(i) != half) return;
             RowWriter o{a.obs[i] + wi * P::obs_dim(i)};
             P::template observe<i>(d, w, o);
         });
     }
 }
 
-#ifndef MPE_BOUND_THREADS
-#define MPE_BOUND_THREADS kMaxThreads   // register-budget experiments: -DMPE_BOUND_THREADS=128 lifts the cap from 128 to 255
-#endif
-#ifndef MPE_MIN_BLOCKS
-#define MPE_MIN_BLOCKS 1   // 512-thread bound x 1 block = a 128-register budget
-#endif
-
-// SPLIT (fused step only): TWO warps share a 32-world tile.  Both load the state and the actions; each evaluates half
-// of the contact forces (exchanged through shared memory, accumulated by both in the reference's order: bit-identical
-// state); warp 2k writes the new state and the observations of the first ceil(2A/3) agents, warp 2k+1 computes and
-// writes the rewards / dones / info and the remaining observations.  It doubles the warps in flight and nearly halves
-// each warp's instruction stream: batches too small to fill the machine with one lane per world (world_comm at 32 768
-// worlds = 1.7 warps per scheduler, ~2500 dependent instructions each) are bound by instruction latency, not by HBM.
+// __launch_bounds__(kMaxThreads, 1): 512 threads x 1 block = a 128-register budget.
 //
 // HOT (fused step only): the specialisation the launcher uses whenever it can -- whole 32-world tiles, 16-byte aligned
 // action rows, float action vectors without force_discrete_action, cp.async staging.  It contains none of the cold
-// alternatives (partial-tile scalar paths, TMA staging, integer decode, arg-max), i.e. about half the static code of
+// alternatives (partial-tile scalar paths, integer decode, arg-max), i.e. about half the static code of
 // the general kernel: with few resident warps per scheduler the step is bound by each warp's own instruction stream,
 // including instruction-fetch stalls across the skipped cold blocks.  Same arithmetic, same order: bit-identical.
 // A ragged tail and every other flag combination run on the general kernel.
@@ -320,21 +187,16 @@ __device__ __forceinline__ void write_observations(const StepArgs &a, const DevD
 // the tag family up to 6 agents, spread N=4) and only launched when the batch has more tiles than the 128-register
 // kernel keeps resident (> #SMs x 16 warps): there occupancy matters more, below it the register-rich version is
 // preferred.
-template <class P, int MODE, bool SPLIT = false, bool HOT = false, bool DENSE = false>
-__global__ void __launch_bounds__(DENSE ? 128 : MPE_BOUND_THREADS, DENSE ? 6 : MPE_MIN_BLOCKS) mpe_kernel(const __grid_constant__ StepArgs a) {
+template <class P, int MODE, bool HOT = false, bool DENSE = false>
+__global__ void __launch_bounds__(DENSE ? 128 : kMaxThreads, DENSE ? 6 : 1) mpe_kernel(const __grid_constant__ StepArgs a) {
     static_assert(!DENSE || HOT, "the low-register build exists for the HOT fused step only");
-    static_assert(!SPLIT || MODE == kFusedStep, "warp pairs exist for the fused step only");
-    static_assert(!HOT || (MODE == kFusedStep && !SPLIT && Shape<P>::all_act_dense()), "HOT = plain fused step, dense tiles");
-    static_assert(!SPLIT || pair_count<P>() * 64 <= Shape<P>::kWarpFloats - Shape<P>::obs_base(), "pair exchange must fit the obs tiles");
+    static_assert(!HOT || (MODE == kFusedStep && Shape<P>::all_act_dense()), "HOT = plain fused step, dense tiles");
     constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     extern __shared__ __align__(16) float smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int half = SPLIT ? (warp & 1) : 0;
     const int64_t n = a.n;
     const int64_t end = a.begin + a.count;
-    const int64_t tile = SPLIT ? static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 6) + (warp >> 1)
-                               : static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + warp;
-    const int64_t w0 = a.begin + tile * 32;
+    const int64_t w0 = a.begin + (static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + warp) * 32;
     // Programmatic dependent launch (MPE_B200_PDL, see launch()): the index arithmetic and the first touches of the
     // parameter block (constant-bank misses) run before the wait; no global memory is touched before the previous
     // grid has completed and flushed.  A warp that exits early counts as having released the dependent grid.
@@ -344,7 +206,6 @@ __global__ void __launch_bounds__(DENSE ? 128 : MPE_BOUND_THREADS, DENSE ? 6 : M
     const bool active = HOT ? true : (lane < rows);
     const int64_t wi = w0 + (active ? lane : 0);  // inactive lanes shadow row 0 and never store
     float *s_warp = smem + warp * Shape<P>::kWarpFloats;
-    uint64_t *bar = reinterpret_cast<uint64_t *>(s_warp);
     const DevDesc &d = a.d;
     {   // pull the parameter lines that the load phase needs into registers / the constant cache now
         uintptr_t touch = reinterpret_cast<uintptr_t>(a.pv) ^ reinterpret_cast<uintptr_t>(a.lm) ^
@@ -354,7 +215,7 @@ __global__ void __launch_bounds__(DENSE ? 128 : MPE_BOUND_THREADS, DENSE ? 6 : M
     }
     asm volatile("griddepcontrol.wait;" ::: "memory");
 
-    // ---- action tiles: asynchronous copies (cp.async, or TMA bulk) issued FIRST, so that they fly together
+    // ---- action tiles: asynchronous copies (cp.async) issued FIRST, so that they fly together
     //      with the state loads -------------------------------------------------------------------------
     bool bulk = false;
     if constexpr (HOT) {
@@ -373,7 +234,7 @@ __global__ void __launch_bounds__(DENSE ? 128 : MPE_BOUND_THREADS, DENSE ? 6 : M
         for (int i = 0; i < A; ++i) bits |= reinterpret_cast<uintptr_t>(a.act[i]);
         // warp-uniform; integer actions (discrete_action_input) are one or two words per world and need no tile
         bulk = (rows == 32) && ((bits & 15u) == 0) && !(a.flags & MPE_FLAG_DISCRETE_ACTION_INPUT);
-        if (bulk && (a.flags & kFlagCpAsync)) {
+        if (bulk) {
             // every lane copies 16-byte pieces of the (contiguous) tiles straight into shared memory
             static_for<A>([&](auto ic) {
                 constexpr int i = decltype(ic)::value;
@@ -384,15 +245,6 @@ __global__ void __launch_bounds__(DENSE ? 128 : MPE_BOUND_THREADS, DENSE ? 6 : M
                 for (int q0 = 0; q0 < kVec; q0 += 32)
                     if (q0 + 32 <= kVec || q0 + lane < kVec) cp_async16(sdst + 4 * (q0 + lane), g + 4 * (q0 + lane));
             });
-        } else if (bulk && lane == 0) {
-            // one UBLKCP per agent tile (32 rows x act_dim floats, contiguous in global memory)
-            mbar_init(bar, 1);
-            mbar_expect_tx(bar, Shape<P>::act_bytes_total());
-            static_for<A>([&](auto ic) {
-                constexpr int i = decltype(ic)::value;
-                constexpr int AD = P::act_dim(i);
-                bulk_g2s(s_warp + Shape<P>::act_off(i), a.act[i] + w0 * AD, 32 * AD * 4, bar);
-            });
         }
     }
 
@@ -401,12 +253,12 @@ __global__ void __launch_bounds__(DENSE ? 128 : MPE_BOUND_THREADS, DENSE ? 6 : M
     if constexpr (MODE != kSetAction) {
 #pragma unroll
         for (int i = 0; i < A; ++i) {
-            const float4 v = state_load(a.pv + i * n + wi);
+            const float4 v = a.pv[i * n + wi];
             w.px[i] = v.x; w.py[i] = v.y; w.vx[i] = v.z; w.vy[i] = v.w;
         }
 #pragma unroll
         for (int l = 0; l < L; ++l) {
-            const float2 v = state_load(a.lm + l * n + wi);
+            const float2 v = a.lm[l * n + wi];
             w.lx[l] = v.x; w.ly[l] = v.y;
         }
         if constexpr (MODE == kObserve && NC > 0) {
@@ -454,12 +306,9 @@ __global__ void __launch_bounds__(DENSE ? 128 : MPE_BOUND_THREADS, DENSE ? 6 : M
                 }
             });
         } else {
-        if (bulk && (a.flags & kFlagCpAsync)) {
+        if (bulk) {
             cp_async_wait_all();
             __syncwarp();
-        } else if (bulk) {
-            __syncwarp();
-            mbar_wait(bar, 0);
         } else {
             static_for<A>([&](auto ic) {
                 constexpr int i = decltype(ic)::value;
@@ -494,17 +343,10 @@ __global__ void __launch_bounds__(DENSE ? 128 : MPE_BOUND_THREADS, DENSE ? 6 : M
     if (a.flags & kFlagPdlAfterLoads) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     // ---- World.step (core.py:117-131) --------------------------------------------------------
     if constexpr (MODE == kFusedStep || MODE == kWorldStep) {
-        if constexpr (SPLIT) {
-            // exchange buffer = the observation-tile area of the pair's even warp (idle until the observations are
-            // written; the second barrier below keeps it intact until the partner has read every pair force)
-            float2 *ex = reinterpret_cast<float2 *>(smem + (warp & ~1) * Shape<P>::kWarpFloats + Shape<P>::obs_base());
-            physics_split<P>(d, w, ux, uy, half, ex, lane, 1 + (warp >> 1));
-        } else {
-            physics<P>(d, w, ux, uy);
-        }
+        physics<P>(d, w, ux, uy);
 #pragma unroll
         for (int q = 0; q < NC; ++q) w.c[q] = cact[q];  // update_agent_state (core.py:171-177)
-        if (active && half == 0) {
+        if (active) {
 #pragma unroll
             for (int i = 0; i < A; ++i)
                 if (P::movable(i)) a.pv[i * n + wi] = make_float4(w.px[i], w.py[i], w.vx[i], w.vy[i]);
@@ -518,20 +360,17 @@ __global__ void __launch_bounds__(DENSE ? 128 : MPE_BOUND_THREADS, DENSE ? 6 : M
     float rew[A];
     float info[(P::INFO > 0 ? P::INFO : 1) * A];
     P::prepare(d, w);   // per-world predicates shared by all agents' observations (world_comm: forest membership)
-    if (!SPLIT || half == 1) {   // warp pairs: only the warp that stores the rewards computes them
-        P::reward(d, w, rew, (P::INFO > 0 && a.info != nullptr) ? info : nullptr);
-        if (a.flags & MPE_FLAG_SHARED_REWARD) {                                  // :100-102 np.sum(reward_n)
-            float s = 0.0f;
+    P::reward(d, w, rew, (P::INFO > 0 && a.info != nullptr) ? info : nullptr);
+    if (a.flags & MPE_FLAG_SHARED_REWARD) {                                      // :100-102 np.sum(reward_n)
+        float s = 0.0f;
 #pragma unroll
-            for (int i = 0; i < A; ++i) s += rew[i];
+        for (int i = 0; i < A; ++i) s += rew[i];
 #pragma unroll
-            for (int i = 0; i < A; ++i) rew[i] = s;
-        }
+        for (int i = 0; i < A; ++i) rew[i] = s;
     }
-    if constexpr (SPLIT) pair_sync(1 + (warp >> 1));   // the partner has consumed the exchange buffer (= obs tiles of the even warp)
     if (!(a.flags & (kFlagPdlEarly | kFlagPdlAfterLoads | kFlagPdlAtExit | kFlagPdlAfterIssue))) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi, SPLIT ? half : -1);
-    if (active && (!SPLIT || half == 1)) {
+    write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi);
+    if (active) {
 #pragma unroll
         for (int i = 0; i < A; ++i) {
             a.rew[i * n + wi] = rew[i];
@@ -545,120 +384,6 @@ __global__ void __launch_bounds__(DENSE ? 128 : MPE_BOUND_THREADS, DENSE ? 6 : M
 }
 
 
-
-// ---- software-pipelined persistent fused step (MPE_B200_PIPE=1) ------------------------------------------------
-// A grid of (tiles / tiles-per-warp) warps; every warp walks its 32-world tiles with a two-deep pipeline: ALL inputs
-// of tile k+1 (action tiles, agent state, landmarks, goal indices) are fetched with cp.async into the second half of
-// the warp's staging while tile k is decoded, integrated, observed and streamed out.  Load, compute and store phases
-// of different tiles overlap inside one strictly ordered launch.  Same arithmetic functions as mpe_kernel: results
-// are bit-identical (tests/test_gpu_parity.py).  Full tiles only; the launcher sends a ragged tail to mpe_kernel.
-template <class P>
-__global__ void __launch_bounds__(MPE_BOUND_THREADS, MPE_MIN_BLOCKS) mpe_pipe_kernel(const __grid_constant__ StepArgs a) {
-    constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
-    using S = Shape<P>;
-    extern __shared__ __align__(16) float smem[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t n = a.n;
-    const int64_t n_tiles = a.count >> 5;
-    const int64_t nwarps = static_cast<int64_t>(gridDim.x) * (blockDim.x >> 5);
-    int64_t t = static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + warp;
-    float *s_warp = smem + warp * S::kPipeWarpFloats;
-    const DevDesc &d = a.d;
-    {
-        uintptr_t touch = reinterpret_cast<uintptr_t>(a.pv) ^ reinterpret_cast<uintptr_t>(a.lm) ^
-                          reinterpret_cast<uintptr_t>(a.obs[0]) ^ reinterpret_cast<uintptr_t>(a.rew) ^ a.flags ^
-                          __float_as_uint(d.dt) ^ __float_as_uint(d.a_size[0]);
-        asm volatile("" ::"l"(touch));
-    }
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    if (t >= n_tiles) return;
-
-    auto act_base = [&](int b) { return s_warp + b * S::kPipeAct1; };
-    auto state_base = [&](int b) { return s_warp + S::kPipeState0 + b * S::kStateFloats; };
-    auto prefetch = [&](int64_t tile, int b) {
-        const int64_t w0 = a.begin + tile * 32;
-        float *ab = act_base(b);
-        static_for<A>([&](auto ic) {
-            constexpr int i = decltype(ic)::value;
-            constexpr int AD = P::act_dim(i), kVec = 32 * AD / 4;
-            const float *g = a.act[i] + w0 * AD;
-            float *sdst = ab + S::act_off(i);
-#pragma unroll
-            for (int q0 = 0; q0 < kVec; q0 += 32)
-                if (q0 + 32 <= kVec || q0 + lane < kVec) cp_async16(sdst + 4 * (q0 + lane), g + 4 * (q0 + lane));
-        });
-        float *sb = state_base(b);
-#pragma unroll
-        for (int i = 0; i < A; ++i) cp_async16(sb + (i * 32 + lane) * 4, a.pv + i * n + w0 + lane);
-#pragma unroll
-        for (int l = 0; l < L; ++l) cp_async8(sb + A * 128 + (l * 32 + lane) * 2, a.lm + l * n + w0 + lane);
-#pragma unroll
-        for (int q = 0; q < P::G; ++q) cp_async4(sb + A * 128 + L * 64 + q * 32 + lane, a.goal + q * n + w0 + lane);
-    };
-
-    prefetch(t, 0);
-    cp_async_commit();
-    bool first = true;
-#pragma unroll 1
-    for (int b = 0; t < n_tiles; t += nwarps, b ^= 1) {
-        const int64_t w0 = a.begin + t * 32, wi = w0 + lane;
-        if (t + nwarps < n_tiles) prefetch(t + nwarps, b ^ 1);
-        cp_async_commit();
-        cp_async_wait_group<1>();
-        __syncwarp();
-        if (first && (a.flags & kFlagPdlAfterLoads)) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        first = false;
-        typename P::W w;
-        const float *sb = state_base(b);
-#pragma unroll
-        for (int i = 0; i < A; ++i) {
-            const float4 v = *reinterpret_cast<const float4 *>(sb + (i * 32 + lane) * 4);
-            w.px[i] = v.x; w.py[i] = v.y; w.vx[i] = v.z; w.vy[i] = v.w;
-        }
-#pragma unroll
-        for (int l = 0; l < L; ++l) {
-            const float2 v = *reinterpret_cast<const float2 *>(sb + A * 128 + (l * 32 + lane) * 2);
-            w.lx[l] = v.x; w.ly[l] = v.y;
-        }
-        if constexpr (P::G > 0) {
-#pragma unroll
-            for (int q = 0; q < P::G; ++q) w.g[q] = reinterpret_cast<const int *>(sb + A * 128 + L * 64)[q * 32 + lane];
-        }
-        float ux[A], uy[A];
-        float cact[NC > 0 ? NC : 1];
-        decode_rows<P>(act_base(b), lane, d, a.flags, ux, uy, cact);
-        physics<P>(d, w, ux, uy);
-#pragma unroll
-        for (int q = 0; q < NC; ++q) w.c[q] = cact[q];
-#pragma unroll
-        for (int i = 0; i < A; ++i)
-            if (P::movable(i)) a.pv[i * n + wi] = make_float4(w.px[i], w.py[i], w.vx[i], w.vy[i]);
-#pragma unroll
-        for (int q = 0; q < NC; ++q) a.comm[q * n + wi] = w.c[q];
-        float rew[A];
-        float info[(P::INFO > 0 ? P::INFO : 1) * A];
-        P::prepare(d, w);
-        P::reward(d, w, rew, (P::INFO > 0 && a.info != nullptr) ? info : nullptr);
-        if (a.flags & MPE_FLAG_SHARED_REWARD) {
-            float sum = 0.0f;
-#pragma unroll
-            for (int i = 0; i < A; ++i) sum += rew[i];
-#pragma unroll
-            for (int i = 0; i < A; ++i) rew[i] = sum;
-        }
-        write_observations<P>(a, d, w, s_warp, lane, 32, true, w0, wi, -1);
-#pragma unroll
-        for (int i = 0; i < A; ++i) {
-            a.rew[i * n + wi] = rew[i];
-            a.done[i * n + wi] = 0;
-        }
-        if (P::INFO > 0 && a.info != nullptr) {
-#pragma unroll
-            for (int q = 0; q < P::INFO * A; ++q) a.info[q * n + wi] = info[q];
-        }
-        __syncwarp();   // every lane is done with buffer b (inputs) and the obs tiles before they are reused
-    }
-}
 
 // ---- K-step open-loop rollout (SURVEY.md 8(f) rank 3: the persistent multi-step form) --------------------------
 // T consecutive MultiAgentEnv.step calls on pre-generated actions act[i] : [T][n_env][act_dim_i] in ONE launch: a
@@ -675,7 +400,7 @@ struct RolloutArgs {
 };
 
 template <class P>
-__global__ void __launch_bounds__(MPE_BOUND_THREADS, MPE_MIN_BLOCKS) mpe_rollout_kernel(const __grid_constant__ RolloutArgs ra) {
+__global__ void __launch_bounds__(kMaxThreads, 1) mpe_rollout_kernel(const __grid_constant__ RolloutArgs ra) {
     constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     const StepArgs &a = ra.s;
     extern __shared__ __align__(16) float smem[];
@@ -715,12 +440,12 @@ __global__ void __launch_bounds__(MPE_BOUND_THREADS, MPE_MIN_BLOCKS) mpe_rollout
     typename P::W w;
 #pragma unroll
     for (int i = 0; i < A; ++i) {
-        const float4 v = state_load(a.pv + i * n + wi);
+        const float4 v = a.pv[i * n + wi];
         w.px[i] = v.x; w.py[i] = v.y; w.vx[i] = v.z; w.vy[i] = v.w;
     }
 #pragma unroll
     for (int l = 0; l < L; ++l) {
-        const float2 v = state_load(a.lm + l * n + wi);
+        const float2 v = a.lm[l * n + wi];
         w.lx[l] = v.x; w.ly[l] = v.y;
     }
     if constexpr (NC > 0) {   // only matters for T == 0; every step overwrites it (update_agent_state)
@@ -774,7 +499,7 @@ __global__ void __launch_bounds__(MPE_BOUND_THREADS, MPE_MIN_BLOCKS) mpe_rollout
         for (int q = 0; q < NC; ++q) a.comm[q * n + wi] = w.c[q];
     }
     P::prepare(d, w);
-    write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi, -1);
+    write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi);
     if (active) {
 #pragma unroll
         for (int i = 0; i < A; ++i) {
@@ -921,12 +646,12 @@ __global__ void __launch_bounds__(128) mpe_policy_rollout_kernel(const __grid_co
     typename P::W w;
 #pragma unroll
     for (int i = 0; i < A; ++i) {
-        const float4 v = state_load(a.pv + i * n + wi);
+        const float4 v = a.pv[i * n + wi];
         w.px[i] = v.x; w.py[i] = v.y; w.vx[i] = v.z; w.vy[i] = v.w;
     }
 #pragma unroll
     for (int l = 0; l < L; ++l) {
-        const float2 v = state_load(a.lm + l * n + wi);
+        const float2 v = a.lm[l * n + wi];
         w.lx[l] = v.x; w.ly[l] = v.y;
     }
     if constexpr (P::G > 0) {
@@ -972,7 +697,7 @@ __global__ void __launch_bounds__(128) mpe_policy_rollout_kernel(const __grid_co
             if (P::movable(i)) a.pv[i * n + wi] = make_float4(w.px[i], w.py[i], w.vx[i], w.vy[i]);
     }
     P::prepare(d, w);
-    write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi, -1);
+    write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi);
     if (active) {
 #pragma unroll
         for (int i = 0; i < A; ++i) {
@@ -1083,7 +808,6 @@ struct MlpShape {
     static constexpr int kLogitPitch = max_nout() + 1;
     static constexpr int kLogitOff = obs_tile_floats();
     static constexpr int kWarpFloats = (kLogitOff + 32 * kLogitPitch + 3) & ~3;
-    static_assert(MPE_COMPACT_OBS, "write_observations must use one shared observation slot");
     static_assert(Shape<P>::kWarpFloats - Shape<P>::obs_base() <= kLogitOff, "final observations fit the tile");
 };
 
@@ -1326,12 +1050,12 @@ __global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_r
     typename P::W w;
 #pragma unroll
     for (int i = 0; i < A; ++i) {
-        const float4 v = state_load(a.pv + i * n + wi);
+        const float4 v = a.pv[i * n + wi];
         w.px[i] = v.x; w.py[i] = v.y; w.vx[i] = v.z; w.vy[i] = v.w;
     }
 #pragma unroll
     for (int l = 0; l < L; ++l) {
-        const float2 v = state_load(a.lm + l * n + wi);
+        const float2 v = a.lm[l * n + wi];
         w.lx[l] = v.x; w.ly[l] = v.y;
     }
     if constexpr (P::G > 0) {
@@ -1385,9 +1109,9 @@ __global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_r
     }
     P::prepare(d, w);
     __syncwarp();                  // every lane has read its logits before the tile is reused
-    // write_observations addresses the observation slot at Shape<P>::obs_off(i) == obs_base(): shift the base so that
-    // the slot is this warp's observation tile
-    write_observations<P>(a, d, w, s_warp - Shape<P>::obs_base(), lane, rows, active, w0, wi, -1);
+    // write_observations addresses the observation slot at obs_base(): shift the base so that the slot is this warp's
+    // observation tile
+    write_observations<P>(a, d, w, s_warp - Shape<P>::obs_base(), lane, rows, active, w0, wi);
     if (active) {
 #pragma unroll
         for (int i = 0; i < A; ++i) {
@@ -1596,9 +1320,6 @@ struct Program {
     int smem_bytes;  // dynamic shared memory per WARP
     KernelFn hot_fn;    // fused step specialised for whole tiles / float actions / cp.async staging (null: no such program)
     KernelFn hot_dense_fn;   // the same compiled for 80 registers (large batches of programs that fit without spilling)
-    KernelFn split_fn;  // fused step with a warp PAIR per 32-world tile (small batches of heavy scenarios)
-    KernelFn pipe_fn;   // software-pipelined persistent fused step (null unless every action tile is dense)
-    int pipe_smem;      // dynamic shared memory per WARP of the pipelined kernel
     void (*policy_fn[2])(PolicyArgs);  // K-step closed-loop rollout, hidden width 32 / 64 (null: not built for this program)
     int policy_weight_floats[2];
     void (*mlp_fn[2])(MlpPolicyArgs);  // the same with the two-hidden-layer actor on the tensor cores, H = 32 / 64
@@ -1606,8 +1327,6 @@ struct Program {
     int mlp_explore_stride;            // Philox blocks per (step, agent) of its exploration noise
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
     int rollout_smem;   // dynamic shared memory per WARP of the rollout kernel
-    KernelFn lanes_fn;  // lane-per-agent fused step (simple_spread only), else null
-    int lanes_smem, lanes_wpw;
     int A, L, NS, DIMC, INFO, G;
     int obs_dim[kMaxA], act_dim[kMaxA];
     int unread_state_floats;   // state floats per world that this scenario's step never needs (not compulsory traffic)
@@ -1622,16 +1341,8 @@ static Program make_program() {
     p.fn[kSetAction] = mpe_kernel<P, kSetAction>;
     p.fn[kWorldStep] = mpe_kernel<P, kWorldStep>;
     p.fn[kObserve] = mpe_kernel<P, kObserve>;
-    // the two restructurings that measurements rejected (warp pairs, software-pipelined persistent grid) stay available as
-    // opt-in, bit-identical alternatives for the BASELINE.json worlds only (compile time)
-    constexpr bool kAlternatives = PolicyBuilt<P>::value || std::is_same<P, Spread<6>>::value ||
-                                   std::is_same<P, WorldComm<4, 2, 1, 2>>::value;
-    if constexpr (kAlternatives && P::A >= 2 && pair_count<P>() * 64 <= Shape<P>::kWarpFloats - Shape<P>::obs_base())
-        p.split_fn = mpe_kernel<P, kFusedStep, true>;     // (the pair exchange must fit the observation tiles)
-    if constexpr (Shape<P>::all_act_dense()) p.hot_fn = mpe_kernel<P, kFusedStep, false, true>;
-    if constexpr (Shape<P>::all_act_dense() && P::kLowRegVariant) p.hot_dense_fn = mpe_kernel<P, kFusedStep, false, true, true>;
-    if constexpr (kAlternatives && Shape<P>::all_act_dense()) p.pipe_fn = mpe_pipe_kernel<P>;
-    p.pipe_smem = Shape<P>::kPipeWarpBytes;
+    if constexpr (Shape<P>::all_act_dense()) p.hot_fn = mpe_kernel<P, kFusedStep, true>;
+    if constexpr (Shape<P>::all_act_dense() && P::kLowRegVariant) p.hot_dense_fn = mpe_kernel<P, kFusedStep, true, true>;
     p.rollout_fn = mpe_rollout_kernel<P>;
     p.rollout_smem = Shape<P>::kRolloutWarpBytes;
     // the closed-loop rollout is built for the BASELINE.json scenarios whose agents all move and are silent
@@ -1673,21 +1384,12 @@ static Program make_generic_program() {
     return p;
 }
 
-template <int N>
-static Program make_spread_program() {
-    Program p = make_program<Spread<N>>();
-    p.lanes_fn = spread_lanes_kernel<N>;
-    p.lanes_smem = SpreadLanes<N>::kWarpBytes;
-    p.lanes_wpw = SpreadLanes<N>::WPW;
-    return p;
-}
-
 static const Program *programs(int *count) {
     static const Program table[] = {
         make_generic_program(),
         make_program<Simple<1, 1>>(),
-        make_spread_program<2>(), make_spread_program<3>(), make_spread_program<4>(),
-        make_spread_program<5>(), make_spread_program<6>(),
+        make_program<Spread<2>>(), make_program<Spread<3>>(), make_program<Spread<4>>(),
+        make_program<Spread<5>>(), make_program<Spread<6>>(),
         make_program<Tag<3, 1, 2>>(), make_program<Tag<1, 1, 2>>(), make_program<Tag<2, 1, 2>>(),
         make_program<Tag<4, 2, 2>>(), make_program<Tag<6, 2, 3>>(),
         make_program<WorldComm<4, 2, 1, 2>>(),
@@ -1782,16 +1484,11 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
             if (prog->fn[m] && prog->smem_bytes > 0)
                 CUDA_TRY(cudaFuncSetAttribute(prog->fn[m], cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               prog->smem_bytes * max_warps_per_block(prog->smem_bytes)));
-        if (prog->lanes_fn)
-            CUDA_TRY(cudaFuncSetAttribute(prog->lanes_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, prog->lanes_smem * 4));
         if (prog->hot_fn && prog->smem_bytes > 0)
             CUDA_TRY(cudaFuncSetAttribute(prog->hot_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->smem_bytes * max_warps_per_block(prog->smem_bytes)));
         if (prog->hot_dense_fn && prog->smem_bytes > 0)
             CUDA_TRY(cudaFuncSetAttribute(prog->hot_dense_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, prog->smem_bytes * 4));
-        if (prog->pipe_fn)
-            CUDA_TRY(cudaFuncSetAttribute(prog->pipe_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          prog->pipe_smem * max_warps_per_block(prog->pipe_smem)));
         for (int k = 0; k < 2; ++k)
             if (prog->policy_fn[k])
                 CUDA_TRY(cudaFuncSetAttribute(prog->policy_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1803,9 +1500,6 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
         if (prog->rollout_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->rollout_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->rollout_smem * max_warps_per_block(prog->rollout_smem)));
-        if (prog->split_fn && prog->smem_bytes > 0)
-            CUDA_TRY(cudaFuncSetAttribute(prog->split_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          prog->smem_bytes * max_warps_per_block(prog->smem_bytes)));
         CUDA_TRY(cudaSetDevice(prev));
     }
 
@@ -1901,7 +1595,31 @@ extern "C" int64_t mpe_bytes_per_env_step(mpe_handle h) {
     return 4 * f + p->A;
 }
 
-constexpr int64_t kLanesMaxWorlds = 0;  // the lane-per-agent kernel is opt-in only
+// One kernel launch on the handle's device, counted in mpe_kernel_launches.  `pdl` sets programmatic stream
+// serialization: the kernel may start while the previous one on the stream is finishing (the step kernels wait for it
+// with griddepcontrol.wait before touching global memory).
+static int launch_kernel(mpe_handle h, const void *fn, int64_t blocks, int threads, size_t smem, void *stream,
+                         void **params, bool pdl, const char *what) {
+    if (blocks > 0x7fffffffLL) return MPE_ERR_BAD_ARG;
+    int prev = 0;
+    CUDA_TRY(cudaGetDevice(&prev));
+    if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(static_cast<unsigned>(blocks));
+    cfg.blockDim = dim3(static_cast<unsigned>(threads));
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = static_cast<cudaStream_t>(stream);
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = pdl ? 1 : 0;
+    cudaError_t e = cudaLaunchKernelExC(&cfg, fn, params);
+    if (prev != h->device) cudaSetDevice(prev);
+    if (e != cudaSuccess) return cuda_fail(e, what);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    return MPE_OK;
+}
 
 // Programmatic dependent launch between consecutive step kernels.  MPE_B200_PDL: 0 = off, 1 = release the next grid
 // before our stores, 2 = at entry, 3 = once our inputs have arrived (DEFAULT), 4 = implicitly at exit, 5 = as soon as our
@@ -1917,137 +1635,35 @@ static int launch(mpe_handle h, int mode, StepArgs &args, void *stream, int64_t 
     args.n = h->n;
     args.begin = begin;
     args.count = count < 0 ? h->n - begin : count;
-    // simple_spread fused steps may run on the lane-per-agent kernel (mpe_spread_lanes.cuh): MPE_B200_SPREAD_LANES
-    // = 0 never, 1 always, unset: up to kLanesMaxWorlds worlds, where the lane-per-world kernel has too few warps
-    static const int lanes_env = [] { const char *e = getenv("MPE_B200_SPREAD_LANES"); return e ? atoi(e) : -1; }();
-    const bool lanes = mode == kFusedStep && h->prog->lanes_fn != nullptr &&
-                       (lanes_env == 1 || (lanes_env < 0 && args.count <= kLanesMaxWorlds));
-    if (lanes) {
-        const int64_t lw = (args.count + h->prog->lanes_wpw - 1) / h->prog->lanes_wpw;
-        constexpr int kLanesWpb = 4;
-        const int64_t lb = (lw + kLanesWpb - 1) / kLanesWpb;
-        int prev = 0;
-        CUDA_TRY(cudaGetDevice(&prev));
-        if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
-        void *params[] = {&args};
-        cudaError_t e = cudaLaunchKernel(reinterpret_cast<const void *>(h->prog->lanes_fn), dim3(static_cast<unsigned>(lb)),
-                                         dim3(32 * kLanesWpb), params, static_cast<size_t>(h->prog->lanes_smem) * kLanesWpb,
-                                         static_cast<cudaStream_t>(stream));
-        if (prev != h->device) cudaSetDevice(prev);
-        if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchKernel(spread_lanes)");
-        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
-        return MPE_OK;
-    }
     if (h->prog->scenario == MPE_SCN_CUSTOM) {   // generic program: one thread per world, no staging
         if (h->prog->fn[mode] == nullptr) return MPE_ERR_UNSUPPORTED;
-        int prev = 0;
-        CUDA_TRY(cudaGetDevice(&prev));
-        if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
         void *params[] = {&args};
-        cudaError_t e = cudaLaunchKernel(reinterpret_cast<const void *>(h->prog->fn[mode]),
-                                         dim3(static_cast<unsigned>((args.count + 127) / 128)), dim3(128), params, 0,
-                                         static_cast<cudaStream_t>(stream));
-        if (prev != h->device) cudaSetDevice(prev);
-        if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchKernel(generic)");
-        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
-        return MPE_OK;
+        return launch_kernel(h, reinterpret_cast<const void *>(h->prog->fn[mode]), (args.count + 127) / 128, 128, 0, stream,
+                             params, false, "cudaLaunchKernelExC(generic)");
     }
-    // Software-pipelined persistent kernel (mpe_pipe_kernel): MPE_B200_PIPE=1, MPE_B200_PIPE_TPW tiles per warp (default 2)
-    static const int pipe_env = [] { const char *e = getenv("MPE_B200_PIPE"); return e ? atoi(e) : 0; }();
-    static const int pipe_tpw = [] { const char *e = getenv("MPE_B200_PIPE_TPW"); int v = e ? atoi(e) : 2; return v < 1 ? 1 : v; }();
-    if (pipe_env == 1 && mode == kFusedStep && h->prog->pipe_fn != nullptr && args.count >= 32 &&
-        !(args.flags & MPE_FLAG_DISCRETE_ACTION_INPUT)) {
-        bool aligned = true;
-        for (int i = 0; i < h->prog->A; ++i)
-            aligned = aligned && ((reinterpret_cast<uintptr_t>(args.act[i]) + static_cast<uintptr_t>(begin) * h->prog->act_dim[i] * 4) & 15u) == 0;
-        if (aligned && (begin % 32) == 0 && (h->n % 4) == 0) {
-            const int64_t tiles = args.count / 32, tail = args.count - tiles * 32;
-            static const int pwpb_env = [] { const char *e = getenv("MPE_B200_WPB"); int v = e ? atoi(e) : 0; return (v >= 1 && v <= kMaxWarpsPerBlock) ? v : 0; }();
-            int pwpb = pwpb_env ? pwpb_env : 2;
-            if (pwpb > max_warps_per_block(h->prog->pipe_smem)) pwpb = max_warps_per_block(h->prog->pipe_smem);
-            const int64_t pwarps = (tiles + pipe_tpw - 1) / pipe_tpw;
-            const int64_t pblocks = (pwarps + pwpb - 1) / pwpb;
-            int prev = 0;
-            CUDA_TRY(cudaGetDevice(&prev));
-            if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
-            cudaLaunchConfig_t cfg{};
-            cfg.gridDim = dim3(static_cast<unsigned>(pblocks));
-            cfg.blockDim = dim3(32 * pwpb);
-            cfg.dynamicSmemBytes = static_cast<size_t>(h->prog->pipe_smem) * pwpb;
-            cfg.stream = static_cast<cudaStream_t>(stream);
-            cudaLaunchAttribute attr[1];
-            attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            attr[0].val.programmaticStreamSerializationAllowed = 1;
-            cfg.attrs = attr;
-            cfg.numAttrs = pdl_mode() ? 1 : 0;
-            StepArgs pa = args;
-            pa.count = tiles * 32;
-            if (pdl_mode() == 3) pa.flags |= kFlagPdlAfterLoads;
-            void *params[] = {&pa};
-            cudaError_t e = cudaLaunchKernelExC(&cfg, reinterpret_cast<const void *>(h->prog->pipe_fn), params);
-            if (prev != h->device) cudaSetDevice(prev);
-            if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchKernelExC(pipe)");
-            __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
-            if (tail == 0) return MPE_OK;
-            args.begin = begin + tiles * 32;      // the ragged tail goes through the regular kernel below
-            args.count = tail;
-        }
-    }
-    int64_t warps = (args.count + 31) / 32;
-    // Warp pairs (see mpe_kernel<..., SPLIT>): MPE_B200_SPLIT = 1 always, 2 = for small batches of >= 4-agent scenarios,
-    // unset / 0 never: the duplicated physics + reward usually cost more than the extra warps hide.  Kept as an opt-in,
-    // bit-identical alternative.
-    static const int split_env = [] { const char *e = getenv("MPE_B200_SPLIT"); return e ? atoi(e) : -1; }();
-    static const int64_t split_max_env = [] { const char *e = getenv("MPE_B200_SPLIT_MAX_WARPS"); return e ? atoll(e) : -1LL; }();
-    const int64_t split_max_warps = split_max_env >= 0 ? split_max_env : 10LL * h->sms;
-    const bool split = mode == kFusedStep && h->prog->split_fn != nullptr &&
-                       (split_env == 1 || (split_env == 2 && h->prog->A >= 4 && warps <= split_max_warps));
-    if (split) warps *= 2;
     static const int wpb_env = [] { const char *e = getenv("MPE_B200_WPB"); int v = e ? atoi(e) : 0; return (v >= 1 && v <= kMaxWarpsPerBlock) ? v : 0; }();
-    // action tiles: cp.async (LDGSTS) by default -- no barrier init / proxy fence in the prologue, unlike the TMA bulk
-    // copy + mbarrier; MPE_B200_ACT_STAGING=tma selects the TMA path
-    static const bool cpasync = [] { const char *e = getenv("MPE_B200_ACT_STAGING"); return !(e && e[0] == 't'); }();
     static const bool hot_env = [] { const char *e = getenv("MPE_B200_HOT"); return !(e && e[0] == '0'); }();   // 0 = general kernel only
-    int prev = 0;
-    CUDA_TRY(cudaGetDevice(&prev));
-    if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
     if (pdl_mode() == 2) args.flags |= kFlagPdlEarly;
     if (pdl_mode() == 3) args.flags |= kFlagPdlAfterLoads;
     if (pdl_mode() == 4) args.flags |= kFlagPdlAtExit;
     if (pdl_mode() == 5) args.flags |= kFlagPdlAfterIssue;
-    if (cpasync) args.flags |= kFlagCpAsync;
     // one grid of autonomous warps over [sa.begin, sa.begin + sa.count)
-    auto launch_grid = [&](KernelFn fn, StepArgs &sa, bool pairs, int max_wpb = kMaxWarpsPerBlock) -> int {
-        int64_t nw = (sa.count + 31) / 32;
-        if (pairs) nw *= 2;
+    auto launch_grid = [&](KernelFn fn, StepArgs &sa, int max_wpb = kMaxWarpsPerBlock) -> int {
+        const int64_t nw = (sa.count + 31) / 32;
         // Warps are autonomous, so the block size only sets scheduling granularity.  While every warp of the batch is
         // resident at once (<= 16 per SM) one warp per block balances the SMs best; mid-size batches use two, large
         // ones four.
         int wpb = wpb_env ? wpb_env : (nw <= 16LL * h->sms ? 1 : (nw <= 64LL * h->sms ? 2 : 4));
         if (wpb > max_warps_per_block(h->prog->smem_bytes)) wpb = max_warps_per_block(h->prog->smem_bytes);
         if (wpb > max_wpb) wpb = max_wpb;
-        if (pairs) wpb = (wpb < 2) ? 2 : (wpb & ~1);      // a pair lives in one block
-        const int64_t blocks = (nw + wpb - 1) / wpb;
-        if (blocks > 0x7fffffffLL) return MPE_ERR_BAD_ARG;
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(static_cast<unsigned>(blocks));
-        cfg.blockDim = dim3(32 * wpb);
-        cfg.dynamicSmemBytes = static_cast<size_t>(h->prog->smem_bytes) * wpb;
-        cfg.stream = static_cast<cudaStream_t>(stream);
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = pdl_mode() ? 1 : 0;
         void *params[] = {&sa};
-        cudaError_t e = cudaLaunchKernelExC(&cfg, reinterpret_cast<const void *>(fn), params);
-        if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchKernelExC");
-        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
-        return MPE_OK;
+        return launch_kernel(h, reinterpret_cast<const void *>(fn), (nw + wpb - 1) / wpb, 32 * wpb,
+                             static_cast<size_t>(h->prog->smem_bytes) * wpb, stream, params, pdl_mode() != 0,
+                             "cudaLaunchKernelExC(step)");
     };
     int rc = MPE_OK;
     // the specialised fused step (mpe_kernel<..., HOT>) takes every whole tile it is eligible for
-    bool hot = hot_env && cpasync && !split && mode == kFusedStep && h->prog->hot_fn != nullptr && args.count >= 32 &&
+    bool hot = hot_env && mode == kFusedStep && h->prog->hot_fn != nullptr && args.count >= 32 &&
                !(args.flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION));
     for (int i = 0; hot && i < h->prog->A; ++i)
         hot = ((reinterpret_cast<uintptr_t>(args.act[i]) + static_cast<uintptr_t>(args.begin) * h->prog->act_dim[i] * 4) & 15u) == 0;
@@ -2058,12 +1674,11 @@ static int launch(mpe_handle h, int mode, StepArgs &args, void *stream, int64_t 
         static const int dense_env = [] { const char *e = getenv("MPE_B200_DENSE"); return e ? atoi(e) : -1; }();   // 0 never, 1 always
         const bool dense = h->prog->hot_dense_fn != nullptr &&
                            (dense_env == 1 || (dense_env < 0 && ha.count / 32 > 16LL * h->sms));
-        rc = dense ? launch_grid(h->prog->hot_dense_fn, ha, false, 4) : launch_grid(h->prog->hot_fn, ha, false);
+        rc = dense ? launch_grid(h->prog->hot_dense_fn, ha, 4) : launch_grid(h->prog->hot_fn, ha);
         args.begin += ha.count;
         args.count -= ha.count;
     }
-    if (rc == MPE_OK && args.count > 0) rc = launch_grid(split ? h->prog->split_fn : h->prog->fn[mode], args, split);
-    if (prev != h->device) cudaSetDevice(prev);
+    if (rc == MPE_OK && args.count > 0) rc = launch_grid(h->prog->fn[mode], args);
     return rc;
 }
 
@@ -2187,19 +1802,9 @@ extern "C" int mpe_rollout(mpe_handle h, void *pv, const void *lm, float *comm, 
     const int64_t warps = (h->n + 31) / 32;
     int wpb = warps <= 4LL * h->sms ? 1 : (warps <= 64LL * h->sms ? 2 : 4);
     if (wpb > max_warps_per_block(h->prog->rollout_smem)) wpb = max_warps_per_block(h->prog->rollout_smem);
-    const int64_t blocks = (warps + wpb - 1) / wpb;
-    if (blocks > 0x7fffffffLL) return MPE_ERR_BAD_ARG;
-    int prev = 0;
-    CUDA_TRY(cudaGetDevice(&prev));
-    if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
     void *params[] = {&ra};
-    cudaError_t e = cudaLaunchKernel(reinterpret_cast<const void *>(h->prog->rollout_fn), dim3(static_cast<unsigned>(blocks)),
-                                     dim3(32 * wpb), params, static_cast<size_t>(h->prog->rollout_smem) * wpb,
-                                     static_cast<cudaStream_t>(stream));
-    if (prev != h->device) cudaSetDevice(prev);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchKernel(rollout)");
-    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
-    return MPE_OK;
+    return launch_kernel(h, reinterpret_cast<const void *>(h->prog->rollout_fn), (warps + wpb - 1) / wpb, 32 * wpb,
+                         static_cast<size_t>(h->prog->rollout_smem) * wpb, stream, params, false, "cudaLaunchKernelExC(rollout)");
 }
 
 extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
@@ -2236,19 +1841,10 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
     pa.rew_steps = rew_steps;
     const int64_t warps = (h->n + 31) / 32;
     const int wpb = warps <= 16LL * h->sms ? 1 : (warps <= 64LL * h->sms ? 2 : 4);
-    const int64_t blocks = (warps + wpb - 1) / wpb;
-    if (blocks > 0x7fffffffLL) return MPE_ERR_BAD_ARG;
-    int prev = 0;
-    CUDA_TRY(cudaGetDevice(&prev));
-    if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
     void *params[] = {&pa};
     const size_t smem = static_cast<size_t>(h->prog->policy_weight_floats[k]) * 4 + static_cast<size_t>(h->prog->smem_bytes) * wpb;
-    cudaError_t e = cudaLaunchKernel(reinterpret_cast<const void *>(h->prog->policy_fn[k]), dim3(static_cast<unsigned>(blocks)),
-                                     dim3(32 * wpb), params, smem, static_cast<cudaStream_t>(stream));
-    if (prev != h->device) cudaSetDevice(prev);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchKernel(rollout_policy)");
-    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
-    return MPE_OK;
+    return launch_kernel(h, reinterpret_cast<const void *>(h->prog->policy_fn[k]), (warps + wpb - 1) / wpb, 32 * wpb, smem,
+                         stream, params, false, "cudaLaunchKernelExC(rollout_policy)");
 }
 
 extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
@@ -2300,19 +1896,10 @@ extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, fl
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
     if (wpb > h->prog->mlp_warps[k]) wpb = h->prog->mlp_warps[k];
-    const int64_t blocks = (warps + wpb - 1) / wpb;
-    if (blocks > 0x7fffffffLL) return MPE_ERR_BAD_ARG;
-    int prev = 0;
-    CUDA_TRY(cudaGetDevice(&prev));
-    if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
     void *params[] = {&pa};
     const size_t smem = (static_cast<size_t>(h->prog->mlp_weight_floats[k]) + static_cast<size_t>(h->prog->mlp_warp_floats[k]) * wpb) * 4;
-    cudaError_t e = cudaLaunchKernel(reinterpret_cast<const void *>(h->prog->mlp_fn[k]), dim3(static_cast<unsigned>(blocks)),
-                                     dim3(static_cast<unsigned>(32 * wpb)), params, smem, static_cast<cudaStream_t>(stream));
-    if (prev != h->device) cudaSetDevice(prev);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchKernel(rollout_policy_mlp)");
-    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
-    return MPE_OK;
+    return launch_kernel(h, reinterpret_cast<const void *>(h->prog->mlp_fn[k]), (warps + wpb - 1) / wpb,
+                         static_cast<int>(32 * wpb), smem, stream, params, false, "cudaLaunchKernelExC(rollout_policy_mlp)");
 }
 
 // adjacent (dst, src, bytes) copies with equal small gaps on both sides are issued as one DMA

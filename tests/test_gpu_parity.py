@@ -314,45 +314,6 @@ def test_host_buffers_path_equals_device_path(n):
         assert not any(d.any() for d in db)
 
 
-_LANES_SCRIPT = r"""
-import sys, numpy as np, torch
-sys.path.insert(0, %(root)r); sys.path.insert(0, %(root)r + "/tests")
-from helpers import make_product_env
-out = {}
-for tag, n in (("simple_spread_n3", 5003), ("simple_spread_n6", 2049)):
-    env = make_product_env(tag, num_envs=n, seed=21)
-    env.reset()
-    g = torch.Generator(device="cuda").manual_seed(4)
-    for t in range(3):
-        acts = [torch.softmax(3 * torch.randn(n, 5, device="cuda", generator=g), 1) for _ in range(env.n)]
-        obs_n, rew_n, _, _ = env.step(acts)
-    out[tag + "_obs"] = torch.cat(obs_n, 1).cpu().numpy()
-    out[tag + "_rew"] = torch.stack(rew_n).cpu().numpy()
-    out[tag + "_pv"] = env.world.native.agent_pv.cpu().numpy()
-    out[tag + "_info"] = env._last_out.info.cpu().numpy()
-np.savez(sys.argv[1], **out)
-"""
-
-
-def test_lane_per_agent_spread_kernel_is_bit_identical(tmp_path):
-    """MPE_B200_SPREAD_LANES=1 routes simple_spread's fused step through the lane-per-agent kernel
-    (warp-shuffle exchange and min-reduction, csrc/mpe_spread_lanes.cuh); it must reproduce the default
-    lane-per-world kernel bit for bit, including partial warps (5003 and 2049 worlds)."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    res = {}
-    for mode in ("0", "1"):
-        path = str(tmp_path / ("lanes%s.npz" % mode))
-        env = dict(os.environ, MPE_B200_SPREAD_LANES=mode)
-        subprocess.run([sys.executable, "-c", _LANES_SCRIPT % {"root": root}, path], check=True, env=env, timeout=600)
-        res[mode] = dict(np.load(path))
-    assert set(res["0"]) == set(res["1"]) and len(res["0"]) == 8
-    for k in res["0"]:
-        assert np.array_equal(res["0"][k], res["1"][k]), k
-
-
 def test_step_async_matches_step_and_interleaves_two_envs():
     """step_async / step_wait == step, and two envs can be in flight at once (the use case: overlap the
     transfers of one batch with host work on another)"""
@@ -376,7 +337,7 @@ def test_step_async_matches_step_and_interleaves_two_envs():
         envs[0].step_wait()
 
 
-_SPLIT_SCRIPT = r"""
+_ALT_SCRIPT = r"""
 import sys, numpy as np, torch
 sys.path.insert(0, %(root)r); sys.path.insert(0, %(root)r + "/tests")
 from helpers import make_product_env
@@ -409,8 +370,6 @@ np.savez(sys.argv[1], **out)
 ALT_KERNELS = {
     "general_kernel_instead_of_hot": {"MPE_B200_HOT": "0"},     # the un-specialised fused step for every tile
     "low_register_build": {"MPE_B200_DENSE": "1"},                # the 80-register HOT variant (tag family, spread N=4)
-    "warp_pair_split": {"MPE_B200_SPLIT": "1"},
-    "software_pipelined_persistent": {"MPE_B200_PIPE": "1"},
     # the default kernels (HOT whole tiles, general-kernel tails) in 3- and 4-warp blocks instead of 1-warp blocks:
     # per-warp shared-memory offsets and partial last blocks
     "three_warp_blocks": {"MPE_B200_WPB": "3"},
@@ -422,10 +381,8 @@ ALT_KERNELS = {
 @pytest.mark.parametrize("variant", list(ALT_KERNELS))
 def test_alternative_step_kernels_are_bit_identical(tmp_path, variant):
     """The default fused step runs whole tiles on the HOT specialisation and ragged tails on the general kernel.
-    MPE_B200_HOT=0 runs everything on the general kernel; MPE_B200_SPLIT=1 uses a warp PAIR per 32-world tile (both
-    warps do the physics, each writes half of the outputs; the in-place state update is ordered by a pair barrier);
-    MPE_B200_PIPE=1 runs the software-pipelined persistent kernel (all inputs of the next tile prefetched with
-    cp.async).  Three consecutive steps of eight scenarios with ragged batch sizes must agree bit for bit."""
+    MPE_B200_HOT=0 runs everything on the general kernel.  Three consecutive steps of eight scenarios with ragged batch
+    sizes must agree bit for bit."""
     import os
     import subprocess
     import sys
@@ -434,11 +391,11 @@ def test_alternative_step_kernels_are_bit_identical(tmp_path, variant):
     for mode in ("0", "1"):
         path = str(tmp_path / ("alt%s.npz" % mode))
         env = dict(os.environ)
-        for k in ("MPE_B200_SPLIT", "MPE_B200_PIPE", "MPE_B200_HOT", "MPE_B200_DENSE", "MPE_B200_WPB"):
+        for k in ("MPE_B200_HOT", "MPE_B200_DENSE", "MPE_B200_WPB"):
             env.pop(k, None)
         if mode == "1":
             env.update(ALT_KERNELS[variant])
-        subprocess.run([sys.executable, "-c", _SPLIT_SCRIPT % {"root": root}, path], check=True, env=env, timeout=900)
+        subprocess.run([sys.executable, "-c", _ALT_SCRIPT % {"root": root}, path], check=True, env=env, timeout=900)
         res[mode] = dict(np.load(path))
     assert set(res["0"]) == set(res["1"]) and len(res["0"]) >= 40
     for k in res["0"]:

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Static view of every fused-step kernel in libmpe_b200.so (no GPU needed): registers / stack from
 `cuobjdump -res-usage`, instruction mix from `cuobjdump -sass`.  The counts are STATIC instructions of the whole
-kernel; every entity loop is unrolled, but the runtime-selected alternatives (cp.async vs TMA action staging, the
-partial-warp tail path with scalar loads / stores, exact-image vs padded tile streaming) are all in the binary, so a
+kernel; every entity loop is unrolled, but the runtime-selected alternatives (the partial-warp tail path with scalar
+loads / stores, exact-image vs padded tile streaming) are all in the binary, so a
 full warp executes roughly half of them (spread N=3: 664 executed per warp in ncu vs 1252 static).
 
     python tools/sass_stats.py > profiles/r1_static_resources.md
@@ -57,11 +57,10 @@ def main():
     rows = []
     for mangled, (reg, stack) in usage.items():
         nm = names[mangled]
-        m = re.match(r"void mpe::mpe_kernel<mpe::(.+), 0, (false|true), (false|true), (false|true)>\(", nm)
+        m = re.match(r"void mpe::mpe_kernel<mpe::(.+), 0, (false|true), (false|true)>\(", nm)
         if not m:
             continue
-        label = (m.group(1) + (" (warp pair)" if m.group(2) == "true" else "") + (" HOT" if m.group(3) == "true" else "")
-                 + (" 80-reg" if m.group(4) == "true" else ""))
+        label = m.group(1) + (" HOT" if m.group(2) == "true" else "") + (" 80-reg" if m.group(3) == "true" else "")
         c = mix.get(mangled, {})
         fp = sum(c[k] for k in ("FADD", "FMUL", "FFMA", "FSETP", "FSEL", "FMNMX", "FMNMX3"))
         rows.append((label, reg, stack, c["total"], fp, c["MUFU"], c["LDG"], c["LDGSTS"], c["LDS"], c["STS"], c["STG"],
@@ -69,7 +68,7 @@ def main():
     rows.sort(key=lambda r: r[3])
     print("# Static resources of the fused-step kernels (`tools/sass_stats.py`, sm_90a, %s)\n" % os.path.basename(LIB))
     print("`__launch_bounds__(512, 1)` caps registers at 128.  No kernel spills (STACK 0).  Columns are static SASS counts of "
-          "the whole kernel including the runtime-selected alternatives (TMA vs cp.async staging, partial-warp tail), NOPs excluded; `fp` = FADD+FMUL+FFMA+FSETP+FSEL+FMNMX, `branch` = BRA+BSSY+BSYNC.\n")
+          "the whole kernel including the runtime-selected alternatives (partial-warp tail), NOPs excluded; `fp` = FADD+FMUL+FFMA+FSETP+FSEL+FMNMX, `branch` = BRA+BSSY+BSYNC.\n")
     print("| program | regs | stack | instr | fp | MUFU | LDG | LDGSTS | LDS | STS | STG | branch | sync |")
     print("|---|---|---|---|---|---|---|---|---|---|---|---|---|")
     for r in rows:
