@@ -228,9 +228,10 @@ MPE_API int mpe_rollout_policy(mpe_handle h, void *agent_pv_dev, const void *lm_
  * Records (NULL: not written): act_record_n[i] float [n_steps][n_env][act_dim_i], the action applied (the sample when
  * exploring); obs_record_n[i] float [n_steps][n_env][obs_dim_i] (16-byte aligned), the observation agent i acted on at
  * step t; rew_steps_dev as in mpe_rollout_policy.  Feeding act_record_n to mpe_step reproduces state, comm state,
- * observations and rewards bit for bit.  Built for simple, simple_spread N = 3, simple_tag 3 + 1,
- * simple_speaker_listener, simple_reference, simple_crypto, simple_adversary (1 + 2 agents) and simple_push (1 + 1);
- * otherwise, or for another hidden width, MPE_ERR_UNSUPPORTED.  The scenario and hidden width are checked before any
+ * observations and rewards bit for bit.  Built for simple, simple_spread N = 2 to 6, simple_tag 3 + 1, 1 + 1, 2 + 1,
+ * 4 + 2 and 6 + 2 (3 landmarks), simple_speaker_listener, simple_reference, simple_crypto, simple_adversary (1 + 2 and
+ * 1 + 3 agents) and simple_push (1 + 1); otherwise (simple_world_comm), or for another hidden width,
+ * MPE_ERR_UNSUPPORTED.  The scenario and hidden width are checked before any
  * state, weight or output pointer: a call with those null returns MPE_ERR_UNSUPPORTED or MPE_ERR_BAD_ARG and runs
  * nothing. */
 MPE_API int mpe_rollout_policy_mlp(mpe_handle h, void *agent_pv_dev, const void *lm_p_dev, float *comm_dev,

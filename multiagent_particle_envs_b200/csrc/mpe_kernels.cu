@@ -726,6 +726,16 @@ template <> struct MlpBuilt<Reference> { static constexpr bool value = true; };
 template <> struct MlpBuilt<Crypto> { static constexpr bool value = true; };
 template <> struct MlpBuilt<Adversary<1, 2, 2>> { static constexpr bool value = true; };
 template <> struct MlpBuilt<Push<1, 1, 2>> { static constexpr bool value = true; };
+// ... and for the entity-count variants the scenario kwargs reach (movable, silent agents with 5-entry actions)
+template <> struct MlpBuilt<Spread<2>> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Spread<4>> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Spread<5>> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Spread<6>> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Tag<1, 1, 2>> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Tag<2, 1, 2>> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Tag<4, 2, 2>> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Tag<6, 2, 3>> { static constexpr bool value = true; };
+template <> struct MlpBuilt<Adversary<1, 3, 3>> { static constexpr bool value = true; };
 
 
 // ---- K-step closed-loop rollout with MADDPG's two-hidden-layer actor on the tensor cores ---------------------------
@@ -765,12 +775,6 @@ template <class P>
 __host__ __device__ constexpr int mlp_max_act_dim() { int m = 0; for (int i = 0; i < P::A; ++i) m = P::act_dim(i) > m ? P::act_dim(i) : m; return m; }
 template <class P>
 __host__ __device__ constexpr int mlp_explore_stride() { return mlp_max_act_dim<P>() <= 8 ? 2 : 4; }
-// Warps per block at most: one copy of the weights serves all of them, and with 45-90 KB of weights one block is what
-// fits an SM, so this is also the residency.  16 warps leave 128 registers per thread.  Two programs need more at
-// H = 64 and get 12-warp blocks and up to 168 registers instead: tag 3+1 (four agents' state next to the 64 registers
-// of h1) and simple_reference (two 8-column logit tiles and 20 comm floats next to h1; it spills at 128).
-template <class P, int H>
-__host__ __device__ constexpr int mlp_block_warps() { return (H == 64 && (P::A >= 4 || mlp_max_act_dim<P>() > 8)) ? 12 : 16; }
 
 struct MlpPolicyArgs {
     StepArgs s;
@@ -810,6 +814,39 @@ struct MlpShape {
     static constexpr int kWarpFloats = (kLogitOff + 32 * kLogitPitch + 3) & ~3;
     static_assert(Shape<P>::kWarpFloats - Shape<P>::obs_base() <= kLogitOff, "final observations fit the tile");
 };
+
+// Warps per block at most: one copy of the weights serves all of them, and with 6-212 KB of weights one block is what
+// fits an SM, so this is also the residency.  The smaller of two limits:
+//  - registers (MlpRegisterWarps): a block's warps share the four SM sub-partitions' 16 K registers each, so 16 warps
+//    leave 128 registers per thread, 9-12 warps 168 and 8 or fewer 255.  Blocks are 16 warps unless that spills
+//    (ptxas -v): then 12, or 8 where 168 spills too.  At H = 64 every program with four or more agents (their state
+//    next to the 64 registers of h1) and simple_reference (two 8-column logit tiles and 20 comm floats next to h1)
+//    take 12; the listed specialisations are the rest.
+//  - shared memory (mlp_smem_warps): the weights plus kWarpFloats per warp within the 227 KB a block may opt in to on
+//    H100.  Below the register limit only for tag 6+2 at H = 64 (212 KB of weights, 3 warps).
+template <class P, int H>
+struct MlpRegisterWarps { static constexpr int value = (H == 64 && (P::A >= 4 || mlp_max_act_dim<P>() > 8)) ? 12 : 16; };
+template <> struct MlpRegisterWarps<Spread<2>, 64> { static constexpr int value = 12; };       // 8 bytes of stack at 128
+template <> struct MlpRegisterWarps<Tag<1, 1, 2>, 64> { static constexpr int value = 12; };    // 8 at 128
+template <> struct MlpRegisterWarps<Tag<2, 1, 2>, 64> { static constexpr int value = 12; };    // 8 at 128
+template <> struct MlpRegisterWarps<Spread<6>, 64> { static constexpr int value = 8; };        // 16 at 168
+template <> struct MlpRegisterWarps<Spread<6>, 32> { static constexpr int value = 12; };       // 48 at 128
+template <> struct MlpRegisterWarps<Tag<4, 2, 2>, 32> { static constexpr int value = 12; };    // 16 at 128
+template <> struct MlpRegisterWarps<Tag<6, 2, 3>, 32> { static constexpr int value = 8; };     // 64 at 128, 8 at 168
+constexpr int kMlpSmemBytes = 232448;
+template <class P, int H>
+__host__ __device__ constexpr int mlp_smem_warps() {
+    return (kMlpSmemBytes / 4 - MlpShape<P, H>::kWeightFloats) / MlpShape<P, H>::kWarpFloats;
+}
+template <class P, int H>
+__host__ __device__ constexpr int mlp_block_warps() {
+    return MlpRegisterWarps<P, H>::value < mlp_smem_warps<P, H>() ? MlpRegisterWarps<P, H>::value : mlp_smem_warps<P, H>();
+}
+// the two programs whose weights fill most of the 227 KB
+static_assert(MlpShape<Spread<6>, 64>::kWeightFloats * 4 == 175296 && MlpShape<Spread<6>, 64>::kWarpFloats * 4 == 6016 &&
+              mlp_smem_warps<Spread<6>, 64>() == 9, "spread N=6, H = 64: 175 296 + 9 x 6016 = 229 440 B");
+static_assert(MlpShape<Tag<6, 2, 3>, 64>::kWeightFloats * 4 == 217344 && MlpShape<Tag<6, 2, 3>, 64>::kWarpFloats * 4 == 4992 &&
+              mlp_smem_warps<Tag<6, 2, 3>, 64>() == 3, "tag 6+2, H = 64: 217 344 + 3 x 4992 = 232 320 B");
 
 __device__ __forceinline__ uint32_t to_tf32(float x) {
     uint32_t r;
@@ -1018,6 +1055,8 @@ __global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_r
     static_assert(H == 32 || H == 64, "MLP policy rollout: hidden width 32 or 64");
     constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     using S = MlpShape<P, H>;
+    static_assert(mlp_block_warps<P, H>() >= 1 &&
+                  (S::kWeightFloats + mlp_block_warps<P, H>() * S::kWarpFloats) * 4 <= kMlpSmemBytes, "one block fits an SM");
     const StepArgs &a = pa.s;
     extern __shared__ __align__(16) float smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;

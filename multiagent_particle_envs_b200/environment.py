@@ -261,8 +261,9 @@ class MultiAgentEnv(_Env):
         by (explore_seed, self.explore_epoch, global world index, step, agent) and self.explore_epoch advances by one per
         exploring call.  record_observations=True returns extras["observations"], a list of [T, N, obs_dim_i] tensors:
         the observation agent i acted on at each step.  Both options need the two-hidden-layer actor.  Built for simple,
-        simple_spread N=3, simple_tag 3+1, simple_speaker_listener, simple_reference, simple_crypto, simple_adversary
-        (3 agents) and simple_push (2 agents); other programs raise MpeError.
+        simple_spread N=2 to 6, simple_tag 3+1, 1+1, 2+1, 4+2 and 6+2 (3 landmarks), simple_speaker_listener,
+        simple_reference, simple_crypto, simple_adversary (3 or 4 agents) and simple_push (2 agents); other programs
+        (simple_world_comm) raise MpeError.
 
         Returns (obs_n, reward_sum_n, done_n, info_n, extras) for the state after the last step; extras["actions"]
         (record_actions) is a list of [T, N, act_dim_i] tensors with the actions taken ([T, N, 5] for the one-hidden-layer

@@ -43,6 +43,8 @@ def card_info():
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scenario", default="simple_spread")
+    ap.add_argument("--scenario-kwargs", nargs="*", default=[], metavar="KEY=INT",
+                    help="scenario keyword arguments, e.g. num_agents=6 or num_adversaries=6 num_good_agents=2")
     ap.add_argument("--num-envs", type=int, default=65536)
     ap.add_argument("--steps", type=int, default=25)
     ap.add_argument("--hidden", type=int, default=64)
@@ -50,6 +52,10 @@ def main():
     ap.add_argument("--layers", type=int, choices=(2, 3), default=2, help="Linear layers of the actor")
     ap.add_argument("--explore", action="store_true", help="Gumbel-softmax exploration (--layers 3)")
     args = ap.parse_args()
+    try:
+        skw = {k: int(v) for k, v in (kv.split("=", 1) for kv in args.scenario_kwargs)}
+    except ValueError:
+        ap.error("--scenario-kwargs takes KEY=INT pairs")
     if args.explore and args.layers != 3:
         ap.error("--explore needs --layers 3")
     import torch
@@ -59,7 +65,7 @@ def main():
     from multiagent_particle_envs_b200.rollout import GraphedRollout
     dev = torch.device("cuda", 0)
     n, T, H = args.num_envs, args.steps, args.hidden
-    env = make_env(args.scenario, num_envs=n, device=dev)
+    env = make_env(args.scenario, num_envs=n, device=dev, **skw)
     env.reuse_buffers = True
     env.reset()
     nw = env.world.native
@@ -70,7 +76,7 @@ def main():
         mods = [torch.nn.Sequential(torch.nn.Linear(od, H), torch.nn.ReLU(), torch.nn.Linear(H, H), torch.nn.ReLU(),
                                     torch.nn.Linear(H, ad)).to(dev) for od, ad in zip(nw.obs_dims, nw.act_dims)]
     segs = sub_spaces(env.world) if args.layers == 3 else [[5]] * len(nw.obs_dims)
-    res = {"config": {"scenario": args.scenario, "n_env": n, "T": T, "hidden": H}}
+    res = {"config": {"scenario": args.scenario, "scenario_kwargs": skw, "n_env": n, "T": T, "hidden": H}}
     if args.layers == 3:
         res["config"].update(layers=3, explore=args.explore, torch_float32_matmul_precision=torch.get_float32_matmul_precision())
     kw = {"explore_seed": 1} if args.explore else {}
@@ -90,7 +96,7 @@ def main():
         flops = actor_flops_per_step(nw.obs_dims, nw.act_dims, H, n)
         res["in_kernel"].update(actor_flop_per_step=flops, actor_tflops=flops / sec / 1e12)
     # (b) torch actors + env.step in one CUDA graph
-    env2 = make_env(args.scenario, num_envs=n, device=dev)
+    env2 = make_env(args.scenario, num_envs=n, device=dev, **skw)
     env2.reset()
 
     def act(z, seg):   # one softmax per action sub-space
