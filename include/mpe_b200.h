@@ -243,6 +243,34 @@ MPE_API int mpe_rollout_policy_mlp(mpe_handle h, void *agent_pv_dev, const void 
                                    float *const *act_record_n, float *const *obs_record_n, uint8_t *done_dev,
                                    uint32_t flags, void *stream);
 
+/* n_episodes MADDPG episodes of episode_length steps each in ONE launch: mpe_rollout_policy_mlp with the reset between
+ * episodes inside the kernel.  Bit for bit the same as, for e = 0 .. n_episodes - 1, mpe_rollout_policy_mlp(n_steps =
+ * episode_length, explore_epoch + e) followed by mpe_reset(reset_seed, world_offset, reset_epoch + e) without a mask:
+ *  - exploration: episode e uses explore epoch explore_epoch + e and its step counter t restarts at 0, so an exploring
+ *    call with episode_length * A * S > 2^30 is refused with MPE_ERR_BAD_ARG before anything runs;
+ *  - reset: after the last step of episode e every world is redrawn as mpe_reset draws it with epoch reset_epoch + e
+ *    (agents, immovable ones included, at U(-1, 1)^2 and at rest, landmarks, comm 0, goals), so lm_p_dev and goal_dev are
+ *    written;
+ *  - records span all n_episodes * episode_length steps, at global step e * episode_length + t: rew_steps_dev
+ *    [T][A][n_env], act_record_n[i] [T][n_env][act_dim_i], obs_record_n[i] [T][n_env][obs_dim_i];
+ *  - final_obs_record_n (NULL, or one 16-byte aligned pointer for every agent): [n_episodes][n_env][obs_dim_i], the
+ *    observation after the last step of episode e, before its reset (MADDPG's new_obs of the terminal transition);
+ *  - ep_rew_dev [n_episodes][A][n_env]: each episode's per-agent rewards summed in step order;
+ *  - obs_n_dev: the observations of the state after the last reset; done_dev: all 0.
+ * The state arrays end as the last reset left them.  episode_length and n_episodes must be >= 1 with a product below
+ * 2^31 (else MPE_ERR_BAD_ARG).  Built for the programs of mpe_rollout_policy_mlp; the scenario and hidden width are
+ * checked before any pointer, as there. */
+MPE_API int mpe_rollout_policy_mlp_episodes(mpe_handle h, void *agent_pv_dev, void *lm_p_dev, float *comm_dev,
+                                            int32_t *goal_dev, const float *const *w1_n, const float *const *b1_n,
+                                            const float *const *w2_n, const float *const *b2_n, const float *const *w3_n,
+                                            const float *const *b3_n, int32_t hidden, int32_t episode_length,
+                                            int32_t n_episodes, int32_t explore, uint64_t explore_seed,
+                                            uint64_t explore_epoch, uint64_t reset_seed, uint64_t reset_epoch,
+                                            uint64_t world_offset, float *const *obs_n_dev, float *ep_rew_dev,
+                                            float *rew_steps_dev, float *const *act_record_n, float *const *obs_record_n,
+                                            float *const *final_obs_record_n, uint8_t *done_dev, uint32_t flags,
+                                            void *stream);
+
 /* Same step for a caller that holds HOST buffers (what the reference's callers hold):
  * act_n_host[i] -> (async H2D into act_n_dev[i]) -> mpe_step -> (async D2H) obs_n_host[i],
  * rew_host, done_host, all ordered on `stream`.  Host buffers should be pinned for the copies

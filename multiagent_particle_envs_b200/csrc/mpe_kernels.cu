@@ -737,6 +737,46 @@ template <> struct MlpBuilt<Tag<4, 2, 2>> { static constexpr bool value = true; 
 template <> struct MlpBuilt<Tag<6, 2, 3>> { static constexpr bool value = true; };
 template <> struct MlpBuilt<Adversary<1, 3, 3>> { static constexpr bool value = true; };
 
+// ---- initial conditions of one world (e.g. simple_spread.py:31-45, simple_tag.py:45-53) -----------------------------
+// Agents ~ U(-1, 1)^2 at rest (immovable ones too), landmarks ~ U(-landmark_range, landmark_range)^2, comm 0, goal g =
+// word g of Philox block 0x80000000 mod goal_mod.  One Philox4x32-10 block = 4 x 32 bits = two entities' (x, y), entities
+// in the order agents then landmarks; key = seed, counter = (global world index lo, hi, low 32 bits of epoch, block).
+// The one definition of a reset: reset_kernel writes the draw to the state arrays, the episode form of the MLP rollout
+// to the world's registers, through `out` (agent(i, x, y), landmark(l, x, y), comm(q), goal(g, v)).
+__host__ __device__ constexpr float reset_landmark_range(int scenario) {   // simple_tag.py:53, simple_world_comm.py:105-113
+    return (scenario == MPE_SCN_TAG || scenario == MPE_SCN_WORLD_COMM) ? 0.9f : 1.0f;
+}
+template <class Out>
+__device__ __forceinline__ void draw_initial_state(int A, int L, int NC, int G, uint64_t seed, uint64_t gw, uint64_t epoch,
+                                                   float landmark_range, uint32_t goal_mod, Out &out) {
+    const uint2 key = make_uint2(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+    const int E = A + L;
+#pragma unroll
+    for (int e = 0; e < E; e += 2) {
+        const uint4 r = philox4x32_10(make_uint4(static_cast<uint32_t>(gw), static_cast<uint32_t>(gw >> 32),
+                                                 static_cast<uint32_t>(epoch), static_cast<uint32_t>(e >> 1)), key);
+        const uint32_t bits[4] = {r.x, r.y, r.z, r.w};
+        for (int k = 0; k < 2 && e + k < E; ++k) {
+            const int ent = e + k;
+            if (ent < A) {
+                out.agent(ent, uniform_from_bits(bits[2 * k], -1.0f, 1.0f), uniform_from_bits(bits[2 * k + 1], -1.0f, 1.0f));
+            } else {
+                out.landmark(ent - A, uniform_from_bits(bits[2 * k], -landmark_range, landmark_range),
+                             uniform_from_bits(bits[2 * k + 1], -landmark_range, landmark_range));
+            }
+        }
+    }
+#pragma unroll
+    for (int q = 0; q < NC; ++q) out.comm(q);
+    if (G > 0) {
+        const uint4 r = philox4x32_10(make_uint4(static_cast<uint32_t>(gw), static_cast<uint32_t>(gw >> 32),
+                                                 static_cast<uint32_t>(epoch), 0x80000000u), key);
+        const uint32_t bits[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+        for (int g = 0; g < G && g < 4; ++g) out.goal(g, static_cast<int32_t>(bits[g] % goal_mod));
+    }
+}
+
 
 // ---- K-step closed-loop rollout with MADDPG's two-hidden-layer actor on the tensor cores ---------------------------
 // The persistent structure of mpe_policy_rollout_kernel (state in registers for all T steps, nothing read from HBM per
@@ -790,6 +830,20 @@ struct MlpPolicyArgs {
 };
 static_assert(sizeof(MlpPolicyArgs) <= 4096, "kernel parameter space");
 
+// Episode form (mpe_policy_mlp_episode_kernel): `episodes` episodes of p.T steps in one launch.  After the last step of
+// episode e the world is redrawn as reset_kernel draws it with (reset_seed, global world index, reset_epoch + e); the
+// exploration of episode e uses epoch p.epoch + e and restarts its step counter at 0.  Records are indexed by the
+// global step e * p.T + t, and p.s.rew receives the per-episode returns [episodes][A][n].
+struct MlpEpisodeArgs {
+    MlpPolicyArgs p;
+    float2 *lm;                     // p.s.lm and p.s.goal, writable: every episode end redraws them
+    int32_t *goal;
+    int32_t episodes;
+    uint64_t reset_seed, reset_epoch;
+    float *final_obs[kMaxA];        // [episodes][n][obs_dim_i] per agent, or null: the observation after the last step
+};
+static_assert(sizeof(MlpEpisodeArgs) <= 4096, "kernel parameter space");
+
 template <class P, int H>
 struct MlpShape {
     static constexpr int NT = H / 8;                                   // n-tiles of a hidden layer (= its k-tiles)
@@ -838,9 +892,19 @@ template <class P, int H>
 __host__ __device__ constexpr int mlp_smem_warps() {
     return (kMlpSmemBytes / 4 - MlpShape<P, H>::kWeightFloats) / MlpShape<P, H>::kWarpFloats;
 }
+// The episode form (the reset draw and the episode-end stores next to the step's state): the rollout kernel's block,
+// smaller where ptxas -v shows a spill there
 template <class P, int H>
+struct MlpEpisodeRegisterWarps : MlpRegisterWarps<P, H> {};
+template <> struct MlpEpisodeRegisterWarps<Spread<3>, 64> { static constexpr int value = 12; };          // 8 bytes of stack at 128
+template <> struct MlpEpisodeRegisterWarps<SpeakerListener, 64> { static constexpr int value = 12; };    // 8 at 128
+template <> struct MlpEpisodeRegisterWarps<Adversary<1, 2, 2>, 64> { static constexpr int value = 12; }; // 16 at 128
+template <> struct MlpEpisodeRegisterWarps<Reference, 64> { static constexpr int value = 8; };           // 8 at 168
+template <> struct MlpEpisodeRegisterWarps<Tag<4, 2, 2>, 64> { static constexpr int value = 8; };        // 8 at 168
+template <class P, int H, bool EPISODES = false>
 __host__ __device__ constexpr int mlp_block_warps() {
-    return MlpRegisterWarps<P, H>::value < mlp_smem_warps<P, H>() ? MlpRegisterWarps<P, H>::value : mlp_smem_warps<P, H>();
+    constexpr int r = EPISODES ? MlpEpisodeRegisterWarps<P, H>::value : MlpRegisterWarps<P, H>::value;
+    return r < mlp_smem_warps<P, H>() ? r : mlp_smem_warps<P, H>();
 }
 // the two programs whose weights fill most of the 227 KB
 static_assert(MlpShape<Spread<6>, 64>::kWeightFloats * 4 == 175296 && MlpShape<Spread<6>, 64>::kWarpFloats * 4 == 6016 &&
@@ -900,11 +964,12 @@ __device__ __forceinline__ void softmax_segment(const float (&z)[N], float (&pr)
 
 // one agent of the tensor-core actor for the warp's 32 worlds: observation -> tile -> 3 GEMMs -> this lane's logits ->
 // (Gumbel-)softmax per sub-space -> decoded (u.x, u.y), and a speaker's utterance into cact[I * dim_c ...].  Called by
-// all 32 lanes (mma.sync is warp-collective).
-template <class P, int H, int I>
+// all 32 lanes (mma.sync is warp-collective).  t indexes the records.  The exploration noise is keyed by (pa.epoch, t),
+// and in the episode form (EPISODES) by (epoch, step) = (pa.epoch + e, t - e * T) in episode e.
+template <class P, int H, int I, bool EPISODES = false>
 __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typename P::W &w, const float *__restrict__ Wsm,
                                             float *s_warp, int lane, int t, int rows, bool active, int64_t w0, int64_t wi,
-                                            float *cact) {
+                                            float *cact, int step = 0, uint64_t epoch = 0) {
     using S = MlpShape<P, H>;
     constexpr int OD = P::obs_dim(I), KT1 = S::kt1(I), NT = S::NT, PITCH = ObsTile<OD>::kPitch;
     constexpr int AD = P::act_dim(I), NO = S::nout(I) / 8;
@@ -1013,12 +1078,14 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
     if (pa.explore) {                                      // Gumbel-softmax sample (see the definition above)
         const uint64_t gw = pa.world_offset + static_cast<uint64_t>(wi);
         const uint2 key = make_uint2(static_cast<uint32_t>(pa.seed), static_cast<uint32_t>(pa.seed >> 32));
-        const uint32_t c3 = kExploreTag | (static_cast<uint32_t>(t * P::A + I) * static_cast<uint32_t>(mlp_explore_stride<P>()));
+        const uint32_t c3 = kExploreTag | (static_cast<uint32_t>((EPISODES ? step : t) * P::A + I) *
+                                           static_cast<uint32_t>(mlp_explore_stride<P>()));
         uint32_t bits[(AD + 3) / 4 * 4];
 #pragma unroll
         for (int b = 0; b < (AD + 3) / 4; ++b) {
             const uint4 r = philox4x32_10(make_uint4(static_cast<uint32_t>(gw), static_cast<uint32_t>(gw >> 32),
-                                                     static_cast<uint32_t>(pa.epoch), c3 | static_cast<uint32_t>(b)), key);
+                                                     static_cast<uint32_t>(EPISODES ? epoch : pa.epoch),
+                                                     c3 | static_cast<uint32_t>(b)), key);
             bits[4 * b] = r.x; bits[4 * b + 1] = r.y; bits[4 * b + 2] = r.z; bits[4 * b + 3] = r.w;
         }
 #pragma unroll
@@ -1050,13 +1117,15 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
     }
 }
 
-template <class P, int H>
-__global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_rollout_kernel(const __grid_constant__ MlpPolicyArgs pa) {
+// the body of both forms; ea is null in the single-episode form (EPISODES = false)
+template <class P, int H, bool EPISODES>
+__device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEpisodeArgs *ea) {
     static_assert(H == 32 || H == 64, "MLP policy rollout: hidden width 32 or 64");
     constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     using S = MlpShape<P, H>;
-    static_assert(mlp_block_warps<P, H>() >= 1 &&
-                  (S::kWeightFloats + mlp_block_warps<P, H>() * S::kWarpFloats) * 4 <= kMlpSmemBytes, "one block fits an SM");
+    static_assert(mlp_block_warps<P, H, EPISODES>() >= 1 &&
+                  (S::kWeightFloats + mlp_block_warps<P, H, EPISODES>() * S::kWarpFloats) * 4 <= kMlpSmemBytes,
+                  "one block fits an SM");
     const StepArgs &a = pa.s;
     extern __shared__ __align__(16) float smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1107,42 +1176,89 @@ __global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_r
     }
 
     float rsum[A];
-#pragma unroll
-    for (int i = 0; i < A; ++i) rsum[i] = 0.0f;
 #pragma unroll 1
-    for (int t = 0; t < pa.T; ++t) {
-        float ux[A], uy[A];
-        float cact[NC > 0 ? NC : 1];
-        P::prepare(d, w);
-        static_for<A>([&](auto ic) {
-            constexpr int i = decltype(ic)::value;
-            const float2 u = mlp_agent<P, H, i>(pa, w, smem + S::agent_off(i), s_warp, lane, t, rows, active, w0, wi, cact);
-            ux[i] = u.x;
-            uy[i] = u.y;
-        });
-        physics<P>(d, w, ux, uy);
+    for (int e = 0; e < (EPISODES ? ea->episodes : 1); ++e) {   // the single-episode form runs one
 #pragma unroll
-        for (int q = 0; q < NC; ++q) w.c[q] = cact[q];      // update_agent_state (core.py:171-177), as the fused step
-        float rew[A];
-        P::reward(d, w, rew, nullptr);
-        if (a.flags & MPE_FLAG_SHARED_REWARD) {
-            float sum = 0.0f;
+        for (int i = 0; i < A; ++i) rsum[i] = 0.0f;
+#pragma unroll 1
+        for (int t = 0; t < pa.T; ++t) {
+            const int tg = EPISODES ? e * pa.T + t : t;         // the records' step
+            float ux[A], uy[A];
+            float cact[NC > 0 ? NC : 1];
+            P::prepare(d, w);
+            static_for<A>([&](auto ic) {
+                constexpr int i = decltype(ic)::value;
+                const float2 u = mlp_agent<P, H, i, EPISODES>(pa, w, smem + S::agent_off(i), s_warp, lane, tg, rows, active,
+                                                              w0, wi, cact, t, pa.epoch + e);
+                ux[i] = u.x;
+                uy[i] = u.y;
+            });
+            physics<P>(d, w, ux, uy);
 #pragma unroll
-            for (int i = 0; i < A; ++i) sum += rew[i];
+            for (int q = 0; q < NC; ++q) w.c[q] = cact[q];      // update_agent_state (core.py:171-177), as the fused step
+            float rew[A];
+            P::reward(d, w, rew, nullptr);
+            if (a.flags & MPE_FLAG_SHARED_REWARD) {
+                float sum = 0.0f;
 #pragma unroll
-            for (int i = 0; i < A; ++i) rew[i] = sum;
+                for (int i = 0; i < A; ++i) sum += rew[i];
+#pragma unroll
+                for (int i = 0; i < A; ++i) rew[i] = sum;
+            }
+#pragma unroll
+            for (int i = 0; i < A; ++i) rsum[i] = __fadd_rn(rsum[i], rew[i]);
+            if (pa.rew_steps != nullptr && active) {
+#pragma unroll
+                for (int i = 0; i < A; ++i) pa.rew_steps[(static_cast<int64_t>(tg) * A + i) * n + wi] = rew[i];
+            }
         }
+        if constexpr (EPISODES) {                          // episode end: returns, final observations, reset
+            if (active) {
 #pragma unroll
-        for (int i = 0; i < A; ++i) rsum[i] = __fadd_rn(rsum[i], rew[i]);
-        if (pa.rew_steps != nullptr && active) {
+                for (int i = 0; i < A; ++i) a.rew[(static_cast<int64_t>(e) * A + i) * n + wi] = rsum[i];
+            }
+            if (ea->final_obs[0] != nullptr) {                 // all agents or none (checked by the launcher)
+                P::prepare(d, w);
+                __syncwarp();                                  // every lane has read its logits before the tile is reused
+                static_for<A>([&](auto ic) {
+                    constexpr int i = decltype(ic)::value;
+                    constexpr int OD = P::obs_dim(i);
+                    {
+                        TileWriter<OD> o(s_warp, lane);
+                        P::template observe<i>(d, w, o);
+                    }
+                    __syncwarp();
+                    float *g = ea->final_obs[i] + (static_cast<int64_t>(e) * n + w0) * OD;
+                    if (rows == 32 && (reinterpret_cast<uintptr_t>(g) & 15u) == 0) {
+                        obs_tile_store<OD>(g, s_warp, lane);
+                    } else if (active) {
 #pragma unroll
-            for (int i = 0; i < A; ++i) pa.rew_steps[(static_cast<int64_t>(t) * A + i) * n + wi] = rew[i];
+                        for (int k = 0; k < OD; ++k) g[lane * OD + k] = s_warp[lane * ObsTile<OD>::kPitch + k];
+                    }
+                    __syncwarp();
+                });
+            }
+            struct ToRegs {
+                typename P::W &w;
+                __device__ void agent(int i, float x, float y) const { w.px[i] = x; w.py[i] = y; w.vx[i] = 0.0f; w.vy[i] = 0.0f; }
+                __device__ void landmark(int l, float x, float y) const { w.lx[l] = x; w.ly[l] = y; }
+                __device__ void comm(int q) const { w.c[q] = 0.0f; }
+                __device__ void goal(int g, int32_t v) const { w.g[g] = v; }
+            } out{w};
+            draw_initial_state(A, L, NC, P::G, ea->reset_seed, pa.world_offset + static_cast<uint64_t>(wi), ea->reset_epoch + e,
+                               reset_landmark_range(P::kScenario), L > 0 ? L : 1, out);
         }
     }
     if (active) {
 #pragma unroll
-        for (int i = 0; i < A; ++i)
-            if (P::movable(i)) a.pv[i * n + wi] = make_float4(w.px[i], w.py[i], w.vx[i], w.vy[i]);
+        for (int i = 0; i < A; ++i)                        // the reset moves immovable agents too
+            if (EPISODES || P::movable(i)) a.pv[i * n + wi] = make_float4(w.px[i], w.py[i], w.vx[i], w.vy[i]);
+        if constexpr (EPISODES) {
+#pragma unroll
+            for (int l = 0; l < L; ++l) ea->lm[l * n + wi] = make_float2(w.lx[l], w.ly[l]);
+#pragma unroll
+            for (int q = 0; q < P::G; ++q) ea->goal[q * n + wi] = w.g[q];
+        }
 #pragma unroll
         for (int q = 0; q < NC; ++q) a.comm[q * n + wi] = w.c[q];
     }
@@ -1154,10 +1270,21 @@ __global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_r
     if (active) {
 #pragma unroll
         for (int i = 0; i < A; ++i) {
-            a.rew[i * n + wi] = rsum[i];
+            if constexpr (!EPISODES) a.rew[i * n + wi] = rsum[i];
             a.done[i * n + wi] = 0;
         }
     }
+}
+
+template <class P, int H>
+__global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_rollout_kernel(const __grid_constant__ MlpPolicyArgs pa) {
+    mlp_rollout<P, H, false>(pa, nullptr);
+}
+
+template <class P, int H>
+__global__ void __launch_bounds__(mlp_block_warps<P, H, true>() * 32)
+    mpe_policy_mlp_episode_kernel(const __grid_constant__ MlpEpisodeArgs ea) {
+    mlp_rollout<P, H, true>(ea.p, &ea);
 }
 
 // ---- generic program for user scenarios (MPE_SCN_CUSTOM) ------------------------------------------
@@ -1288,43 +1415,24 @@ struct ResetArgs {
     const uint8_t *mask;
     uint64_t seed, world_offset, epoch;
     const unsigned long long *epoch_dev;   // when non-null the epoch is read from device memory
-    float agent_range, landmark_range[kMaxL];
-    int goal_mod[4];
+    float landmark_range;
+    uint32_t goal_mod;
 };
 
 __global__ void __launch_bounds__(256) reset_kernel(const __grid_constant__ ResetArgs a) {
     const int64_t w = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (w >= a.n) return;
     if (a.mask != nullptr && a.mask[w] == 0) return;
-    const uint64_t epoch = a.epoch_dev ? *a.epoch_dev : a.epoch;
-    const uint64_t gw = a.world_offset + static_cast<uint64_t>(w);
-    const uint2 key = make_uint2(static_cast<uint32_t>(a.seed), static_cast<uint32_t>(a.seed >> 32));
-    // one Philox block = 4 x 32 bits = two entities' (x, y); counter = (world lo, world hi, epoch, block)
-    const int E = a.A + a.L;
-    for (int e = 0; e < E; e += 2) {
-        const uint4 r = philox4x32_10(make_uint4(static_cast<uint32_t>(gw), static_cast<uint32_t>(gw >> 32),
-                                                 static_cast<uint32_t>(epoch), static_cast<uint32_t>(e >> 1)), key);
-        const uint32_t bits[4] = {r.x, r.y, r.z, r.w};
-        for (int k = 0; k < 2 && e + k < E; ++k) {
-            const int ent = e + k;
-            if (ent < a.A) {
-                const float x = uniform_from_bits(bits[2 * k], -a.agent_range, a.agent_range);
-                const float y = uniform_from_bits(bits[2 * k + 1], -a.agent_range, a.agent_range);
-                a.pv[ent * a.n + w] = make_float4(x, y, 0.0f, 0.0f);
-            } else {
-                const float rg = a.landmark_range[ent - a.A];
-                a.lm[(ent - a.A) * a.n + w] = make_float2(uniform_from_bits(bits[2 * k], -rg, rg),
-                                                           uniform_from_bits(bits[2 * k + 1], -rg, rg));
-            }
-        }
-    }
-    for (int q = 0; q < a.NC; ++q) a.comm[q * a.n + w] = 0.0f;
-    if (a.G > 0) {
-        const uint4 r = philox4x32_10(make_uint4(static_cast<uint32_t>(gw), static_cast<uint32_t>(gw >> 32),
-                                                 static_cast<uint32_t>(epoch), 0x80000000u), key);
-        const uint32_t bits[4] = {r.x, r.y, r.z, r.w};
-        for (int g = 0; g < a.G && g < 4; ++g) a.goal[g * a.n + w] = static_cast<int32_t>(bits[g] % static_cast<uint32_t>(a.goal_mod[g]));
-    }
+    struct ToState {
+        const ResetArgs &a;
+        int64_t w;
+        __device__ void agent(int i, float x, float y) const { a.pv[i * a.n + w] = make_float4(x, y, 0.0f, 0.0f); }
+        __device__ void landmark(int l, float x, float y) const { a.lm[l * a.n + w] = make_float2(x, y); }
+        __device__ void comm(int q) const { a.comm[q * a.n + w] = 0.0f; }
+        __device__ void goal(int g, int32_t v) const { a.goal[g * a.n + w] = v; }
+    } out{a, w};
+    draw_initial_state(a.A, a.L, a.NC, a.G, a.seed, a.world_offset + static_cast<uint64_t>(w),
+                       a.epoch_dev ? *a.epoch_dev : a.epoch, a.landmark_range, a.goal_mod, out);
 }
 
 __global__ void bump_epoch_kernel(unsigned long long *epoch) { *epoch += 1ull; }
@@ -1363,6 +1471,8 @@ struct Program {
     int policy_weight_floats[2];
     void (*mlp_fn[2])(MlpPolicyArgs);  // the same with the two-hidden-layer actor on the tensor cores, H = 32 / 64
     int mlp_weight_floats[2], mlp_warp_floats[2], mlp_warps[2];
+    void (*mlp_episode_fn[2])(MlpEpisodeArgs);   // its episode form (in-kernel reset between episodes)
+    int mlp_episode_warps[2];
     int mlp_explore_stride;            // Philox blocks per (step, agent) of its exploration noise
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
     int rollout_smem;   // dynamic shared memory per WARP of the rollout kernel
@@ -1400,6 +1510,10 @@ static Program make_program() {
         p.mlp_warp_floats[1] = MlpShape<P, 64>::kWarpFloats;
         p.mlp_warps[0] = mlp_block_warps<P, 32>();
         p.mlp_warps[1] = mlp_block_warps<P, 64>();
+        p.mlp_episode_fn[0] = mpe_policy_mlp_episode_kernel<P, 32>;
+        p.mlp_episode_fn[1] = mpe_policy_mlp_episode_kernel<P, 64>;
+        p.mlp_episode_warps[0] = mlp_block_warps<P, 32, true>();
+        p.mlp_episode_warps[1] = mlp_block_warps<P, 64, true>();
         p.mlp_explore_stride = mlp_explore_stride<P>();
     }
     p.smem_bytes = Shape<P>::kWarpBytes;  // per warp
@@ -1536,6 +1650,10 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
             if (prog->mlp_fn[k])
                 CUDA_TRY(cudaFuncSetAttribute(prog->mlp_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp_warps[k]) * 4));
+        for (int k = 0; k < 2; ++k)
+            if (prog->mlp_episode_fn[k])
+                CUDA_TRY(cudaFuncSetAttribute(prog->mlp_episode_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp_episode_warps[k]) * 4));
         if (prog->rollout_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->rollout_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->rollout_smem * max_warps_per_block(prog->rollout_smem)));
@@ -1941,6 +2059,75 @@ extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, fl
                          static_cast<int>(32 * wpb), smem, stream, params, false, "cudaLaunchKernelExC(rollout_policy_mlp)");
 }
 
+extern "C" int mpe_rollout_policy_mlp_episodes(mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal,
+                                               const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
+                                               const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
+                                               int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
+                                               uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed,
+                                               uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew,
+                                               float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
+                                               float *const *final_obs_record_n, uint8_t *done, uint32_t flags, void *stream) {
+    if (!h) return MPE_ERR_BAD_ARG;
+    if (h->device < 0) return MPE_ERR_NO_DEVICE;
+    const int k = hidden == 32 ? 0 : (hidden == 64 ? 1 : -1);
+    if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || h->prog->mlp_episode_fn[k] == nullptr) return MPE_ERR_UNSUPPORTED;
+    if (flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
+    // records are indexed by the global step e * episode_length + t, an int
+    if (episode_length < 1 || n_episodes < 1 || static_cast<int64_t>(episode_length) * n_episodes > 0x7fffffffLL)
+        return MPE_ERR_BAD_ARG;
+    // the Philox counter word holds (t * A + i) * S + b below the tag bit; t restarts at 0 every episode
+    if (explore && static_cast<int64_t>(episode_length) * h->prog->A * h->prog->mlp_explore_stride > static_cast<int64_t>(kExploreTag))
+        return MPE_ERR_BAD_ARG;
+    if (!w1_n || !b1_n || !w2_n || !b2_n || !w3_n || !b3_n) return MPE_ERR_BAD_ARG;
+    if (rew_steps != nullptr && !ok4(rew_steps)) return MPE_ERR_BAD_ARG;
+    NvtxRange range("mpe_rollout_policy_mlp_episodes");
+    MlpEpisodeArgs ea{};
+    MlpPolicyArgs &pa = ea.p;
+    StepArgs &a = pa.s;
+    int r = fill_state(h, a, pv, lm, comm, goal);
+    if (r) return r;
+    r = fill_outputs(h, a, obs_n, ep_rew, done, nullptr);
+    if (r) return r;
+    for (int i = 0; i < h->prog->A; ++i) {
+        if (!ok4(w1_n[i]) || !ok4(b1_n[i]) || !ok4(w2_n[i]) || !ok4(b2_n[i]) || !ok4(w3_n[i]) || !ok4(b3_n[i]))
+            return MPE_ERR_BAD_ARG;
+        pa.w1[i] = w1_n[i]; pa.b1[i] = b1_n[i]; pa.w2[i] = w2_n[i]; pa.b2[i] = b2_n[i]; pa.w3[i] = w3_n[i]; pa.b3[i] = b3_n[i];
+        pa.act_rec[i] = act_record_n ? act_record_n[i] : nullptr;
+        if (pa.act_rec[i] != nullptr && !ok4(pa.act_rec[i])) return MPE_ERR_BAD_ARG;
+        pa.obs_rec[i] = obs_record_n ? obs_record_n[i] : nullptr;
+        if (pa.obs_rec[i] != nullptr && !ok16(pa.obs_rec[i])) return MPE_ERR_BAD_ARG;   // 16-byte tile stores
+        ea.final_obs[i] = final_obs_record_n ? final_obs_record_n[i] : nullptr;
+        if (final_obs_record_n != nullptr && !ok16(ea.final_obs[i])) return MPE_ERR_BAD_ARG;   // every agent's, or none
+    }
+    a.info = nullptr;
+    a.flags = flags;
+    a.d = h->dev;
+    a.n = h->n;
+    a.begin = 0;
+    a.count = h->n;
+    pa.T = episode_length;
+    pa.explore = explore ? 1 : 0;
+    pa.seed = explore_seed;
+    pa.epoch = explore_epoch;
+    pa.world_offset = world_offset;
+    pa.rew_steps = rew_steps;
+    ea.lm = static_cast<float2 *>(lm);
+    ea.goal = goal;
+    ea.episodes = n_episodes;
+    ea.reset_seed = reset_seed;
+    ea.reset_epoch = reset_epoch;
+    // the launch geometry of mpe_rollout_policy_mlp with the episode form's block cap
+    const int64_t warps = (h->n + 31) / 32;
+    int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
+    if (wpb < 1) wpb = 1;
+    if (wpb > h->prog->mlp_episode_warps[k]) wpb = h->prog->mlp_episode_warps[k];
+    void *params[] = {&ea};
+    const size_t smem = (static_cast<size_t>(h->prog->mlp_weight_floats[k]) + static_cast<size_t>(h->prog->mlp_warp_floats[k]) * wpb) * 4;
+    return launch_kernel(h, reinterpret_cast<const void *>(h->prog->mlp_episode_fn[k]), (warps + wpb - 1) / wpb,
+                         static_cast<int>(32 * wpb), smem, stream, params, false,
+                         "cudaLaunchKernelExC(rollout_policy_mlp_episodes)");
+}
+
 // adjacent (dst, src, bytes) copies with equal small gaps on both sides are issued as one DMA
 struct CopySeg { char *dst; const char *src; size_t bytes; };
 static int issue_copies(CopySeg *seg, int n, cudaMemcpyKind kind, cudaStream_t s, const char *what, bool coalesce) {
@@ -2090,11 +2277,8 @@ static int reset_impl(mpe_handle h, void *pv, void *lm, float *comm, int32_t *go
     a.n = h->n; a.A = p->A; a.L = p->L; a.NC = p->NS * p->DIMC; a.G = p->G;
     a.pv = static_cast<float4 *>(pv); a.lm = static_cast<float2 *>(lm); a.comm = comm; a.goal = goal; a.mask = mask;
     a.seed = seed; a.world_offset = world_offset; a.epoch = epoch; a.epoch_dev = epoch_dev;
-    a.agent_range = 1.0f;  // every scenario: agents ~ U(-1, +1)^2
-    // landmarks: U(-1,+1) (simple.py:37, simple_spread.py:44) or U(-0.9,+0.9) (simple_tag.py:53, simple_world_comm.py:105-113)
-    const bool narrow = (p->scenario == MPE_SCN_TAG || p->scenario == MPE_SCN_WORLD_COMM);
-    for (int l = 0; l < kMaxL; ++l) a.landmark_range[l] = narrow ? 0.9f : 1.0f;
-    for (int g = 0; g < 4; ++g) a.goal_mod[g] = p->L > 0 ? p->L : 1;
+    a.landmark_range = reset_landmark_range(p->scenario);
+    a.goal_mod = p->L > 0 ? p->L : 1;
     int prev = 0;
     CUDA_TRY(cudaGetDevice(&prev));
     if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));

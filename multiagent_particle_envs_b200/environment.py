@@ -244,7 +244,7 @@ class MultiAgentEnv(_Env):
         return obs_n, reward_n, done_n, info_n
 
     def rollout_policy(self, policies, n_steps, record_actions=False, per_step_rewards=False, record_observations=False,
-                       explore_seed=None):
+                       explore_seed=None, episode_length=None):
         """T closed-loop steps in ONE kernel launch with the actors inside the kernel.
 
         One hidden layer (mpe_rollout_policy, fp32): agent i acts with softmax(W2_i relu(W1_i obs_i + b1_i) + b2_i).
@@ -269,7 +269,17 @@ class MultiAgentEnv(_Env):
         (record_actions) is a list of [T, N, act_dim_i] tensors with the actions taken ([T, N, 5] for the one-hidden-layer
         actor), extras["rewards"] (per_step_rewards) a [T, n, N] tensor.  World state lives in registers for all T steps.
         Batched CUDA mode.  The one-hidden-layer actor needs a scenario whose agents all move and are silent and whose
-        program was built with that kernel (simple, simple_spread N=3, simple_tag 3+1) -- anything else raises."""
+        program was built with that kernel (simple, simple_spread N=3, simple_tag 3+1) -- anything else raises.
+
+        episode_length=L (two-hidden-layer actor only) collects E = n_steps / L whole MADDPG episodes in the one launch,
+        resetting every world inside the kernel after each episode.  Bit for bit the same as E calls
+        rollout_policy(policies, L, ...) each followed by env.reset(): episode e explores with epoch explore_epoch + e
+        (its step counter restarts at 0; explore_epoch advances by E when exploring), and the reset after it draws what
+        that reset() would draw (the world's reset epoch advances by E).  Records span all n_steps steps (global step
+        e * L + t).  reward_sum_n[i] is [E, N], the return of every episode; obs_n holds the observations of the freshly
+        reset state, done_n is all False, and with record_observations extras["final_observations"] is a list of
+        [E, N, obs_dim_i] tensors: the observation after the last step of each episode, before its reset (the next
+        observation of the terminal transition).  n_steps must be a positive multiple of L (else ValueError)."""
         import torch
         world = self.world
         if not world.batched:
@@ -278,9 +288,16 @@ class MultiAgentEnv(_Env):
             raise NotImplementedError("rollout_policy: compiled scenarios with plain action vectors only")
         if len(policies) != self.n:
             raise ValueError("expected %d policies, got %d" % (self.n, len(policies)))
+        if episode_length is not None and (int(episode_length) < 1 or int(n_steps) < int(episode_length)
+                                           or int(n_steps) % int(episode_length) != 0):
+            raise ValueError("rollout_policy: n_steps (%d) must be a positive multiple of episode_length (%d)"
+                             % (int(n_steps), int(episode_length)))
         if any(_has_two_hidden_layers(p) for p in policies):
             return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
-                                            explore_seed)
+                                            explore_seed, episode_length)
+        if episode_length is not None:
+            raise NotImplementedError("rollout_policy: episode_length needs the two-hidden-layer actor "
+                                      "(Linear -> ReLU -> Linear -> ReLU -> Linear)")
         if record_observations or explore_seed is not None:
             raise NotImplementedError("rollout_policy: observation records and exploration need the two-hidden-layer "
                                       "actor (Linear -> ReLU -> Linear -> ReLU -> Linear)")
@@ -316,7 +333,8 @@ class MultiAgentEnv(_Env):
         info_n = {'n': [{} for _ in range(self.n)]}
         return list(out.obs), list(out.rew_list), list(out.done_list), info_n, {"actions": actions, "rewards": rew_steps}
 
-    def _rollout_policy_mlp(self, policies, n_steps, record_actions, per_step_rewards, record_observations, explore_seed):
+    def _rollout_policy_mlp(self, policies, n_steps, record_actions, per_step_rewards, record_observations, explore_seed,
+                            episode_length=None):
         import torch
         world = self.world
         nw = world.bind()
@@ -331,17 +349,30 @@ class MultiAgentEnv(_Env):
         actions = [torch.empty((T, N, ad), **dev) for ad in nw.act_dims] if record_actions else None
         observations = [torch.empty((T, N, od), **dev) for od in nw.obs_dims] if record_observations else None
         seed = None if explore_seed is None else int(explore_seed) & 0xFFFFFFFFFFFFFFFF
-        nw.rollout_policy_mlp(w_ptrs, hidden, T, out, self._flags(), rew_steps,
-                              _lib.ptr_array([a.data_ptr() for a in actions]) if actions is not None else None,
-                              _lib.ptr_array([o.data_ptr() for o in observations]) if observations is not None else None,
-                              explore_seed=seed, explore_epoch=self.explore_epoch)
+        act_ptrs = _lib.ptr_array([a.data_ptr() for a in actions]) if actions is not None else None
+        obs_ptrs = _lib.ptr_array([o.data_ptr() for o in observations]) if observations is not None else None
+        extras = {"actions": actions, "rewards": rew_steps, "observations": observations}
+        if episode_length is None:
+            E = 1
+            nw.rollout_policy_mlp(w_ptrs, hidden, T, out, self._flags(), rew_steps, act_ptrs, obs_ptrs,
+                                  explore_seed=seed, explore_epoch=self.explore_epoch)
+            reward_n = list(out.rew_list)
+        else:
+            L = int(episode_length)
+            E = T // L
+            ep_rew = torch.empty((E, self.n, N), **dev)
+            final = [torch.empty((E, N, od), **dev) for od in nw.obs_dims] if record_observations else None
+            nw.rollout_policy_mlp_episodes(w_ptrs, hidden, L, E, out, ep_rew, self._flags(), rew_steps, act_ptrs, obs_ptrs,
+                                           _lib.ptr_array([o.data_ptr() for o in final]) if final is not None else None,
+                                           explore_seed=seed, explore_epoch=self.explore_epoch)
+            reward_n = list(ep_rew.unbind(1))
+            extras["final_observations"] = final
         if seed is not None:
-            self.explore_epoch += 1
+            self.explore_epoch += E
         self._last_out = out
         world._obs_valid = False
         info_n = {'n': [{} for _ in range(self.n)]}
-        return list(out.obs), list(out.rew_list), list(out.done_list), info_n, \
-            {"actions": actions, "rewards": rew_steps, "observations": observations}
+        return list(out.obs), reward_n, list(out.done_list), info_n, extras
 
     # ---- user scenarios: native _set_action + World.step, callbacks in the user's torch code -------
     def _step_custom(self, action_n, nw, flags):
