@@ -271,6 +271,43 @@ MPE_API int mpe_rollout_policy_mlp_episodes(mpe_handle h, void *agent_pv_dev, vo
                                             float *const *final_obs_record_n, uint8_t *done_dev, uint32_t flags,
                                             void *stream);
 
+/* Policy-gradient (PPO / A2C) experience with the same actor: mpe_rollout_policy_mlp and mpe_rollout_policy_mlp_episodes
+ * with categorical actions.  The logits z are those of the default form (same TF32 GEMMs); then, per action sub-space in
+ * action-vector order (5 movement logits if movable, then dim_c utterance logits if not silent):
+ *  - explore != 0: k = argmax_c (z_c - log(-log u_c)) with the u of the default form's exploration (same Philox counters,
+ *    stride S, epochs, episode step restart), so k is the arg-max of the Gumbel-softmax sample that form would take;
+ *    explore == 0: k = argmax_c z_c.  Ties go to the lowest index.
+ *  - the action applied is the one-hot vector of k, concatenated over sub-spaces, through the same _set_action arithmetic
+ *    as any float action vector: bit for bit what mpe_step does with that one-hot vector.  A speaker's utterance becomes
+ *    a one-hot comm state after the physics.
+ *  - its log-probability is the sum over sub-spaces, in order, of (z_k - m) - logf(sum_c expf(z_c - m)), m the maximum
+ *    of the unperturbed segment, the sum in index order with round-to-nearest adds: Categorical(logits=z).log_prob(k) on
+ *    the logits the kernel acted with.
+ * k is the POSITION IN THE LOGIT SEGMENT (the one-hot convention, environment.py:173-175), NOT the discrete_action_input
+ * code (environment.py:164-167): movement index 1 is +x here, -x there.  Replay the indices as one-hot float vectors.
+ * Records (NULL: not written): act_index_record_n[i] int32 [n_steps][n_env][n_sub_i] (n_sub_i = 1 or 2 sub-spaces,
+ * movement first), logp_steps_dev float [n_steps][A][n_env] (the layout of rew_steps_dev); everything else, the refusals
+ * (scenario and hidden width before any pointer, the exploration counter limit) and the programs built are those of the
+ * default form. */
+MPE_API int mpe_rollout_policy_mlp_categorical(mpe_handle h, void *agent_pv_dev, const void *lm_p_dev, float *comm_dev,
+                                               const int32_t *goal_dev, const float *const *w1_n,
+                                               const float *const *b1_n, const float *const *w2_n,
+                                               const float *const *b2_n, const float *const *w3_n,
+                                               const float *const *b3_n, int32_t hidden, int32_t n_steps, int32_t explore,
+                                               uint64_t explore_seed, uint64_t explore_epoch, uint64_t world_offset,
+                                               float *const *obs_n_dev, float *rew_sum_dev, float *rew_steps_dev,
+                                               float *logp_steps_dev, int32_t *const *act_index_record_n,
+                                               float *const *obs_record_n, uint8_t *done_dev, uint32_t flags,
+                                               void *stream);
+MPE_API int mpe_rollout_policy_mlp_categorical_episodes(
+    mpe_handle h, void *agent_pv_dev, void *lm_p_dev, float *comm_dev, int32_t *goal_dev, const float *const *w1_n,
+    const float *const *b1_n, const float *const *w2_n, const float *const *b2_n, const float *const *w3_n,
+    const float *const *b3_n, int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
+    uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset,
+    float *const *obs_n_dev, float *ep_rew_dev, float *rew_steps_dev, float *logp_steps_dev,
+    int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n, uint8_t *done_dev,
+    uint32_t flags, void *stream);
+
 /* Same step for a caller that holds HOST buffers (what the reference's callers hold):
  * act_n_host[i] -> (async H2D into act_n_dev[i]) -> mpe_step -> (async D2H) obs_n_host[i],
  * rew_host, done_host, all ordered on `stream`.  Host buffers should be pinned for the copies

@@ -93,6 +93,15 @@ _SIGNATURES = {
                                                        ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_uint64,
                                                        ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64,
                                                        _PP, _P, _P, _PP, _PP, _PP, _P, ctypes.c_uint32, _P]),
+    "mpe_rollout_policy_mlp_categorical": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _PP, _PP, _PP, ctypes.c_int32,
+                                                          ctypes.c_int32, ctypes.c_int32, ctypes.c_uint64, ctypes.c_uint64,
+                                                          ctypes.c_uint64, _PP, _P, _P, _P, _PP, _PP, _P, ctypes.c_uint32,
+                                                          _P]),
+    "mpe_rollout_policy_mlp_categorical_episodes": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _PP, _PP, _PP,
+                                                                   ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                                                   ctypes.c_int32, ctypes.c_uint64, ctypes.c_uint64,
+                                                                   ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, _PP,
+                                                                   _P, _P, _P, _PP, _PP, _PP, _P, ctypes.c_uint32, _P]),
     "mpe_step_host": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _P, _P, _P, _PP, _P, _P, _P,
                                      ctypes.c_uint32, _P]),
     "mpe_strerror": (ctypes.c_char_p, [ctypes.c_int]),

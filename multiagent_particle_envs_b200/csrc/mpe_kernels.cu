@@ -844,6 +844,27 @@ struct MlpEpisodeArgs {
 };
 static_assert(sizeof(MlpEpisodeArgs) <= 4096, "kernel parameter space");
 
+// Categorical form (CATEGORICAL): the policy-gradient action.  Per sub-space the agent applies the one-hot vector of
+// k = argmax_c (z_c - log(-log u_c)) when exploring (the same u as the Gumbel-softmax sample), k = argmax_c z_c when not,
+// the lowest index winning ties; k is the position in the logit segment (the one-hot convention, environment.py:173-175),
+// not the discrete_action_input code.  The log-probability of the agent's action is the sum over its sub-spaces, in
+// order, of log_softmax(z)[k] = (z_k - m) - log(sum_c exp(z_c - m)), m the maximum of the unperturbed segment.  The
+// records live next to, not inside, MlpPolicyArgs / MlpEpisodeArgs so that the default kernels' parameters keep their
+// layout; p.act_rec is null in this form.
+struct MlpCategoricalRecords {
+    int32_t *index[kMaxA];          // [T][n][n_sub_i] per agent, or null: k of each sub-space, movement first
+    float *logp;                    // [T][A][n] or null: the log-probability of the action applied
+};
+struct MlpCategoricalArgs {
+    MlpPolicyArgs p;
+    MlpCategoricalRecords c;
+};
+struct MlpCategoricalEpisodeArgs {
+    MlpEpisodeArgs e;
+    MlpCategoricalRecords c;
+};
+static_assert(sizeof(MlpCategoricalEpisodeArgs) <= 4096, "kernel parameter space");
+
 template <class P, int H>
 struct MlpShape {
     static constexpr int NT = H / 8;                                   // n-tiles of a hidden layer (= its k-tiles)
@@ -901,9 +922,21 @@ template <> struct MlpEpisodeRegisterWarps<SpeakerListener, 64> { static constex
 template <> struct MlpEpisodeRegisterWarps<Adversary<1, 2, 2>, 64> { static constexpr int value = 12; }; // 16 at 128
 template <> struct MlpEpisodeRegisterWarps<Reference, 64> { static constexpr int value = 8; };           // 8 at 168
 template <> struct MlpEpisodeRegisterWarps<Tag<4, 2, 2>, 64> { static constexpr int value = 8; };        // 8 at 168
-template <class P, int H, bool EPISODES = false>
+// The categorical form (the arg-max, the log-probability and the index stores in place of the softmax): the default
+// kernel of the same form's block, smaller where ptxas -v shows a spill there
+template <class P, int H, bool EPISODES>
+struct MlpCategoricalRegisterWarps {
+    static constexpr int value = EPISODES ? MlpEpisodeRegisterWarps<P, H>::value : MlpRegisterWarps<P, H>::value;
+};
+template <> struct MlpCategoricalRegisterWarps<Spread<3>, 64, false> { static constexpr int value = 12; };     // 8 bytes of stack at 128
+template <> struct MlpCategoricalRegisterWarps<Push<1, 1, 2>, 64, false> { static constexpr int value = 12; }; // 8 at 128
+template <> struct MlpCategoricalRegisterWarps<Push<1, 1, 2>, 64, true> { static constexpr int value = 12; };  // 8 at 128
+template <> struct MlpCategoricalRegisterWarps<Crypto, 64, true> { static constexpr int value = 12; };         // 16 at 128
+template <> struct MlpCategoricalRegisterWarps<Spread<4>, 64, true> { static constexpr int value = 8; };       // 8 at 168
+template <class P, int H, bool EPISODES = false, bool CATEGORICAL = false>
 __host__ __device__ constexpr int mlp_block_warps() {
-    constexpr int r = EPISODES ? MlpEpisodeRegisterWarps<P, H>::value : MlpRegisterWarps<P, H>::value;
+    constexpr int r = CATEGORICAL ? MlpCategoricalRegisterWarps<P, H, EPISODES>::value
+                    : (EPISODES ? MlpEpisodeRegisterWarps<P, H>::value : MlpRegisterWarps<P, H>::value);
     return r < mlp_smem_warps<P, H>() ? r : mlp_smem_warps<P, H>();
 }
 // the two programs whose weights fill most of the 227 KB
@@ -962,14 +995,38 @@ __device__ __forceinline__ void softmax_segment(const float (&z)[N], float (&pr)
     for (int c = 0; c < K; ++c) pr[B + c] = __fdiv_rn(e[c], sum);
 }
 
+// One sub-space of the categorical form: pr[B, B + K) = one_hot(k), k = argmax zs[B, B + K) with the lowest index
+// winning ties (zs: the perturbed logits when exploring, else z), and the return value log_softmax(z[B, B + K))[k] of
+// the unperturbed logits, its max and sum formed as in softmax_segment.  k is selected, never used as an index, so
+// the arrays stay in registers.
+template <int B, int K, int N>
+__device__ __forceinline__ float categorical_segment(const float (&zs)[N], const float (&z)[N], float (&pr)[N], int &k) {
+    static_assert(B + K <= N, "segment inside the action vector");
+    float best = zs[B], zk = z[B], m = z[B];
+    k = 0;
+#pragma unroll
+    for (int c = 1; c < K; ++c) {
+        if (zs[B + c] > best) { best = zs[B + c]; zk = z[B + c]; k = c; }
+        m = fmaxf(m, z[B + c]);
+    }
+    float sum = 0.0f;
+#pragma unroll
+    for (int c = 0; c < K; ++c) sum = __fadd_rn(sum, expf(__fsub_rn(z[B + c], m)));
+#pragma unroll
+    for (int c = 0; c < K; ++c) pr[B + c] = c == k ? 1.0f : 0.0f;
+    return __fsub_rn(__fsub_rn(zk, m), logf(sum));
+}
+
 // one agent of the tensor-core actor for the warp's 32 worlds: observation -> tile -> 3 GEMMs -> this lane's logits ->
 // (Gumbel-)softmax per sub-space -> decoded (u.x, u.y), and a speaker's utterance into cact[I * dim_c ...].  Called by
 // all 32 lanes (mma.sync is warp-collective).  t indexes the records.  The exploration noise is keyed by (pa.epoch, t),
-// and in the episode form (EPISODES) by (epoch, step) = (pa.epoch + e, t - e * T) in episode e.
-template <class P, int H, int I, bool EPISODES = false>
+// and in the episode form (EPISODES) by (epoch, step) = (pa.epoch + e, t - e * T) in episode e.  The categorical form
+// (CATEGORICAL) applies one-hot vectors instead of the softmax and writes the records of cr.
+template <class P, int H, int I, bool EPISODES = false, bool CATEGORICAL = false>
 __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typename P::W &w, const float *__restrict__ Wsm,
                                             float *s_warp, int lane, int t, int rows, bool active, int64_t w0, int64_t wi,
-                                            float *cact, int step = 0, uint64_t epoch = 0) {
+                                            float *cact, int step = 0, uint64_t epoch = 0,
+                                            const MlpCategoricalRecords *cr = nullptr) {
     using S = MlpShape<P, H>;
     constexpr int OD = P::obs_dim(I), KT1 = S::kt1(I), NT = S::NT, PITCH = ObsTile<OD>::kPitch;
     constexpr int AD = P::act_dim(I), NO = S::nout(I) / 8;
@@ -1075,6 +1132,11 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
     float z[AD];
 #pragma unroll
     for (int c = 0; c < AD; ++c) z[c] = lgs[lane * S::kLogitPitch + c];
+    float zl[CATEGORICAL ? AD : 1];                        // the unperturbed logits: the log-probability's
+    if constexpr (CATEGORICAL) {
+#pragma unroll
+        for (int c = 0; c < AD; ++c) zl[c] = z[c];
+    }
     if (pa.explore) {                                      // Gumbel-softmax sample (see the definition above)
         const uint64_t gw = pa.world_offset + static_cast<uint64_t>(wi);
         const uint2 key = make_uint2(static_cast<uint32_t>(pa.seed), static_cast<uint32_t>(pa.seed >> 32));
@@ -1095,9 +1157,28 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
         }
     }
     float pr[AD];
-    if constexpr (MOVE > 0) softmax_segment<0, MOVE>(z, pr);
-    if constexpr (COMM > 0) softmax_segment<MOVE, COMM>(z, pr);
-    if (pa.act_rec[I] != nullptr && active) {
+    if constexpr (CATEGORICAL) {                           // one-hot of the (perturbed) arg-max per sub-space
+        constexpr int NSUB = (MOVE > 0) + (COMM > 0);
+        int k[NSUB];
+        float lp = 0.0f;
+        if constexpr (MOVE > 0) lp = categorical_segment<0, MOVE>(z, zl, pr, k[0]);
+        if constexpr (COMM > 0) {
+            const float lc = categorical_segment<MOVE, COMM>(z, zl, pr, k[NSUB - 1]);
+            lp = MOVE > 0 ? __fadd_rn(lp, lc) : lc;
+        }
+        if (active) {
+            if (cr->index[I] != nullptr) {
+                int32_t *rec = cr->index[I] + (static_cast<int64_t>(t) * n + wi) * NSUB;
+#pragma unroll
+                for (int s = 0; s < NSUB; ++s) rec[s] = k[s];
+            }
+            if (cr->logp != nullptr) cr->logp[(static_cast<int64_t>(t) * P::A + I) * n + wi] = lp;
+        }
+    } else {
+        if constexpr (MOVE > 0) softmax_segment<0, MOVE>(z, pr);
+        if constexpr (COMM > 0) softmax_segment<MOVE, COMM>(z, pr);
+    }
+    if (!CATEGORICAL && pa.act_rec[I] != nullptr && active) {
         float *rec = pa.act_rec[I] + (static_cast<int64_t>(t) * n + wi) * AD;
 #pragma unroll
         for (int c = 0; c < AD; ++c) rec[c] = pr[c];
@@ -1117,14 +1198,15 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
     }
 }
 
-// the body of both forms; ea is null in the single-episode form (EPISODES = false)
-template <class P, int H, bool EPISODES>
-__device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEpisodeArgs *ea) {
+// the body of both forms; ea is null in the single-episode form (EPISODES = false), cr unless CATEGORICAL
+template <class P, int H, bool EPISODES, bool CATEGORICAL = false>
+__device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEpisodeArgs *ea,
+                                            const MlpCategoricalRecords *cr = nullptr) {
     static_assert(H == 32 || H == 64, "MLP policy rollout: hidden width 32 or 64");
     constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     using S = MlpShape<P, H>;
-    static_assert(mlp_block_warps<P, H, EPISODES>() >= 1 &&
-                  (S::kWeightFloats + mlp_block_warps<P, H, EPISODES>() * S::kWarpFloats) * 4 <= kMlpSmemBytes,
+    static_assert(mlp_block_warps<P, H, EPISODES, CATEGORICAL>() >= 1 &&
+                  (S::kWeightFloats + mlp_block_warps<P, H, EPISODES, CATEGORICAL>() * S::kWarpFloats) * 4 <= kMlpSmemBytes,
                   "one block fits an SM");
     const StepArgs &a = pa.s;
     extern __shared__ __align__(16) float smem[];
@@ -1188,8 +1270,8 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
             P::prepare(d, w);
             static_for<A>([&](auto ic) {
                 constexpr int i = decltype(ic)::value;
-                const float2 u = mlp_agent<P, H, i, EPISODES>(pa, w, smem + S::agent_off(i), s_warp, lane, tg, rows, active,
-                                                              w0, wi, cact, t, pa.epoch + e);
+                const float2 u = mlp_agent<P, H, i, EPISODES, CATEGORICAL>(pa, w, smem + S::agent_off(i), s_warp, lane, tg,
+                                                                           rows, active, w0, wi, cact, t, pa.epoch + e, cr);
                 ux[i] = u.x;
                 uy[i] = u.y;
             });
@@ -1285,6 +1367,18 @@ template <class P, int H>
 __global__ void __launch_bounds__(mlp_block_warps<P, H, true>() * 32)
     mpe_policy_mlp_episode_kernel(const __grid_constant__ MlpEpisodeArgs ea) {
     mlp_rollout<P, H, true>(ea.p, &ea);
+}
+
+template <class P, int H>
+__global__ void __launch_bounds__(mlp_block_warps<P, H, false, true>() * 32)
+    mpe_policy_mlp_categorical_kernel(const __grid_constant__ MlpCategoricalArgs ca) {
+    mlp_rollout<P, H, false, true>(ca.p, nullptr, &ca.c);
+}
+
+template <class P, int H>
+__global__ void __launch_bounds__(mlp_block_warps<P, H, true, true>() * 32)
+    mpe_policy_mlp_categorical_episode_kernel(const __grid_constant__ MlpCategoricalEpisodeArgs ca) {
+    mlp_rollout<P, H, true, true>(ca.e.p, &ca.e, &ca.c);
 }
 
 // ---- generic program for user scenarios (MPE_SCN_CUSTOM) ------------------------------------------
@@ -1473,7 +1567,10 @@ struct Program {
     int mlp_weight_floats[2], mlp_warp_floats[2], mlp_warps[2];
     void (*mlp_episode_fn[2])(MlpEpisodeArgs);   // its episode form (in-kernel reset between episodes)
     int mlp_episode_warps[2];
-    int mlp_explore_stride;            // Philox blocks per (step, agent) of its exploration noise
+    void (*mlp_cat_fn[2])(MlpCategoricalArgs);                  // the categorical form of both (one-hot actions)
+    void (*mlp_cat_episode_fn[2])(MlpCategoricalEpisodeArgs);
+    int mlp_cat_warps[2], mlp_cat_episode_warps[2];
+    int mlp_explore_stride;           // Philox blocks per (step, agent) of its exploration noise
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
     int rollout_smem;   // dynamic shared memory per WARP of the rollout kernel
     int A, L, NS, DIMC, INFO, G;
@@ -1514,6 +1611,14 @@ static Program make_program() {
         p.mlp_episode_fn[1] = mpe_policy_mlp_episode_kernel<P, 64>;
         p.mlp_episode_warps[0] = mlp_block_warps<P, 32, true>();
         p.mlp_episode_warps[1] = mlp_block_warps<P, 64, true>();
+        p.mlp_cat_fn[0] = mpe_policy_mlp_categorical_kernel<P, 32>;
+        p.mlp_cat_fn[1] = mpe_policy_mlp_categorical_kernel<P, 64>;
+        p.mlp_cat_warps[0] = mlp_block_warps<P, 32, false, true>();
+        p.mlp_cat_warps[1] = mlp_block_warps<P, 64, false, true>();
+        p.mlp_cat_episode_fn[0] = mpe_policy_mlp_categorical_episode_kernel<P, 32>;
+        p.mlp_cat_episode_fn[1] = mpe_policy_mlp_categorical_episode_kernel<P, 64>;
+        p.mlp_cat_episode_warps[0] = mlp_block_warps<P, 32, true, true>();
+        p.mlp_cat_episode_warps[1] = mlp_block_warps<P, 64, true, true>();
         p.mlp_explore_stride = mlp_explore_stride<P>();
     }
     p.smem_bytes = Shape<P>::kWarpBytes;  // per warp
@@ -1654,6 +1759,13 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
             if (prog->mlp_episode_fn[k])
                 CUDA_TRY(cudaFuncSetAttribute(prog->mlp_episode_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp_episode_warps[k]) * 4));
+        for (int k = 0; k < 2; ++k)
+            if (prog->mlp_cat_fn[k]) {
+                CUDA_TRY(cudaFuncSetAttribute(prog->mlp_cat_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp_cat_warps[k]) * 4));
+                CUDA_TRY(cudaFuncSetAttribute(prog->mlp_cat_episode_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp_cat_episode_warps[k]) * 4));
+            }
         if (prog->rollout_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->rollout_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->rollout_smem * max_warps_per_block(prog->rollout_smem)));
@@ -2004,24 +2116,44 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
                          stream, params, false, "cudaLaunchKernelExC(rollout_policy)");
 }
 
-extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
-                                      const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
-                                      const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
-                                      int32_t hidden, int32_t n_steps, int32_t explore, uint64_t explore_seed,
-                                      uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n, float *rew_sum,
-                                      float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
-                                      uint8_t *done, uint32_t flags, void *stream) {
+// the categorical form's records (cat != null; then act_record_n is null) after the checks both forms share
+static int fill_categorical(const mpe_env *h, MlpCategoricalRecords &c, int32_t *const *act_index_record_n, float *logp_steps) {
+    if (logp_steps != nullptr && !ok4(logp_steps)) return MPE_ERR_BAD_ARG;
+    c.logp = logp_steps;
+    for (int i = 0; i < h->prog->A; ++i) {
+        c.index[i] = act_index_record_n ? act_index_record_n[i] : nullptr;
+        if (c.index[i] != nullptr && !ok4(c.index[i])) return MPE_ERR_BAD_ARG;
+    }
+    return MPE_OK;
+}
+
+// mpe_rollout_policy_mlp (categorical = false) and mpe_rollout_policy_mlp_categorical (act_record_n null)
+static int rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
+                              const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
+                              const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
+                              int32_t hidden, int32_t n_steps, int32_t explore, uint64_t explore_seed,
+                              uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n, float *rew_sum,
+                              float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
+                              uint8_t *done, uint32_t flags, void *stream, bool categorical,
+                              int32_t *const *act_index_record_n, float *logp_steps) {
     if (!h || n_steps < 0 || !w1_n || !b1_n || !w2_n || !b2_n || !w3_n || !b3_n) return MPE_ERR_BAD_ARG;
     if (h->device < 0) return MPE_ERR_NO_DEVICE;
     const int k = hidden == 32 ? 0 : (hidden == 64 ? 1 : -1);
-    if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || h->prog->mlp_fn[k] == nullptr) return MPE_ERR_UNSUPPORTED;
+    if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM ||
+        (categorical ? reinterpret_cast<const void *>(h->prog->mlp_cat_fn[k]) : reinterpret_cast<const void *>(h->prog->mlp_fn[k])) == nullptr)
+        return MPE_ERR_UNSUPPORTED;
     if (flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
     if (rew_steps != nullptr && !ok4(rew_steps)) return MPE_ERR_BAD_ARG;
     // the Philox counter word holds (t * A + i) * S + b below the tag bit
     if (explore && static_cast<int64_t>(n_steps) * h->prog->A * h->prog->mlp_explore_stride > static_cast<int64_t>(kExploreTag))
         return MPE_ERR_BAD_ARG;
-    NvtxRange range("mpe_rollout_policy_mlp");
-    MlpPolicyArgs pa{};
+    NvtxRange range(categorical ? "mpe_rollout_policy_mlp_categorical" : "mpe_rollout_policy_mlp");
+    MlpCategoricalArgs ca{};
+    if (categorical) {
+        const int rc = fill_categorical(h, ca.c, act_index_record_n, logp_steps);
+        if (rc) return rc;
+    }
+    MlpPolicyArgs &pa = ca.p;
     StepArgs &a = pa.s;
     int r = fill_state(h, a, pv, lm, comm, goal);
     if (r) return r;
@@ -2052,25 +2184,60 @@ extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, fl
     const int64_t warps = (h->n + 31) / 32;
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
-    if (wpb > h->prog->mlp_warps[k]) wpb = h->prog->mlp_warps[k];
-    void *params[] = {&pa};
+    const int cap = categorical ? h->prog->mlp_cat_warps[k] : h->prog->mlp_warps[k];
+    if (wpb > cap) wpb = cap;
+    void *params[] = {categorical ? static_cast<void *>(&ca) : static_cast<void *>(&pa)};
     const size_t smem = (static_cast<size_t>(h->prog->mlp_weight_floats[k]) + static_cast<size_t>(h->prog->mlp_warp_floats[k]) * wpb) * 4;
-    return launch_kernel(h, reinterpret_cast<const void *>(h->prog->mlp_fn[k]), (warps + wpb - 1) / wpb,
-                         static_cast<int>(32 * wpb), smem, stream, params, false, "cudaLaunchKernelExC(rollout_policy_mlp)");
+    return launch_kernel(h, categorical ? reinterpret_cast<const void *>(h->prog->mlp_cat_fn[k])
+                                        : reinterpret_cast<const void *>(h->prog->mlp_fn[k]),
+                         (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb), smem, stream, params, false,
+                         categorical ? "cudaLaunchKernelExC(rollout_policy_mlp_categorical)"
+                                     : "cudaLaunchKernelExC(rollout_policy_mlp)");
 }
 
-extern "C" int mpe_rollout_policy_mlp_episodes(mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal,
-                                               const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
-                                               const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
-                                               int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
-                                               uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed,
-                                               uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew,
-                                               float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
-                                               float *const *final_obs_record_n, uint8_t *done, uint32_t flags, void *stream) {
+extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
+                                      const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
+                                      const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
+                                      int32_t hidden, int32_t n_steps, int32_t explore, uint64_t explore_seed,
+                                      uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n, float *rew_sum,
+                                      float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
+                                      uint8_t *done, uint32_t flags, void *stream) {
+    return rollout_policy_mlp(h, pv, lm, comm, goal, w1_n, b1_n, w2_n, b2_n, w3_n, b3_n, hidden, n_steps, explore,
+                              explore_seed, explore_epoch, world_offset, obs_n, rew_sum, rew_steps, act_record_n,
+                              obs_record_n, done, flags, stream, false, nullptr, nullptr);
+}
+
+extern "C" int mpe_rollout_policy_mlp_categorical(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
+                                                  const float *const *w1_n, const float *const *b1_n,
+                                                  const float *const *w2_n, const float *const *b2_n,
+                                                  const float *const *w3_n, const float *const *b3_n, int32_t hidden,
+                                                  int32_t n_steps, int32_t explore, uint64_t explore_seed,
+                                                  uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n,
+                                                  float *rew_sum, float *rew_steps, float *logp_steps,
+                                                  int32_t *const *act_index_record_n, float *const *obs_record_n,
+                                                  uint8_t *done, uint32_t flags, void *stream) {
+    return rollout_policy_mlp(h, pv, lm, comm, goal, w1_n, b1_n, w2_n, b2_n, w3_n, b3_n, hidden, n_steps, explore,
+                              explore_seed, explore_epoch, world_offset, obs_n, rew_sum, rew_steps, nullptr,
+                              obs_record_n, done, flags, stream, true, act_index_record_n, logp_steps);
+}
+
+// mpe_rollout_policy_mlp_episodes (categorical = false) and mpe_rollout_policy_mlp_categorical_episodes
+static int rollout_policy_mlp_episodes(mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal,
+                                       const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
+                                       const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
+                                       int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
+                                       uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed,
+                                       uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew,
+                                       float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
+                                       float *const *final_obs_record_n, uint8_t *done, uint32_t flags, void *stream,
+                                       bool categorical, int32_t *const *act_index_record_n, float *logp_steps) {
     if (!h) return MPE_ERR_BAD_ARG;
     if (h->device < 0) return MPE_ERR_NO_DEVICE;
     const int k = hidden == 32 ? 0 : (hidden == 64 ? 1 : -1);
-    if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || h->prog->mlp_episode_fn[k] == nullptr) return MPE_ERR_UNSUPPORTED;
+    if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM ||
+        (categorical ? reinterpret_cast<const void *>(h->prog->mlp_cat_episode_fn[k])
+                     : reinterpret_cast<const void *>(h->prog->mlp_episode_fn[k])) == nullptr)
+        return MPE_ERR_UNSUPPORTED;
     if (flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
     // records are indexed by the global step e * episode_length + t, an int
     if (episode_length < 1 || n_episodes < 1 || static_cast<int64_t>(episode_length) * n_episodes > 0x7fffffffLL)
@@ -2080,8 +2247,13 @@ extern "C" int mpe_rollout_policy_mlp_episodes(mpe_handle h, void *pv, void *lm,
         return MPE_ERR_BAD_ARG;
     if (!w1_n || !b1_n || !w2_n || !b2_n || !w3_n || !b3_n) return MPE_ERR_BAD_ARG;
     if (rew_steps != nullptr && !ok4(rew_steps)) return MPE_ERR_BAD_ARG;
-    NvtxRange range("mpe_rollout_policy_mlp_episodes");
-    MlpEpisodeArgs ea{};
+    NvtxRange range(categorical ? "mpe_rollout_policy_mlp_categorical_episodes" : "mpe_rollout_policy_mlp_episodes");
+    MlpCategoricalEpisodeArgs ca{};
+    if (categorical) {
+        const int rc = fill_categorical(h, ca.c, act_index_record_n, logp_steps);
+        if (rc) return rc;
+    }
+    MlpEpisodeArgs &ea = ca.e;
     MlpPolicyArgs &pa = ea.p;
     StepArgs &a = pa.s;
     int r = fill_state(h, a, pv, lm, comm, goal);
@@ -2120,12 +2292,42 @@ extern "C" int mpe_rollout_policy_mlp_episodes(mpe_handle h, void *pv, void *lm,
     const int64_t warps = (h->n + 31) / 32;
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
-    if (wpb > h->prog->mlp_episode_warps[k]) wpb = h->prog->mlp_episode_warps[k];
-    void *params[] = {&ea};
+    const int cap = categorical ? h->prog->mlp_cat_episode_warps[k] : h->prog->mlp_episode_warps[k];
+    if (wpb > cap) wpb = cap;
+    void *params[] = {categorical ? static_cast<void *>(&ca) : static_cast<void *>(&ea)};
     const size_t smem = (static_cast<size_t>(h->prog->mlp_weight_floats[k]) + static_cast<size_t>(h->prog->mlp_warp_floats[k]) * wpb) * 4;
-    return launch_kernel(h, reinterpret_cast<const void *>(h->prog->mlp_episode_fn[k]), (warps + wpb - 1) / wpb,
-                         static_cast<int>(32 * wpb), smem, stream, params, false,
-                         "cudaLaunchKernelExC(rollout_policy_mlp_episodes)");
+    return launch_kernel(h, categorical ? reinterpret_cast<const void *>(h->prog->mlp_cat_episode_fn[k])
+                                        : reinterpret_cast<const void *>(h->prog->mlp_episode_fn[k]),
+                         (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb), smem, stream, params, false,
+                         categorical ? "cudaLaunchKernelExC(rollout_policy_mlp_categorical_episodes)"
+                                     : "cudaLaunchKernelExC(rollout_policy_mlp_episodes)");
+}
+
+extern "C" int mpe_rollout_policy_mlp_episodes(mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal,
+                                               const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
+                                               const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
+                                               int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
+                                               uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed,
+                                               uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew,
+                                               float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
+                                               float *const *final_obs_record_n, uint8_t *done, uint32_t flags, void *stream) {
+    return rollout_policy_mlp_episodes(h, pv, lm, comm, goal, w1_n, b1_n, w2_n, b2_n, w3_n, b3_n, hidden, episode_length,
+                                       n_episodes, explore, explore_seed, explore_epoch, reset_seed, reset_epoch,
+                                       world_offset, obs_n, ep_rew, rew_steps, act_record_n, obs_record_n,
+                                       final_obs_record_n, done, flags, stream, false, nullptr, nullptr);
+}
+
+extern "C" int mpe_rollout_policy_mlp_categorical_episodes(
+    mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal, const float *const *w1_n, const float *const *b1_n,
+    const float *const *w2_n, const float *const *b2_n, const float *const *w3_n, const float *const *b3_n, int32_t hidden,
+    int32_t episode_length, int32_t n_episodes, int32_t explore, uint64_t explore_seed, uint64_t explore_epoch,
+    uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew, float *rew_steps,
+    float *logp_steps, int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n,
+    uint8_t *done, uint32_t flags, void *stream) {
+    return rollout_policy_mlp_episodes(h, pv, lm, comm, goal, w1_n, b1_n, w2_n, b2_n, w3_n, b3_n, hidden, episode_length,
+                                       n_episodes, explore, explore_seed, explore_epoch, reset_seed, reset_epoch,
+                                       world_offset, obs_n, ep_rew, rew_steps, nullptr, obs_record_n, final_obs_record_n,
+                                       done, flags, stream, true, act_index_record_n, logp_steps);
 }
 
 // adjacent (dst, src, bytes) copies with equal small gaps on both sides are issued as one DMA

@@ -244,7 +244,7 @@ class MultiAgentEnv(_Env):
         return obs_n, reward_n, done_n, info_n
 
     def rollout_policy(self, policies, n_steps, record_actions=False, per_step_rewards=False, record_observations=False,
-                       explore_seed=None, episode_length=None):
+                       explore_seed=None, episode_length=None, action_mode="softmax", record_log_probs=False):
         """T closed-loop steps in ONE kernel launch with the actors inside the kernel.
 
         One hidden layer (mpe_rollout_policy, fp32): agent i acts with softmax(W2_i relu(W1_i obs_i + b1_i) + b2_i).
@@ -279,9 +279,29 @@ class MultiAgentEnv(_Env):
         e * L + t).  reward_sum_n[i] is [E, N], the return of every episode; obs_n holds the observations of the freshly
         reset state, done_n is all False, and with record_observations extras["final_observations"] is a list of
         [E, N, obs_dim_i] tensors: the observation after the last step of each episode, before its reset (the next
-        observation of the terminal transition).  n_steps must be a positive multiple of L (else ValueError)."""
+        observation of the terminal transition).  n_steps must be a positive multiple of L (else ValueError).
+
+        action_mode="categorical" (two-hidden-layer actor only; the default "softmax" is everything above) collects
+        policy-gradient (PPO, A2C) experience: per sub-space the agent takes k = argmax(logits - log(-log u)) when
+        exploring -- a categorical sample, the arg-max of the Gumbel-softmax sample the default mode would take from the
+        same state, seed and epoch -- or k = argmax(logits) without explore_seed, the lowest index winning ties, and
+        applies the one-hot vector of k, exactly as env.step applies that float vector.  extras["actions"]
+        (record_actions) is then a list of int32 [T, N, n_sub_i] tensors, n_sub_i the agent's number of sub-spaces (1,
+        or 2 for a movable speaker: movement, then utterance).  k is the position in the logit segment, i.e. the one-hot
+        convention: movement index 1 is +x.  It is NOT the code env.discrete_action_input takes (there 1 is -x), so
+        replay the indices as one-hot vectors, never through discrete_action_input.  record_log_probs=True returns
+        extras["log_probs"], a float32 [T, n, N] tensor: the sum over the agent's sub-spaces of
+        log_softmax(logits)[k] on the logits the kernel acted with (Categorical(logits).log_prob(k), the behaviour
+        policy's term of PPO's ratio), else None.  Returns, observations, episode_length and both epochs behave as in
+        the default mode.  An unknown action_mode, or record_log_probs in the default mode, raises ValueError; the
+        one-hidden-layer actor raises NotImplementedError.  Actors with LayerNorm or tanh layers (MAPPO's default MLP)
+        are not this network and are refused."""
         import torch
         world = self.world
+        if action_mode not in ("softmax", "categorical"):
+            raise ValueError("rollout_policy: action_mode must be 'softmax' or 'categorical', got %r" % (action_mode,))
+        if record_log_probs and action_mode != "categorical":
+            raise ValueError("rollout_policy: record_log_probs needs action_mode='categorical'")
         if not world.batched:
             raise ValueError("rollout_policy needs a batched env (make_env(..., num_envs=N))")
         if self._custom or self.discrete_action_input or self.force_discrete_action:
@@ -294,7 +314,10 @@ class MultiAgentEnv(_Env):
                              % (int(n_steps), int(episode_length)))
         if any(_has_two_hidden_layers(p) for p in policies):
             return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
-                                            explore_seed, episode_length)
+                                            explore_seed, episode_length, action_mode == "categorical", record_log_probs)
+        if action_mode == "categorical":
+            raise NotImplementedError("rollout_policy: action_mode='categorical' needs the two-hidden-layer actor "
+                                      "(Linear -> ReLU -> Linear -> ReLU -> Linear)")
         if episode_length is not None:
             raise NotImplementedError("rollout_policy: episode_length needs the two-hidden-layer actor "
                                       "(Linear -> ReLU -> Linear -> ReLU -> Linear)")
@@ -334,7 +357,7 @@ class MultiAgentEnv(_Env):
         return list(out.obs), list(out.rew_list), list(out.done_list), info_n, {"actions": actions, "rewards": rew_steps}
 
     def _rollout_policy_mlp(self, policies, n_steps, record_actions, per_step_rewards, record_observations, explore_seed,
-                            episode_length=None):
+                            episode_length=None, categorical=False, record_log_probs=False):
         import torch
         world = self.world
         nw = world.bind()
@@ -346,16 +369,27 @@ class MultiAgentEnv(_Env):
         out = nw.out if self.reuse_buffers else nw.new_outputs()
         dev = dict(dtype=torch.float32, device=nw.device)
         rew_steps = torch.empty((T, self.n, N), **dev) if per_step_rewards else None
-        actions = [torch.empty((T, N, ad), **dev) for ad in nw.act_dims] if record_actions else None
+        if categorical:   # int32 [T, N, n_sub_i]: movement if movable, then utterance if it speaks
+            n_sub = [int(bool(nw.desc.agent_movable[i])) + int(not nw.desc.agent_silent[i]) for i in range(self.n)]
+            actions = [torch.empty((T, N, s), dtype=torch.int32, device=nw.device) for s in n_sub] if record_actions else None
+        else:
+            actions = [torch.empty((T, N, ad), **dev) for ad in nw.act_dims] if record_actions else None
+        log_probs = torch.empty((T, self.n, N), **dev) if record_log_probs else None
         observations = [torch.empty((T, N, od), **dev) for od in nw.obs_dims] if record_observations else None
         seed = None if explore_seed is None else int(explore_seed) & 0xFFFFFFFFFFFFFFFF
         act_ptrs = _lib.ptr_array([a.data_ptr() for a in actions]) if actions is not None else None
         obs_ptrs = _lib.ptr_array([o.data_ptr() for o in observations]) if observations is not None else None
         extras = {"actions": actions, "rewards": rew_steps, "observations": observations}
+        if categorical:
+            extras["log_probs"] = log_probs
         if episode_length is None:
             E = 1
-            nw.rollout_policy_mlp(w_ptrs, hidden, T, out, self._flags(), rew_steps, act_ptrs, obs_ptrs,
-                                  explore_seed=seed, explore_epoch=self.explore_epoch)
+            if categorical:
+                nw.rollout_policy_mlp_categorical(w_ptrs, hidden, T, out, self._flags(), rew_steps, log_probs, act_ptrs,
+                                                  obs_ptrs, explore_seed=seed, explore_epoch=self.explore_epoch)
+            else:
+                nw.rollout_policy_mlp(w_ptrs, hidden, T, out, self._flags(), rew_steps, act_ptrs, obs_ptrs,
+                                      explore_seed=seed, explore_epoch=self.explore_epoch)
             reward_n = list(out.rew_list)
         else:
             L = int(episode_length)
@@ -364,7 +398,8 @@ class MultiAgentEnv(_Env):
             final = [torch.empty((E, N, od), **dev) for od in nw.obs_dims] if record_observations else None
             nw.rollout_policy_mlp_episodes(w_ptrs, hidden, L, E, out, ep_rew, self._flags(), rew_steps, act_ptrs, obs_ptrs,
                                            _lib.ptr_array([o.data_ptr() for o in final]) if final is not None else None,
-                                           explore_seed=seed, explore_epoch=self.explore_epoch)
+                                           explore_seed=seed, explore_epoch=self.explore_epoch, categorical=categorical,
+                                           logp_steps=log_probs)
             reward_n = list(ep_rew.unbind(1))
             extras["final_observations"] = final
         if seed is not None:

@@ -1,0 +1,98 @@
+"""CPU checks of the categorical form of the two-hidden-layer actor (env.rollout_policy(..., action_mode="categorical")):
+the new C entry points are declared and bound, the NumPy models the GPU tests judge the kernel by (log-probability,
+Gumbel arg-max, one-hot replay) agree with independent formulations, and the refusals that need no device."""
+import os
+import re
+
+import numpy as np
+import pytest
+
+import mlp_helpers
+from helpers import make_product_env
+from mlp_categorical_helpers import bounds, categorical_pick, log_softmax_at, one_hot
+from mlp_comm_helpers import gumbel_noise, segment_softmax
+
+torch = pytest.importorskip("torch")
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+ENTRY_POINTS = ("mpe_rollout_policy_mlp_categorical", "mpe_rollout_policy_mlp_categorical_episodes")
+
+
+def test_categorical_entry_points_are_declared_and_bound():
+    import ctypes
+    from multiagent_particle_envs_b200 import _lib
+    header = open(os.path.join(ROOT, "include", "mpe_b200.h")).read()
+    declared = set(re.findall(r"MPE_API[^;(]*?\b(mpe_[a-z_]+)\s*\(", header))
+    lib = ctypes.CDLL(_lib.LIB_PATH)
+    for name in ENTRY_POINTS:
+        assert name in declared and name in _lib.EXPORTED_SYMBOLS and hasattr(lib, name), name
+    # the parameters of the default form, with the int32 index records in place of the float action records and the
+    # log-probabilities next to the per-step rewards
+    for name, base in zip(ENTRY_POINTS, ("mpe_rollout_policy_mlp", "mpe_rollout_policy_mlp_episodes")):
+        got, want = _lib._SIGNATURES[name][1], list(_lib._SIGNATURES[base][1])
+        rew_steps = 19 if base == "mpe_rollout_policy_mlp" else 22
+        assert got == want[:rew_steps + 1] + [_lib._P] + want[rew_steps + 1:], name
+    assert _lib.MPE_ABI_VERSION == 1
+
+
+@pytest.mark.parametrize("segs", [[5], [3], [5, 10], [5, 4]])
+def test_log_probability_model_is_scipy_log_softmax(segs):
+    from scipy.special import log_softmax
+    rng = np.random.RandomState(1)
+    z = rng.randn(4096, sum(segs)) * 3.0
+    k = np.stack([rng.randint(0, b - a, 4096) for a, b in bounds(segs)], -1)
+    want = sum(np.take_along_axis(log_softmax(z[:, a:b], -1), k[:, s:s + 1], 1)[:, 0]
+               for s, (a, b) in enumerate(bounds(segs)))
+    np.testing.assert_allclose(log_softmax_at(z, k, segs), want, rtol=0, atol=1e-12)
+
+
+@pytest.mark.parametrize("segs,stride", [([5], 2), ([3], 2), ([5, 10], 4), ([5, 3], 2)])
+def test_gumbel_argmax_model_is_the_argmax_of_the_gumbel_softmax_sample(segs, stride):
+    """categorical_pick(z + g) per sub-space is the arg-max of segment_softmax(z + g), the default mode's sample, with g
+    the exploration stream of mlp_comm_helpers.gumbel_noise (which for five logits is mlp_helpers.gumbel_noise)"""
+    n, A = 4096, 3
+    rng = np.random.RandomState(2)
+    z = rng.randn(n, sum(segs))
+    for t, i in ((0, 0), (7, 2)):
+        g = gumbel_noise(99, 3, np.arange(n) + 10 ** 6, t, i, A, n_logits=sum(segs), stride=stride)
+        if segs == [5]:
+            np.testing.assert_array_equal(g, mlp_helpers.gumbel_noise(99, 3, np.arange(n) + 10 ** 6, t, i, A))
+        k = categorical_pick(z + g, segs)
+        sample = segment_softmax(z + g, segs)
+        for s, (a, b) in enumerate(bounds(segs)):
+            np.testing.assert_array_equal(k[:, s], np.argmax(sample[:, a:b], -1))
+        # the picks are distributed as softmax(z): over many draws of one row the frequencies approach it
+    zz = np.tile(np.array([[0.5, -1.0, 1.2]]), (200000, 1))
+    g = gumbel_noise(5, 0, np.arange(200000), 0, 0, 1, n_logits=3, stride=2)
+    freq = np.bincount(categorical_pick(zz + g, [3])[:, 0], minlength=3) / 200000.0
+    np.testing.assert_allclose(freq, segment_softmax(zz[:1])[0], atol=5e-3)
+
+
+def test_ties_go_to_the_lowest_index_and_one_hot_inverts_the_pick():
+    z = np.array([[1.0, 3.0, 3.0, 0.0, 0.0, 2.0, 2.0, 2.0]])
+    k = categorical_pick(z, [5, 3])
+    assert k.tolist() == [[1, 0]]
+    assert one_hot(k, [5, 3]).tolist() == [[0, 1, 0, 0, 0, 1, 0, 0]]
+    rng = np.random.RandomState(3)
+    k = np.stack([rng.randint(0, 5, 100), rng.randint(0, 10, 100)], -1)
+    np.testing.assert_array_equal(categorical_pick(one_hot(k, [5, 10]), [5, 10]), k)
+
+
+def test_refusals_without_a_device():
+    """action_mode and record_log_probs are checked before anything else; the one-hidden-layer actor has no
+    categorical form"""
+    nn = torch.nn
+    env = make_product_env("simple_spread_n3", num_envs=64)
+    obs_dims = env.world.native_shapes().obs_dims               # device-less handle
+    two = [nn.Sequential(nn.Linear(od, 32), nn.ReLU(), nn.Linear(32, 32), nn.ReLU(), nn.Linear(32, 5)) for od in obs_dims]
+    one = [nn.Sequential(nn.Linear(od, 32), nn.ReLU(), nn.Linear(32, 5)) for od in obs_dims]
+    for mode in ("argmax", "Categorical", None):
+        with pytest.raises(ValueError, match="action_mode"):
+            env.rollout_policy(two, 4, action_mode=mode)
+    with pytest.raises(ValueError, match="record_log_probs"):
+        env.rollout_policy(two, 4, record_log_probs=True)
+    with pytest.raises(ValueError, match="record_log_probs"):
+        env.rollout_policy(two, 4, action_mode="softmax", record_log_probs=True)
+    with pytest.raises(NotImplementedError, match="two-hidden-layer"):
+        env.rollout_policy(one, 4, action_mode="categorical")
+    with pytest.raises(NotImplementedError, match="two-hidden-layer"):
+        env.rollout_policy(one, 4, action_mode="categorical", record_log_probs=True)

@@ -4,7 +4,12 @@
       --layers 2: Linear-ReLU-Linear-softmax in fp32 (mpe_rollout_policy);
       --layers 3: MADDPG's Linear-ReLU-Linear-ReLU-Linear on the tensor cores in TF32 (mpe_rollout_policy_mlp),
       --explore: with the Gumbel-softmax sample instead of softmax (--layers 3 only);
-  (b) the same actors as torch modules + env.step, all captured in one CUDA graph (rollout.GraphedRollout).
+      --categorical: policy-gradient actions (action_mode="categorical", --layers 3 only): the one-hot vector of the
+      arg-max of the logits (--explore: of the Gumbel-perturbed logits) per sub-space, recording the indices and the
+      log-probabilities;
+  (b) the same actors as torch modules + env.step, all captured in one CUDA graph (rollout.GraphedRollout); with
+      --categorical the graphed policy takes argmax(logits - log(-log u)) per sub-space, its one_hot and
+      log_softmax(logits).gather(k) for the log-probabilities.
 Device time per step of each.  With --layers 3 the actor of agent i has act_dim_i outputs and its action is one
 (Gumbel-)softmax per action sub-space (5 movement logits if the agent moves, then dim_c utterance logits if it speaks).
 Also the actor's FLOPs per step, computed from the padded shapes the kernel multiplies (2 (K1 H + H H + NOUT H) per
@@ -51,6 +56,8 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--layers", type=int, choices=(2, 3), default=2, help="Linear layers of the actor")
     ap.add_argument("--explore", action="store_true", help="Gumbel-softmax exploration (--layers 3)")
+    ap.add_argument("--categorical", action="store_true",
+                    help="one-hot arg-max actions with index and log-probability records (--layers 3)")
     args = ap.parse_args()
     try:
         skw = {k: int(v) for k, v in (kv.split("=", 1) for kv in args.scenario_kwargs)}
@@ -58,6 +65,8 @@ def main():
         ap.error("--scenario-kwargs takes KEY=INT pairs")
     if args.explore and args.layers != 3:
         ap.error("--explore needs --layers 3")
+    if args.categorical and args.layers != 3:
+        ap.error("--categorical needs --layers 3")
     import torch
     import __graft_entry__ as g
     g.build(quiet=True)
@@ -78,8 +87,11 @@ def main():
     segs = sub_spaces(env.world) if args.layers == 3 else [[5]] * len(nw.obs_dims)
     res = {"config": {"scenario": args.scenario, "scenario_kwargs": skw, "n_env": n, "T": T, "hidden": H}}
     if args.layers == 3:
-        res["config"].update(layers=3, explore=args.explore, torch_float32_matmul_precision=torch.get_float32_matmul_precision())
+        res["config"].update(layers=3, explore=args.explore, categorical=args.categorical,
+                             torch_float32_matmul_precision=torch.get_float32_matmul_precision())
     kw = {"explore_seed": 1} if args.explore else {}
+    if args.categorical:
+        kw.update(action_mode="categorical", record_actions=True, record_log_probs=True)
     # (a) in-kernel actors
     for _ in range(2):
         env.rollout_policy(mods, T, **kw)
@@ -104,7 +116,21 @@ def main():
             return torch.softmax(z, -1)
         return torch.cat([torch.softmax(p, -1) for p in torch.split(z, seg, -1)], -1)
 
+    def categorical(z, seg):   # one-hot of the (perturbed) arg-max per sub-space, and the log-probability
+        zp = z - torch.log(-torch.log(torch.rand(z.shape, device=dev))) if args.explore else z
+        hot, logp = [], 0.0
+        for zs, ps in zip(torch.split(z, seg, -1), torch.split(zp, seg, -1)):
+            k = ps.argmax(-1, keepdim=True)
+            hot.append(torch.nn.functional.one_hot(k[:, 0], zs.shape[-1]).float())
+            logp = logp + torch.log_softmax(zs, -1).gather(-1, k)[:, 0]
+        logps.append(logp)
+        return torch.cat(hot, -1)
+
+    logps = []   # the graph's log-probability outputs, kept as a trainer would keep them
+
     def policy(obs_n):
+        if args.categorical:
+            return [categorical(m(o), seg) for m, o, seg in zip(mods, obs_n, segs)]
         if args.explore:   # the same Gumbel-softmax sample, noise from torch's generator
             return [act(m(o) - torch.log(-torch.log(torch.rand(o.shape[0], sum(seg), device=dev))), seg)
                     for m, o, seg in zip(mods, obs_n, segs)]

@@ -75,13 +75,14 @@ def main():
         print("| " + " | ".join(str(x) for x in r) + " |")
     mlp = []
     for mangled, (reg, stack) in usage.items():
-        m = re.match(r"void mpe::mpe_policy_mlp_(rollout|episode)_kernel<mpe::(.+), (\d+)>\(", names[mangled])
+        m = re.match(r"void mpe::mpe_policy_mlp_(rollout|episode|categorical|categorical_episode)_kernel<mpe::(.+), (\d+)>\(",
+                     names[mangled])
         if m:
             c = mix.get(mangled, {})
             mlp.append((m.group(2), m.group(3), m.group(1), reg, stack, c["total"], c["HMMA"], c["LDS"], c["MUFU"]))
     if mlp:
-        print("\n## Closed-loop rollout with the two-hidden-layer actor (`mpe_policy_mlp_rollout_kernel`, and its episode form "
-              "`mpe_policy_mlp_episode_kernel`, TF32 mma.sync)\n")
+        print("\n## Closed-loop rollout with the two-hidden-layer actor (`mpe_policy_mlp_rollout_kernel`, its episode form "
+              "`mpe_policy_mlp_episode_kernel` and the categorical forms of both, TF32 mma.sync)\n")
         print("| program | H | form | regs | stack | instr | HMMA | LDS | MUFU |")
         print("|---|---|---|---|---|---|---|---|---|")
         for r in sorted(mlp):
