@@ -892,52 +892,50 @@ struct MlpShape {
 
 // Warps per block at most: one copy of the weights serves all of them, and with 6-212 KB of weights one block is what
 // fits an SM, so this is also the residency.  The smaller of two limits:
-//  - registers (MlpRegisterWarps): a block's warps share the four SM sub-partitions' 16 K registers each, so 16 warps
+//  - registers (mlp_register_warps): a block's warps share the four SM sub-partitions' 16 K registers each, so 16 warps
 //    leave 128 registers per thread, 9-12 warps 168 and 8 or fewer 255.  Blocks are 16 warps unless that spills
 //    (ptxas -v): then 12, or 8 where 168 spills too.  At H = 64 every program with four or more agents (their state
 //    next to the 64 registers of h1) and simple_reference (two 8-column logit tiles and 20 comm floats next to h1)
-//    take 12; the listed specialisations are the rest.
+//    take 12; the exceptions below are the rest.  The episode form adds the reset draw and the episode-end stores, the
+//    categorical form the arg-max, the log-probability and the index stores, so an exception names the forms it holds
+//    for.
 //  - shared memory (mlp_smem_warps): the weights plus kWarpFloats per warp within the 227 KB a block may opt in to on
 //    H100.  Below the register limit only for tag 6+2 at H = 64 (212 KB of weights, 3 warps).
-template <class P, int H>
-struct MlpRegisterWarps { static constexpr int value = (H == 64 && (P::A >= 4 || mlp_max_act_dim<P>() > 8)) ? 12 : 16; };
-template <> struct MlpRegisterWarps<Spread<2>, 64> { static constexpr int value = 12; };       // 8 bytes of stack at 128
-template <> struct MlpRegisterWarps<Tag<1, 1, 2>, 64> { static constexpr int value = 12; };    // 8 at 128
-template <> struct MlpRegisterWarps<Tag<2, 1, 2>, 64> { static constexpr int value = 12; };    // 8 at 128
-template <> struct MlpRegisterWarps<Spread<6>, 64> { static constexpr int value = 8; };        // 16 at 168
-template <> struct MlpRegisterWarps<Spread<6>, 32> { static constexpr int value = 12; };       // 48 at 128
-template <> struct MlpRegisterWarps<Tag<4, 2, 2>, 32> { static constexpr int value = 12; };    // 16 at 128
-template <> struct MlpRegisterWarps<Tag<6, 2, 3>, 32> { static constexpr int value = 8; };     // 64 at 128, 8 at 168
+// The forms, indexed by episodes | categorical << 1, and the masks an exception lists them by
+enum : int { kMlpForms = 4, kFormS = 1, kFormE = 2, kFormC = 4, kFormCE = 8, kFormAll = 15 };
+template <int FORMS, int WARPS>
+struct MlpException { static constexpr int forms = FORMS, warps = WARPS; };
+// One exception per (program, H), so that no kernel matches two: a second one would redefine the specialisation
+template <class P, int H> struct MlpRegisterException : MlpException<0, 0> {};
+template <> struct MlpRegisterException<Spread<2>, 64> : MlpException<kFormAll, 12> {};                   // 8 bytes of stack at 128
+template <> struct MlpRegisterException<Tag<1, 1, 2>, 64> : MlpException<kFormAll, 12> {};                // 8 at 128
+template <> struct MlpRegisterException<Tag<2, 1, 2>, 64> : MlpException<kFormAll, 12> {};                // 8 at 128
+template <> struct MlpRegisterException<Spread<6>, 64> : MlpException<kFormAll, 8> {};                    // 16 at 168
+template <> struct MlpRegisterException<Spread<6>, 32> : MlpException<kFormAll, 12> {};                   // 48 at 128
+template <> struct MlpRegisterException<Tag<4, 2, 2>, 32> : MlpException<kFormAll, 12> {};                // 16 at 128
+template <> struct MlpRegisterException<Tag<6, 2, 3>, 32> : MlpException<kFormAll, 8> {};                 // 64 at 128, 8 at 168
+template <> struct MlpRegisterException<SpeakerListener, 64> : MlpException<kFormE | kFormCE, 12> {};     // 8 at 128
+template <> struct MlpRegisterException<Adversary<1, 2, 2>, 64> : MlpException<kFormE | kFormCE, 12> {};  // 16 at 128
+template <> struct MlpRegisterException<Reference, 64> : MlpException<kFormE | kFormCE, 8> {};            // 8 at 168
+template <> struct MlpRegisterException<Tag<4, 2, 2>, 64> : MlpException<kFormE | kFormCE, 8> {};         // 8 at 168
+template <> struct MlpRegisterException<Spread<3>, 64> : MlpException<kFormE | kFormC | kFormCE, 12> {};  // 8 at 128
+template <> struct MlpRegisterException<Push<1, 1, 2>, 64> : MlpException<kFormC | kFormCE, 12> {};       // 8 at 128
+template <> struct MlpRegisterException<Crypto, 64> : MlpException<kFormCE, 12> {};                       // 16 at 128
+template <> struct MlpRegisterException<Spread<4>, 64> : MlpException<kFormCE, 8> {};                     // 8 at 168
+template <class P, int H, int FORM>
+__host__ __device__ constexpr int mlp_register_warps() {
+    using X = MlpRegisterException<P, H>;
+    return (X::forms >> FORM & 1) ? X::warps : ((H == 64 && (P::A >= 4 || mlp_max_act_dim<P>() > 8)) ? 12 : 16);
+}
 constexpr int kMlpSmemBytes = 232448;
 template <class P, int H>
 __host__ __device__ constexpr int mlp_smem_warps() {
     return (kMlpSmemBytes / 4 - MlpShape<P, H>::kWeightFloats) / MlpShape<P, H>::kWarpFloats;
 }
-// The episode form (the reset draw and the episode-end stores next to the step's state): the rollout kernel's block,
-// smaller where ptxas -v shows a spill there
-template <class P, int H>
-struct MlpEpisodeRegisterWarps : MlpRegisterWarps<P, H> {};
-template <> struct MlpEpisodeRegisterWarps<Spread<3>, 64> { static constexpr int value = 12; };          // 8 bytes of stack at 128
-template <> struct MlpEpisodeRegisterWarps<SpeakerListener, 64> { static constexpr int value = 12; };    // 8 at 128
-template <> struct MlpEpisodeRegisterWarps<Adversary<1, 2, 2>, 64> { static constexpr int value = 12; }; // 16 at 128
-template <> struct MlpEpisodeRegisterWarps<Reference, 64> { static constexpr int value = 8; };           // 8 at 168
-template <> struct MlpEpisodeRegisterWarps<Tag<4, 2, 2>, 64> { static constexpr int value = 8; };        // 8 at 168
-// The categorical form (the arg-max, the log-probability and the index stores in place of the softmax): the default
-// kernel of the same form's block, smaller where ptxas -v shows a spill there
-template <class P, int H, bool EPISODES>
-struct MlpCategoricalRegisterWarps {
-    static constexpr int value = EPISODES ? MlpEpisodeRegisterWarps<P, H>::value : MlpRegisterWarps<P, H>::value;
-};
-template <> struct MlpCategoricalRegisterWarps<Spread<3>, 64, false> { static constexpr int value = 12; };     // 8 bytes of stack at 128
-template <> struct MlpCategoricalRegisterWarps<Push<1, 1, 2>, 64, false> { static constexpr int value = 12; }; // 8 at 128
-template <> struct MlpCategoricalRegisterWarps<Push<1, 1, 2>, 64, true> { static constexpr int value = 12; };  // 8 at 128
-template <> struct MlpCategoricalRegisterWarps<Crypto, 64, true> { static constexpr int value = 12; };         // 16 at 128
-template <> struct MlpCategoricalRegisterWarps<Spread<4>, 64, true> { static constexpr int value = 8; };       // 8 at 168
 template <class P, int H, bool EPISODES = false, bool CATEGORICAL = false>
 __host__ __device__ constexpr int mlp_block_warps() {
-    constexpr int r = CATEGORICAL ? MlpCategoricalRegisterWarps<P, H, EPISODES>::value
-                    : (EPISODES ? MlpEpisodeRegisterWarps<P, H>::value : MlpRegisterWarps<P, H>::value);
-    return r < mlp_smem_warps<P, H>() ? r : mlp_smem_warps<P, H>();
+    constexpr int r = mlp_register_warps<P, H, EPISODES | CATEGORICAL << 1>(), s = mlp_smem_warps<P, H>();
+    return r < s ? r : s;
 }
 // the two programs whose weights fill most of the 227 KB
 static_assert(MlpShape<Spread<6>, 64>::kWeightFloats * 4 == 175296 && MlpShape<Spread<6>, 64>::kWarpFloats * 4 == 6016 &&
@@ -1563,13 +1561,10 @@ struct Program {
     KernelFn hot_dense_fn;   // the same compiled for 80 registers (large batches of programs that fit without spilling)
     void (*policy_fn[2])(PolicyArgs);  // K-step closed-loop rollout, hidden width 32 / 64 (null: not built for this program)
     int policy_weight_floats[2];
-    void (*mlp_fn[2])(MlpPolicyArgs);  // the same with the two-hidden-layer actor on the tensor cores, H = 32 / 64
-    int mlp_weight_floats[2], mlp_warp_floats[2], mlp_warps[2];
-    void (*mlp_episode_fn[2])(MlpEpisodeArgs);   // its episode form (in-kernel reset between episodes)
-    int mlp_episode_warps[2];
-    void (*mlp_cat_fn[2])(MlpCategoricalArgs);                  // the categorical form of both (one-hot actions)
-    void (*mlp_cat_episode_fn[2])(MlpCategoricalEpisodeArgs);
-    int mlp_cat_warps[2], mlp_cat_episode_warps[2];
+    // the same with the two-hidden-layer actor on the tensor cores, by form (episodes | categorical << 1) and H = 32 / 64:
+    // the kernel and its warps per block at most (mlp_block_warps)
+    struct { const void *fn; int warps; } mlp[kMlpForms][2];
+    int mlp_weight_floats[2], mlp_warp_floats[2];
     int mlp_explore_stride;           // Philox blocks per (step, agent) of its exploration noise
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
     int rollout_smem;   // dynamic shared memory per WARP of the rollout kernel
@@ -1577,6 +1572,17 @@ struct Program {
     int obs_dim[kMaxA], act_dim[kMaxA];
     int unread_state_floats;   // state floats per world that this scenario's step never needs (not compulsory traffic)
 };
+
+template <class P, int H>
+static void set_mlp(Program &p, int k) {
+    p.mlp[0][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_rollout_kernel<P, H>), mlp_block_warps<P, H>()};
+    p.mlp[1][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_episode_kernel<P, H>), mlp_block_warps<P, H, true>()};
+    p.mlp[2][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_categorical_kernel<P, H>), mlp_block_warps<P, H, false, true>()};
+    p.mlp[3][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_categorical_episode_kernel<P, H>),
+                   mlp_block_warps<P, H, true, true>()};
+    p.mlp_weight_floats[k] = MlpShape<P, H>::kWeightFloats;
+    p.mlp_warp_floats[k] = MlpShape<P, H>::kWarpFloats;
+}
 
 template <class P>
 static Program make_program() {
@@ -1599,26 +1605,8 @@ static Program make_program() {
         p.policy_weight_floats[1] = PolicyShape<P, 64>::kWeightFloats;
     }
     if constexpr (MlpBuilt<P>::value) {
-        p.mlp_fn[0] = mpe_policy_mlp_rollout_kernel<P, 32>;
-        p.mlp_fn[1] = mpe_policy_mlp_rollout_kernel<P, 64>;
-        p.mlp_weight_floats[0] = MlpShape<P, 32>::kWeightFloats;
-        p.mlp_weight_floats[1] = MlpShape<P, 64>::kWeightFloats;
-        p.mlp_warp_floats[0] = MlpShape<P, 32>::kWarpFloats;
-        p.mlp_warp_floats[1] = MlpShape<P, 64>::kWarpFloats;
-        p.mlp_warps[0] = mlp_block_warps<P, 32>();
-        p.mlp_warps[1] = mlp_block_warps<P, 64>();
-        p.mlp_episode_fn[0] = mpe_policy_mlp_episode_kernel<P, 32>;
-        p.mlp_episode_fn[1] = mpe_policy_mlp_episode_kernel<P, 64>;
-        p.mlp_episode_warps[0] = mlp_block_warps<P, 32, true>();
-        p.mlp_episode_warps[1] = mlp_block_warps<P, 64, true>();
-        p.mlp_cat_fn[0] = mpe_policy_mlp_categorical_kernel<P, 32>;
-        p.mlp_cat_fn[1] = mpe_policy_mlp_categorical_kernel<P, 64>;
-        p.mlp_cat_warps[0] = mlp_block_warps<P, 32, false, true>();
-        p.mlp_cat_warps[1] = mlp_block_warps<P, 64, false, true>();
-        p.mlp_cat_episode_fn[0] = mpe_policy_mlp_categorical_episode_kernel<P, 32>;
-        p.mlp_cat_episode_fn[1] = mpe_policy_mlp_categorical_episode_kernel<P, 64>;
-        p.mlp_cat_episode_warps[0] = mlp_block_warps<P, 32, true, true>();
-        p.mlp_cat_episode_warps[1] = mlp_block_warps<P, 64, true, true>();
+        set_mlp<P, 32>(p, 0);
+        set_mlp<P, 64>(p, 1);
         p.mlp_explore_stride = mlp_explore_stride<P>();
     }
     p.smem_bytes = Shape<P>::kWarpBytes;  // per warp
@@ -1751,21 +1739,11 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
             if (prog->policy_fn[k])
                 CUDA_TRY(cudaFuncSetAttribute(prog->policy_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               prog->policy_weight_floats[k] * 4 + prog->smem_bytes * 4));
-        for (int k = 0; k < 2; ++k)
-            if (prog->mlp_fn[k])
-                CUDA_TRY(cudaFuncSetAttribute(prog->mlp_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp_warps[k]) * 4));
-        for (int k = 0; k < 2; ++k)
-            if (prog->mlp_episode_fn[k])
-                CUDA_TRY(cudaFuncSetAttribute(prog->mlp_episode_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp_episode_warps[k]) * 4));
-        for (int k = 0; k < 2; ++k)
-            if (prog->mlp_cat_fn[k]) {
-                CUDA_TRY(cudaFuncSetAttribute(prog->mlp_cat_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp_cat_warps[k]) * 4));
-                CUDA_TRY(cudaFuncSetAttribute(prog->mlp_cat_episode_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp_cat_episode_warps[k]) * 4));
-            }
+        for (int f = 0; f < kMlpForms; ++f)
+            for (int k = 0; k < 2; ++k)
+                if (prog->mlp[f][k].fn)
+                    CUDA_TRY(cudaFuncSetAttribute(prog->mlp[f][k].fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp[f][k].warps) * 4));
         if (prog->rollout_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->rollout_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->rollout_smem * max_warps_per_block(prog->rollout_smem)));
@@ -2116,83 +2094,107 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
                          stream, params, false, "cudaLaunchKernelExC(rollout_policy)");
 }
 
-// the categorical form's records (cat != null; then act_record_n is null) after the checks both forms share
-static int fill_categorical(const mpe_env *h, MlpCategoricalRecords &c, int32_t *const *act_index_record_n, float *logp_steps) {
-    if (logp_steps != nullptr && !ok4(logp_steps)) return MPE_ERR_BAD_ARG;
-    c.logp = logp_steps;
-    for (int i = 0; i < h->prog->A; ++i) {
-        c.index[i] = act_index_record_n ? act_index_record_n[i] : nullptr;
-        if (c.index[i] != nullptr && !ok4(c.index[i])) return MPE_ERR_BAD_ARG;
-    }
-    return MPE_OK;
-}
+// The arguments of the four two-hidden-layer rollout entry points, filled by name (several neighbours share a type).
+// form: episodes | categorical << 1.  T is the episode length (n_steps in the single-episode forms); a record the form
+// does not have is null.
+struct MlpCall {
+    int form;
+    void *pv;
+    const void *lm;                   // writable in the episode forms: every episode end redraws them
+    float *comm;
+    const int32_t *goal;
+    const float *const *w[6];         // W1, b1, W2, b2, W3, b3: one pointer per agent each
+    int32_t hidden, T, episodes, explore;
+    uint64_t explore_seed, explore_epoch, reset_seed, reset_epoch, world_offset;
+    float *const *obs_n;
+    float *rew, *rew_steps, *logp_steps;
+    float *const *act_record_n;
+    int32_t *const *act_index_record_n;
+    float *const *obs_record_n, *const *final_obs_record_n;
+    uint8_t *done;
+    uint32_t flags;
+    void *stream;
+};
 
-// mpe_rollout_policy_mlp (categorical = false) and mpe_rollout_policy_mlp_categorical (act_record_n null)
-static int rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
-                              const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
-                              const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
-                              int32_t hidden, int32_t n_steps, int32_t explore, uint64_t explore_seed,
-                              uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n, float *rew_sum,
-                              float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
-                              uint8_t *done, uint32_t flags, void *stream, bool categorical,
-                              int32_t *const *act_index_record_n, float *logp_steps) {
-    if (!h || n_steps < 0 || !w1_n || !b1_n || !w2_n || !b2_n || !w3_n || !b3_n) return MPE_ERR_BAD_ARG;
+static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
+    static const char *const kName[kMlpForms][2] = {   // the NVTX range, the launch's error context
+        {"mpe_rollout_policy_mlp", "cudaLaunchKernelExC(rollout_policy_mlp)"},
+        {"mpe_rollout_policy_mlp_episodes", "cudaLaunchKernelExC(rollout_policy_mlp_episodes)"},
+        {"mpe_rollout_policy_mlp_categorical", "cudaLaunchKernelExC(rollout_policy_mlp_categorical)"},
+        {"mpe_rollout_policy_mlp_categorical_episodes", "cudaLaunchKernelExC(rollout_policy_mlp_categorical_episodes)"}};
+    const bool episodes = c.form & 1, categorical = c.form & 2;
+    const bool no_weights = !c.w[0] || !c.w[1] || !c.w[2] || !c.w[3] || !c.w[4] || !c.w[5];
+    // the single-episode forms refuse a negative n_steps and null weight arrays before anything else, the episode forms
+    // after the device, program and length checks
+    if (!h || (!episodes && (c.T < 0 || no_weights))) return MPE_ERR_BAD_ARG;
     if (h->device < 0) return MPE_ERR_NO_DEVICE;
-    const int k = hidden == 32 ? 0 : (hidden == 64 ? 1 : -1);
-    if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM ||
-        (categorical ? reinterpret_cast<const void *>(h->prog->mlp_cat_fn[k]) : reinterpret_cast<const void *>(h->prog->mlp_fn[k])) == nullptr)
-        return MPE_ERR_UNSUPPORTED;
-    if (flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
-    if (rew_steps != nullptr && !ok4(rew_steps)) return MPE_ERR_BAD_ARG;
-    // the Philox counter word holds (t * A + i) * S + b below the tag bit
-    if (explore && static_cast<int64_t>(n_steps) * h->prog->A * h->prog->mlp_explore_stride > static_cast<int64_t>(kExploreTag))
+    const int k = c.hidden == 32 ? 0 : (c.hidden == 64 ? 1 : -1);
+    if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || h->prog->mlp[c.form][k].fn == nullptr) return MPE_ERR_UNSUPPORTED;
+    if (c.flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
+    // records are indexed by the global step e * episode_length + t, an int
+    if (episodes && (c.T < 1 || c.episodes < 1 || static_cast<int64_t>(c.T) * c.episodes > 0x7fffffffLL))
         return MPE_ERR_BAD_ARG;
-    NvtxRange range(categorical ? "mpe_rollout_policy_mlp_categorical" : "mpe_rollout_policy_mlp");
-    MlpCategoricalArgs ca{};
+    // the Philox counter word holds (t * A + i) * S + b below the tag bit; t restarts at 0 every episode
+    if (c.explore && static_cast<int64_t>(c.T) * h->prog->A * h->prog->mlp_explore_stride > static_cast<int64_t>(kExploreTag))
+        return MPE_ERR_BAD_ARG;
+    if (no_weights || (c.rew_steps != nullptr && !ok4(c.rew_steps))) return MPE_ERR_BAD_ARG;
+    NvtxRange range(kName[c.form][0]);
+    MlpCategoricalRecords cr{};
     if (categorical) {
-        const int rc = fill_categorical(h, ca.c, act_index_record_n, logp_steps);
-        if (rc) return rc;
+        if (c.logp_steps != nullptr && !ok4(c.logp_steps)) return MPE_ERR_BAD_ARG;
+        cr.logp = c.logp_steps;
+        for (int i = 0; i < h->prog->A; ++i) {
+            cr.index[i] = c.act_index_record_n ? c.act_index_record_n[i] : nullptr;
+            if (cr.index[i] != nullptr && !ok4(cr.index[i])) return MPE_ERR_BAD_ARG;
+        }
     }
-    MlpPolicyArgs &pa = ca.p;
+    MlpEpisodeArgs ea{};
+    MlpPolicyArgs &pa = ea.p;
     StepArgs &a = pa.s;
-    int r = fill_state(h, a, pv, lm, comm, goal);
+    int r = fill_state(h, a, c.pv, c.lm, c.comm, c.goal);
     if (r) return r;
-    r = fill_outputs(h, a, obs_n, rew_sum, done, nullptr);
+    r = fill_outputs(h, a, c.obs_n, c.rew, c.done, nullptr);
     if (r) return r;
     for (int i = 0; i < h->prog->A; ++i) {
-        if (!ok4(w1_n[i]) || !ok4(b1_n[i]) || !ok4(w2_n[i]) || !ok4(b2_n[i]) || !ok4(w3_n[i]) || !ok4(b3_n[i]))
-            return MPE_ERR_BAD_ARG;
-        pa.w1[i] = w1_n[i]; pa.b1[i] = b1_n[i]; pa.w2[i] = w2_n[i]; pa.b2[i] = b2_n[i]; pa.w3[i] = w3_n[i]; pa.b3[i] = b3_n[i];
-        pa.act_rec[i] = act_record_n ? act_record_n[i] : nullptr;
+        for (int j = 0; j < 6; ++j)
+            if (!ok4(c.w[j][i])) return MPE_ERR_BAD_ARG;
+        pa.w1[i] = c.w[0][i]; pa.b1[i] = c.w[1][i]; pa.w2[i] = c.w[2][i]; pa.b2[i] = c.w[3][i]; pa.w3[i] = c.w[4][i]; pa.b3[i] = c.w[5][i];
+        pa.act_rec[i] = c.act_record_n ? c.act_record_n[i] : nullptr;
         if (pa.act_rec[i] != nullptr && !ok4(pa.act_rec[i])) return MPE_ERR_BAD_ARG;
-        pa.obs_rec[i] = obs_record_n ? obs_record_n[i] : nullptr;
+        pa.obs_rec[i] = c.obs_record_n ? c.obs_record_n[i] : nullptr;
         if (pa.obs_rec[i] != nullptr && !ok16(pa.obs_rec[i])) return MPE_ERR_BAD_ARG;   // 16-byte tile stores
+        ea.final_obs[i] = c.final_obs_record_n ? c.final_obs_record_n[i] : nullptr;
+        if (c.final_obs_record_n != nullptr && !ok16(ea.final_obs[i])) return MPE_ERR_BAD_ARG;   // every agent's, or none
     }
     a.info = nullptr;
-    a.flags = flags;
+    a.flags = c.flags;
     a.d = h->dev;
     a.n = h->n;
     a.begin = 0;
     a.count = h->n;
-    pa.T = n_steps;
-    pa.explore = explore ? 1 : 0;
-    pa.seed = explore_seed;
-    pa.epoch = explore_epoch;
-    pa.world_offset = world_offset;
-    pa.rew_steps = rew_steps;
+    pa.T = c.T;
+    pa.explore = c.explore ? 1 : 0;
+    pa.seed = c.explore_seed;
+    pa.epoch = c.explore_epoch;
+    pa.world_offset = c.world_offset;
+    pa.rew_steps = c.rew_steps;
+    ea.lm = static_cast<float2 *>(const_cast<void *>(c.lm));
+    ea.goal = const_cast<int32_t *>(c.goal);
+    ea.episodes = c.episodes;
+    ea.reset_seed = c.reset_seed;
+    ea.reset_epoch = c.reset_epoch;
+    MlpCategoricalArgs ca{pa, cr};
+    MlpCategoricalEpisodeArgs cea{ea, cr};
+    void *const form_args[kMlpForms] = {&pa, &ea, &ca, &cea};
     // every block stages all agents' weights once, so blocks are as large as possible while every SM still gets work
     const int64_t warps = (h->n + 31) / 32;
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
-    const int cap = categorical ? h->prog->mlp_cat_warps[k] : h->prog->mlp_warps[k];
-    if (wpb > cap) wpb = cap;
-    void *params[] = {categorical ? static_cast<void *>(&ca) : static_cast<void *>(&pa)};
+    if (wpb > h->prog->mlp[c.form][k].warps) wpb = h->prog->mlp[c.form][k].warps;
+    void *params[] = {form_args[c.form]};
     const size_t smem = (static_cast<size_t>(h->prog->mlp_weight_floats[k]) + static_cast<size_t>(h->prog->mlp_warp_floats[k]) * wpb) * 4;
-    return launch_kernel(h, categorical ? reinterpret_cast<const void *>(h->prog->mlp_cat_fn[k])
-                                        : reinterpret_cast<const void *>(h->prog->mlp_fn[k]),
-                         (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb), smem, stream, params, false,
-                         categorical ? "cudaLaunchKernelExC(rollout_policy_mlp_categorical)"
-                                     : "cudaLaunchKernelExC(rollout_policy_mlp)");
+    return launch_kernel(h, h->prog->mlp[c.form][k].fn, (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb), smem, c.stream,
+                         params, false, kName[c.form][1]);
 }
 
 extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
@@ -2202,9 +2204,33 @@ extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, fl
                                       uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n, float *rew_sum,
                                       float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
                                       uint8_t *done, uint32_t flags, void *stream) {
-    return rollout_policy_mlp(h, pv, lm, comm, goal, w1_n, b1_n, w2_n, b2_n, w3_n, b3_n, hidden, n_steps, explore,
-                              explore_seed, explore_epoch, world_offset, obs_n, rew_sum, rew_steps, act_record_n,
-                              obs_record_n, done, flags, stream, false, nullptr, nullptr);
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.w[0] = w1_n; c.w[1] = b1_n; c.w[2] = w2_n; c.w[3] = b2_n; c.w[4] = w3_n; c.w[5] = b3_n;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = 0; c.T = n_steps; c.episodes = 1; c.rew = rew_sum; c.act_record_n = act_record_n;
+    return rollout_policy_mlp(h, c);
+}
+
+extern "C" int mpe_rollout_policy_mlp_episodes(mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal,
+                                               const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
+                                               const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
+                                               int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
+                                               uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed,
+                                               uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew,
+                                               float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
+                                               float *const *final_obs_record_n, uint8_t *done, uint32_t flags, void *stream) {
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.w[0] = w1_n; c.w[1] = b1_n; c.w[2] = w2_n; c.w[3] = b2_n; c.w[4] = w3_n; c.w[5] = b3_n;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = 1; c.T = episode_length; c.episodes = n_episodes; c.rew = ep_rew; c.act_record_n = act_record_n;
+    c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
+    return rollout_policy_mlp(h, c);
 }
 
 extern "C" int mpe_rollout_policy_mlp_categorical(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
@@ -2216,105 +2242,15 @@ extern "C" int mpe_rollout_policy_mlp_categorical(mpe_handle h, void *pv, const 
                                                   float *rew_sum, float *rew_steps, float *logp_steps,
                                                   int32_t *const *act_index_record_n, float *const *obs_record_n,
                                                   uint8_t *done, uint32_t flags, void *stream) {
-    return rollout_policy_mlp(h, pv, lm, comm, goal, w1_n, b1_n, w2_n, b2_n, w3_n, b3_n, hidden, n_steps, explore,
-                              explore_seed, explore_epoch, world_offset, obs_n, rew_sum, rew_steps, nullptr,
-                              obs_record_n, done, flags, stream, true, act_index_record_n, logp_steps);
-}
-
-// mpe_rollout_policy_mlp_episodes (categorical = false) and mpe_rollout_policy_mlp_categorical_episodes
-static int rollout_policy_mlp_episodes(mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal,
-                                       const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
-                                       const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
-                                       int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
-                                       uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed,
-                                       uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew,
-                                       float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
-                                       float *const *final_obs_record_n, uint8_t *done, uint32_t flags, void *stream,
-                                       bool categorical, int32_t *const *act_index_record_n, float *logp_steps) {
-    if (!h) return MPE_ERR_BAD_ARG;
-    if (h->device < 0) return MPE_ERR_NO_DEVICE;
-    const int k = hidden == 32 ? 0 : (hidden == 64 ? 1 : -1);
-    if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM ||
-        (categorical ? reinterpret_cast<const void *>(h->prog->mlp_cat_episode_fn[k])
-                     : reinterpret_cast<const void *>(h->prog->mlp_episode_fn[k])) == nullptr)
-        return MPE_ERR_UNSUPPORTED;
-    if (flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
-    // records are indexed by the global step e * episode_length + t, an int
-    if (episode_length < 1 || n_episodes < 1 || static_cast<int64_t>(episode_length) * n_episodes > 0x7fffffffLL)
-        return MPE_ERR_BAD_ARG;
-    // the Philox counter word holds (t * A + i) * S + b below the tag bit; t restarts at 0 every episode
-    if (explore && static_cast<int64_t>(episode_length) * h->prog->A * h->prog->mlp_explore_stride > static_cast<int64_t>(kExploreTag))
-        return MPE_ERR_BAD_ARG;
-    if (!w1_n || !b1_n || !w2_n || !b2_n || !w3_n || !b3_n) return MPE_ERR_BAD_ARG;
-    if (rew_steps != nullptr && !ok4(rew_steps)) return MPE_ERR_BAD_ARG;
-    NvtxRange range(categorical ? "mpe_rollout_policy_mlp_categorical_episodes" : "mpe_rollout_policy_mlp_episodes");
-    MlpCategoricalEpisodeArgs ca{};
-    if (categorical) {
-        const int rc = fill_categorical(h, ca.c, act_index_record_n, logp_steps);
-        if (rc) return rc;
-    }
-    MlpEpisodeArgs &ea = ca.e;
-    MlpPolicyArgs &pa = ea.p;
-    StepArgs &a = pa.s;
-    int r = fill_state(h, a, pv, lm, comm, goal);
-    if (r) return r;
-    r = fill_outputs(h, a, obs_n, ep_rew, done, nullptr);
-    if (r) return r;
-    for (int i = 0; i < h->prog->A; ++i) {
-        if (!ok4(w1_n[i]) || !ok4(b1_n[i]) || !ok4(w2_n[i]) || !ok4(b2_n[i]) || !ok4(w3_n[i]) || !ok4(b3_n[i]))
-            return MPE_ERR_BAD_ARG;
-        pa.w1[i] = w1_n[i]; pa.b1[i] = b1_n[i]; pa.w2[i] = w2_n[i]; pa.b2[i] = b2_n[i]; pa.w3[i] = w3_n[i]; pa.b3[i] = b3_n[i];
-        pa.act_rec[i] = act_record_n ? act_record_n[i] : nullptr;
-        if (pa.act_rec[i] != nullptr && !ok4(pa.act_rec[i])) return MPE_ERR_BAD_ARG;
-        pa.obs_rec[i] = obs_record_n ? obs_record_n[i] : nullptr;
-        if (pa.obs_rec[i] != nullptr && !ok16(pa.obs_rec[i])) return MPE_ERR_BAD_ARG;   // 16-byte tile stores
-        ea.final_obs[i] = final_obs_record_n ? final_obs_record_n[i] : nullptr;
-        if (final_obs_record_n != nullptr && !ok16(ea.final_obs[i])) return MPE_ERR_BAD_ARG;   // every agent's, or none
-    }
-    a.info = nullptr;
-    a.flags = flags;
-    a.d = h->dev;
-    a.n = h->n;
-    a.begin = 0;
-    a.count = h->n;
-    pa.T = episode_length;
-    pa.explore = explore ? 1 : 0;
-    pa.seed = explore_seed;
-    pa.epoch = explore_epoch;
-    pa.world_offset = world_offset;
-    pa.rew_steps = rew_steps;
-    ea.lm = static_cast<float2 *>(lm);
-    ea.goal = goal;
-    ea.episodes = n_episodes;
-    ea.reset_seed = reset_seed;
-    ea.reset_epoch = reset_epoch;
-    // the launch geometry of mpe_rollout_policy_mlp with the episode form's block cap
-    const int64_t warps = (h->n + 31) / 32;
-    int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
-    if (wpb < 1) wpb = 1;
-    const int cap = categorical ? h->prog->mlp_cat_episode_warps[k] : h->prog->mlp_episode_warps[k];
-    if (wpb > cap) wpb = cap;
-    void *params[] = {categorical ? static_cast<void *>(&ca) : static_cast<void *>(&ea)};
-    const size_t smem = (static_cast<size_t>(h->prog->mlp_weight_floats[k]) + static_cast<size_t>(h->prog->mlp_warp_floats[k]) * wpb) * 4;
-    return launch_kernel(h, categorical ? reinterpret_cast<const void *>(h->prog->mlp_cat_episode_fn[k])
-                                        : reinterpret_cast<const void *>(h->prog->mlp_episode_fn[k]),
-                         (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb), smem, stream, params, false,
-                         categorical ? "cudaLaunchKernelExC(rollout_policy_mlp_categorical_episodes)"
-                                     : "cudaLaunchKernelExC(rollout_policy_mlp_episodes)");
-}
-
-extern "C" int mpe_rollout_policy_mlp_episodes(mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal,
-                                               const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
-                                               const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
-                                               int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
-                                               uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed,
-                                               uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew,
-                                               float *rew_steps, float *const *act_record_n, float *const *obs_record_n,
-                                               float *const *final_obs_record_n, uint8_t *done, uint32_t flags, void *stream) {
-    return rollout_policy_mlp_episodes(h, pv, lm, comm, goal, w1_n, b1_n, w2_n, b2_n, w3_n, b3_n, hidden, episode_length,
-                                       n_episodes, explore, explore_seed, explore_epoch, reset_seed, reset_epoch,
-                                       world_offset, obs_n, ep_rew, rew_steps, act_record_n, obs_record_n,
-                                       final_obs_record_n, done, flags, stream, false, nullptr, nullptr);
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.w[0] = w1_n; c.w[1] = b1_n; c.w[2] = w2_n; c.w[3] = b2_n; c.w[4] = w3_n; c.w[5] = b3_n;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = 2; c.T = n_steps; c.episodes = 1; c.rew = rew_sum;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    return rollout_policy_mlp(h, c);
 }
 
 extern "C" int mpe_rollout_policy_mlp_categorical_episodes(
@@ -2324,10 +2260,16 @@ extern "C" int mpe_rollout_policy_mlp_categorical_episodes(
     uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew, float *rew_steps,
     float *logp_steps, int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n,
     uint8_t *done, uint32_t flags, void *stream) {
-    return rollout_policy_mlp_episodes(h, pv, lm, comm, goal, w1_n, b1_n, w2_n, b2_n, w3_n, b3_n, hidden, episode_length,
-                                       n_episodes, explore, explore_seed, explore_epoch, reset_seed, reset_epoch,
-                                       world_offset, obs_n, ep_rew, rew_steps, nullptr, obs_record_n, final_obs_record_n,
-                                       done, flags, stream, true, act_index_record_n, logp_steps);
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.w[0] = w1_n; c.w[1] = b1_n; c.w[2] = w2_n; c.w[3] = b2_n; c.w[4] = w3_n; c.w[5] = b3_n;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = 3; c.T = episode_length; c.episodes = n_episodes; c.rew = ep_rew;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
+    return rollout_policy_mlp(h, c);
 }
 
 // adjacent (dst, src, bytes) copies with equal small gaps on both sides are issued as one DMA

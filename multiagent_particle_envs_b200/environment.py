@@ -382,24 +382,18 @@ class MultiAgentEnv(_Env):
         extras = {"actions": actions, "rewards": rew_steps, "observations": observations}
         if categorical:
             extras["log_probs"] = log_probs
-        if episode_length is None:
-            E = 1
-            if categorical:
-                nw.rollout_policy_mlp_categorical(w_ptrs, hidden, T, out, self._flags(), rew_steps, log_probs, act_ptrs,
-                                                  obs_ptrs, explore_seed=seed, explore_epoch=self.explore_epoch)
-            else:
-                nw.rollout_policy_mlp(w_ptrs, hidden, T, out, self._flags(), rew_steps, act_ptrs, obs_ptrs,
-                                      explore_seed=seed, explore_epoch=self.explore_epoch)
-            reward_n = list(out.rew_list)
-        else:
-            L = int(episode_length)
-            E = T // L
+        E, ep_rew, final = 1, None, None
+        if episode_length is not None:
+            E = T // int(episode_length)
             ep_rew = torch.empty((E, self.n, N), **dev)
             final = [torch.empty((E, N, od), **dev) for od in nw.obs_dims] if record_observations else None
-            nw.rollout_policy_mlp_episodes(w_ptrs, hidden, L, E, out, ep_rew, self._flags(), rew_steps, act_ptrs, obs_ptrs,
-                                           _lib.ptr_array([o.data_ptr() for o in final]) if final is not None else None,
-                                           explore_seed=seed, explore_epoch=self.explore_epoch, categorical=categorical,
-                                           logp_steps=log_probs)
+        nw.rollout_policy_mlp(w_ptrs, hidden, T, out, self._flags(), episode_length=episode_length, categorical=categorical,
+                              rew_steps=rew_steps, act_rec_ptrs=act_ptrs, obs_rec_ptrs=obs_ptrs,
+                              final_obs_ptrs=_lib.ptr_array([o.data_ptr() for o in final]) if final is not None else None,
+                              logp_steps=log_probs, ep_rew=ep_rew, explore_seed=seed, explore_epoch=self.explore_epoch)
+        if episode_length is None:
+            reward_n = list(out.rew_list)
+        else:
             reward_n = list(ep_rew.unbind(1))
             extras["final_observations"] = final
         if seed is not None:

@@ -282,65 +282,49 @@ class NativeWorld(ShapeHandle):
         if rc == _lib.ERR_UNSUPPORTED:
             check(rc, "mpe_rollout_policy_mlp")
 
-    def rollout_policy_mlp(self, w_ptrs, hidden, n_steps, out=None, flags=0, rew_steps=None, act_rec_ptrs=None,
-                           obs_rec_ptrs=None, explore_seed=None, explore_epoch=0):
+    def rollout_policy_mlp(self, w_ptrs, hidden, n_steps, out=None, flags=0, *, episode_length=None, categorical=False,
+                           rew_steps=None, act_rec_ptrs=None, obs_rec_ptrs=None, final_obs_ptrs=None, logp_steps=None,
+                           ep_rew=None, explore_seed=None, explore_epoch=0):
         """n_steps fused steps in ONE launch with every agent's two-hidden-layer actor evaluated on the tensor cores
         (mpe_rollout_policy_mlp); w_ptrs: the six pointer arrays (W1, b1, W2, b2, W3, b3), one device pointer per
-        agent each.  explore_seed (not None) switches the Gumbel-softmax sampling on."""
-        out = out or self.out
-        pv, lm, comm, goal = self._state_ptrs()
-        explore = explore_seed is not None
-        check(self.lib.mpe_rollout_policy_mlp(self.handle, pv, lm, comm, goal, *w_ptrs, int(hidden), int(n_steps),
-                                              int(explore), int(explore_seed) if explore else 0, int(explore_epoch),
-                                              self.world_offset, out.obs_ptrs, out.rew_ptr,
-                                              rew_steps.data_ptr() if rew_steps is not None else None, act_rec_ptrs,
-                                              obs_rec_ptrs, out.done_ptr, flags, self._stream()), "mpe_rollout_policy_mlp")
-        return out
+        agent each.  explore_seed (not None) switches the Gumbel-softmax sampling on.
 
-    def rollout_policy_mlp_categorical(self, w_ptrs, hidden, n_steps, out=None, flags=0, rew_steps=None, logp_steps=None,
-                                       index_rec_ptrs=None, obs_rec_ptrs=None, explore_seed=None, explore_epoch=0):
-        """rollout_policy_mlp with categorical actions (mpe_rollout_policy_mlp_categorical): every agent applies the
-        one-hot vector of the arg-max per sub-space, of the Gumbel-perturbed logits when explore_seed is not None.
-        index_rec_ptrs: one int32 [n_steps, N, n_sub_i] pointer per agent; logp_steps: float32 [n_steps, A, N]."""
-        out = out or self.out
-        pv, lm, comm, goal = self._state_ptrs()
-        explore = explore_seed is not None
-        check(self.lib.mpe_rollout_policy_mlp_categorical(
-            self.handle, pv, lm, comm, goal, *w_ptrs, int(hidden), int(n_steps), int(explore),
-            int(explore_seed) if explore else 0, int(explore_epoch), self.world_offset, out.obs_ptrs, out.rew_ptr,
-            rew_steps.data_ptr() if rew_steps is not None else None,
-            logp_steps.data_ptr() if logp_steps is not None else None, index_rec_ptrs, obs_rec_ptrs, out.done_ptr, flags,
-            self._stream()), "mpe_rollout_policy_mlp_categorical")
-        return out
+        categorical=True (mpe_rollout_policy_mlp_categorical): every agent applies the one-hot vector of the arg-max per
+        sub-space, of the Gumbel-perturbed logits when exploring; act_rec_ptrs then holds one int32 [n_steps, N, n_sub_i]
+        index record per agent, and logp_steps (float32 [n_steps, A, N]) receives the log-probabilities.
 
-    def rollout_policy_mlp_episodes(self, w_ptrs, hidden, episode_length, n_episodes, out, ep_rew, flags=0,
-                                    rew_steps=None, act_rec_ptrs=None, obs_rec_ptrs=None, final_obs_ptrs=None,
-                                    explore_seed=None, explore_epoch=0, categorical=False, logp_steps=None):
-        """n_episodes episodes of episode_length steps in ONE launch (mpe_rollout_policy_mlp_episodes): rollout_policy_mlp
-        per episode, and after each episode the reset that `reset()` would draw, inside the kernel.  The resets use the
-        epochs `reset()` would use next, and self.epoch (and the device epoch, if enabled) advances by n_episodes.
-        ep_rew: float32 [n_episodes, A, N] CUDA tensor receiving each episode's returns; out.obs receives the observations
-        of the state after the last reset.  categorical=True: mpe_rollout_policy_mlp_categorical_episodes, with
-        act_rec_ptrs the int32 index records and logp_steps the float32 [n_steps, A, N] log-probabilities."""
-        if self.torch.cuda.is_current_stream_capturing():
+        episode_length=L (mpe_rollout_policy_mlp[_categorical]_episodes): n_steps / L episodes, and after each episode
+        the reset that `reset()` would draw, inside the kernel.  The resets use the epochs `reset()` would use next, and
+        self.epoch (and the device epoch, if enabled) advances by the number of episodes.  ep_rew: float32 [episodes, A,
+        N] CUDA tensor receiving each episode's returns; out.obs receives the observations of the state after the last
+        reset; final_obs_ptrs: one [episodes, N, obs_dim_i] record per agent of each episode's last observation."""
+        out = out or self.out
+        episodes = episode_length is not None
+        if episodes and self.torch.cuda.is_current_stream_capturing():
             raise RuntimeError("rollout_policy with episode_length cannot be captured in a CUDA graph: the reset epoch "
                                "is a launch argument")
         pv, lm, comm, goal = self._state_ptrs()
-        epoch = int(self._epoch_dev.item()) if self._epoch_dev is not None else self.epoch
         explore = explore_seed is not None
-        head = (self.handle, pv, lm, comm, goal, *w_ptrs, int(hidden), int(episode_length), int(n_episodes), int(explore),
-                int(explore_seed) if explore else 0, int(explore_epoch), self.seed, epoch, self.world_offset, out.obs_ptrs,
-                ep_rew.data_ptr(), rew_steps.data_ptr() if rew_steps is not None else None)
-        tail = (act_rec_ptrs, obs_rec_ptrs, final_obs_ptrs, out.done_ptr, flags, self._stream())
-        if categorical:
-            check(self.lib.mpe_rollout_policy_mlp_categorical_episodes(
-                *head, logp_steps.data_ptr() if logp_steps is not None else None, *tail),
-                "mpe_rollout_policy_mlp_categorical_episodes")
+        explore_args = (int(explore), int(explore_seed) if explore else 0, int(explore_epoch))
+        rew_ptr = rew_steps.data_ptr() if rew_steps is not None else None
+        logp = (logp_steps.data_ptr() if logp_steps is not None else None,) if categorical else ()
+        name = "mpe_rollout_policy_mlp" + ("_categorical" if categorical else "") + ("_episodes" if episodes else "")
+        if episodes:
+            epoch = int(self._epoch_dev.item()) if self._epoch_dev is not None else self.epoch
+            n_episodes = int(n_steps) // int(episode_length)
+            rc = getattr(self.lib, name)(self.handle, pv, lm, comm, goal, *w_ptrs, int(hidden), int(episode_length),
+                                         n_episodes, *explore_args, self.seed, epoch, self.world_offset, out.obs_ptrs,
+                                         ep_rew.data_ptr(), rew_ptr, *logp, act_rec_ptrs, obs_rec_ptrs, final_obs_ptrs,
+                                         out.done_ptr, flags, self._stream())
         else:
-            check(self.lib.mpe_rollout_policy_mlp_episodes(*head, *tail), "mpe_rollout_policy_mlp_episodes")
-        self.epoch = epoch + int(n_episodes)
-        if self._epoch_dev is not None:
-            self._epoch_dev.fill_(self.epoch)
+            rc = getattr(self.lib, name)(self.handle, pv, lm, comm, goal, *w_ptrs, int(hidden), int(n_steps), *explore_args,
+                                         self.world_offset, out.obs_ptrs, out.rew_ptr, rew_ptr, *logp, act_rec_ptrs,
+                                         obs_rec_ptrs, out.done_ptr, flags, self._stream())
+        check(rc, name)
+        if episodes:
+            self.epoch = epoch + n_episodes
+            if self._epoch_dev is not None:
+                self._epoch_dev.fill_(self.epoch)
         return out
 
     # ---- host callers (what the reference's callers hold: NumPy arrays) -----------------------

@@ -103,26 +103,22 @@ def random_actions(act_dims, n, rng, temperature=2.0, movable=None):
 
 # ---- launch shapes: which block size the library picks for a batch ----------------------------------
 # Mirrors of the launch-shape rules in multiagent_particle_envs_b200/csrc/mpe_kernels.cu (sms = the device's SM count):
-#   "step"   launch() -> launch_grid (~l.1954): the fused step runs whole 32-world tiles on the HOT kernel -- 1 warp per
+#   "step"   launch() -> launch_grid: the fused step runs whole 32-world tiles on the HOT kernel -- 1 warp per
 #            block up to 16*sms tiles, 2 up to 64*sms, else 4 -- and the ragged tail (< 32 worlds) on the general kernel
-#            at begin = whole tiles, in one 1-warp block (~l.1982-1993).  Above 16*sms tiles the programs with a
-#            hot_dense_fn take that 80-register build instead of hot_fn (~l.1987); make_program (~l.1563) builds it
+#            at begin = whole tiles, in one 1-warp block (launch()).  Above 16*sms tiles the programs with a
+#            hot_dense_fn take that 80-register build instead of hot_fn (launch()); make_program builds it
 #            where kLowRegVariant holds: tag with 3 to 6 agents and spread N=4 (csrc/mpe_scenarios.cuh ~l.96, ~l.173).
-#   "rollout" mpe_rollout (~l.2116): 1 warp per block up to 4*sms warps, 2 up to 64*sms, else 4
-#   "policy"  mpe_rollout_policy (~l.2166): 1 up to 16*sms warps, 2 up to 64*sms, else 4
-#   "mlp"     mpe_rollout_policy_mlp (~l.2227-2229): ceil(warps / sms) warps per block, capped at mlp_block_warps
-#            (~l.1026: 12 for H = 64 with four or more agents, else 16)
-# The shared-memory caps (max_warps_per_block, ~l.1647) never bind for the built-in scenarios at 4 warps per block.
+#   "rollout" mpe_rollout: 1 warp per block up to 4*sms warps, 2 up to 64*sms, else 4
+#   "policy"  mpe_rollout_policy: 1 up to 16*sms warps, 2 up to 64*sms, else 4
+#   "mlp"     rollout_policy_mlp, all four forms: ceil(warps / sms) warps per block, capped at mlp_block_warps
+#            (mirrored by mlp_programs.mlp_block_cap)
+# The shared-memory caps (max_warps_per_block) never bind for the built-in scenarios at 4 warps per block.
 STEP_DENSE_TAGS = ("simple_tag", "simple_tag_2v1", "simple_tag_4v2")    # the test tags with a hot_dense_fn
 
 
 def device_sms():
     import torch
     return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def mlp_block_cap(H, n_agents):
-    return 12 if (H == 64 and n_agents >= 4) else 16
 
 
 def launch_shape(kernel, n, sms, cap=16):

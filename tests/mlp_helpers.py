@@ -1,6 +1,7 @@
 """NumPy models of the two-hidden-layer in-kernel actor (env.rollout_policy with a Linear-ReLU-Linear-ReLU-Linear
-policy): TF32 rounding as cvt.rna.tf32.f32 does it, Philox4x32-10, the Gumbel noise stream, and a float64 evaluation
-of the actor with or without the kernel's operand rounding, and the accounting for its TF32 rounding flips."""
+policy): TF32 rounding as cvt.rna.tf32.f32 does it, Philox4x32-10, the Gumbel noise stream of act_dim logits, a float64
+evaluation of the actor with or without the kernel's operand rounding, one softmax per action sub-space (movement,
+utterance), and the accounting for its TF32 rounding flips."""
 import itertools
 
 import numpy as np
@@ -56,19 +57,21 @@ def uniform_from_bits(bits):
     return (s * 2.0 ** -24).astype(np.float32)
 
 
-def gumbel_noise(seed, epoch, world_index, t, agent, n_agents):
-    """-log(-log u) of the five movement logits of `agent` at step `t` for the given global world indices, float64"""
+def gumbel_noise(seed, epoch, world_index, t, agent, n_agents, n_logits=5, stride=2):
+    """-log(-log u) of the `n_logits` logits of `agent` at step `t` for the given global world indices, float64.  Logit
+    k uses word k mod 4 of Philox block b = k div 4, counter word 3 = EXPLORE_TAG | ((t * n_agents + agent) * stride + b);
+    stride is 2 when every action vector of the scenario has at most 8 entries, else 4.  The defaults are the five
+    movement logits."""
     gw = np.asarray(world_index, dtype=np.uint64)
     key = (seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF)
-    base = EXPLORE_TAG | ((t * n_agents + agent) * 2)
+    base = EXPLORE_TAG | ((t * n_agents + agent) * stride)
     words = []
-    for b in (0, 1):
+    for b in range((n_logits + 3) // 4):
         ctr = np.stack([gw & np.uint64(0xFFFFFFFF), gw >> np.uint64(32), np.full_like(gw, epoch & 0xFFFFFFFF),
                         np.full_like(gw, base | b)], -1)
         words.append(philox4x32_10(ctr, key))
-    bits = np.concatenate([words[0], words[1][:, :1]], 1)
-    u = uniform_from_bits(bits).astype(np.float64)
-    return -np.log(-np.log(u))
+    bits = np.concatenate(words, 1)[:, :n_logits]
+    return -np.log(-np.log(uniform_from_bits(bits).astype(np.float64)))
 
 
 def actor_logits(obs, W1, b1, W2, b2, W3, b3, tf32=True):
@@ -84,6 +87,15 @@ def actor_logits(obs, W1, b1, W2, b2, W3, b3, tf32=True):
 def softmax(z):
     e = np.exp(z - z.max(-1, keepdims=True))
     return e / e.sum(-1, keepdims=True)
+
+
+def segment_softmax(z, segments=None):
+    """one softmax per action sub-space: `segments` lists their widths in order (None: one softmax over the row)"""
+    if segments is None:
+        return softmax(z)
+    assert sum(segments) == z.shape[-1], (segments, z.shape)
+    bounds = np.cumsum([0] + list(segments))
+    return np.concatenate([softmax(z[..., a:b]) for a, b in zip(bounds[:-1], bounds[1:])], -1)
 
 
 # ---- accounting for TF32 rounding flips between the kernel and the float64 actor -------------------------------------
@@ -134,11 +146,12 @@ def tf32_flip_choices(pre, bound):
     return r, alt
 
 
-def explain_tf32_mismatches(actions, obs, params, noise=0.0, atol=1e-5):
-    """Assert that every row of the kernel's `actions` [n, 5] that differs from softmax(actor_logits(obs, *params,
-    tf32=True) + noise) by more than atol is a TF32 rounding flip (see above): it has an ambiguous h1 or h2 unit, and
-    rounding some combination of them the other way brings it within atol.  At most TF32_MAX_COMBOS combinations per
-    row; a row that needs more fails.  Returns the number of explained rows."""
+def explain_tf32_mismatches(actions, obs, params, noise=0.0, atol=1e-5, segments=None):
+    """Assert that every row of the kernel's `actions` [n, act_dim] that differs from segment_softmax(actor_logits(obs,
+    *params, tf32=True) + noise, segments) by more than atol is a TF32 rounding flip (see above): it has an ambiguous h1
+    or h2 unit, and rounding some combination of them the other way brings it within atol.  `segments`: the widths of
+    the action sub-spaces, e.g. [5, 10], each with its own softmax; None: one softmax over the row.  At most
+    TF32_MAX_COMBOS combinations per row; a row that needs more fails.  Returns the number of explained rows."""
     f64 = np.float64
     W1, b1, W2, b2, W3, b3 = [np.asarray(p, dtype=np.float32) for p in params]
     H = W1.shape[0]
@@ -150,7 +163,7 @@ def explain_tf32_mismatches(actions, obs, params, noise=0.0, atol=1e-5):
     p1 = x0 @ t1.T + b1
     h1 = tf32_rna(np.maximum(p1, 0.0).astype(np.float32)).astype(f64)
     h2 = tf32_rna(np.maximum(h1 @ t2.T + b2, 0.0).astype(np.float32)).astype(f64)
-    want = softmax(h2 @ t3.T + b3 + noise)
+    want = segment_softmax(h2 @ t3.T + b3 + noise, segments)
     bad = np.where((np.abs(got - want) > atol).any(-1))[0]
     if bad.size == 0:
         return 0
@@ -164,36 +177,34 @@ def explain_tf32_mismatches(actions, obs, params, noise=0.0, atol=1e-5):
             if f1 not in h2_of:
                 h = h1[w].copy()
                 h[list(f1)] = alt1[r, list(f1)]
-                q = h @ t2.T + b2
-                r2, alt2 = tf32_flip_choices(q, tf32_accumulation_bound(h[None], t2, b2)[0])
+                r2, alt2 = tf32_flip_choices(h @ t2.T + b2, tf32_accumulation_bound(h[None], t2, b2)[0])
                 h2_of[f1] = (r2, alt2, list(np.where(~np.isnan(alt2))[0]))
             return h2_of[f1]
 
+        def candidates():                            # flip sets in order of their size, h1 choices first
+            for nflips in range(1, len(amb1) + H + 1):
+                produced = False
+                for k1 in range(min(nflips, len(amb1)) + 1):
+                    for f1 in itertools.combinations(amb1, k1):
+                        r2, alt2, amb2 = layer2(f1)
+                        for f2 in itertools.combinations(amb2, nflips - k1):
+                            g = r2.copy()
+                            g[list(f2)] = alt2[list(f2)]
+                            produced = True
+                            yield g
+                if not produced:                     # no flip set of this size, hence none larger
+                    return
+
         any_ambiguous = bool(amb1) or bool(layer2(())[2])
-        ok, combos = False, 0
-        for nflips in range(1, len(amb1) + H + 1) if any_ambiguous else ():
-            tried = combos
-            for k1 in range(min(nflips, len(amb1)) + 1):
-                for f1 in itertools.combinations(amb1, k1):
-                    r2, alt2, amb2 = layer2(f1)
-                    for f2 in itertools.combinations(amb2, nflips - k1):
-                        combos += 1
-                        if combos > TF32_MAX_COMBOS:
-                            break
-                        g = r2.copy()
-                        g[list(f2)] = alt2[list(f2)]
-                        ok = bool((np.abs(softmax(g @ t3.T + b3 + noise[w]) - got[w]) <= atol).all())
-                        if ok:
-                            break
-                    if ok or combos > TF32_MAX_COMBOS:
-                        break
-                if ok or combos > TF32_MAX_COMBOS:
+        tried, ok = 0, False
+        if any_ambiguous:
+            for g in itertools.islice(candidates(), TF32_MAX_COMBOS):
+                tried += 1
+                if (np.abs(segment_softmax(g @ t3.T + b3 + noise[w], segments) - got[w]) <= atol).all():
+                    ok = True
                     break
-            if ok or combos > TF32_MAX_COMBOS or combos == tried:
-                break
         if not ok:
-            unexplained.append((int(w), any_ambiguous, min(combos, TF32_MAX_COMBOS + 1),
-                                float(np.abs(got[w] - want[w]).max())))
+            unexplained.append((int(w), any_ambiguous, tried, float(np.abs(got[w] - want[w]).max())))
     assert not unexplained, ("%d of %d rows beyond %g are not TF32 rounding flips (row, has an ambiguous unit, "
                              "combinations tried, max |difference|): %s" % (len(unexplained), bad.size, atol,
                                                                             unexplained[:8]))

@@ -1,0 +1,105 @@
+"""CPU checks that tie the two-hidden-layer actor's host side to the built library: every one of its 136 kernels (17
+programs x H = 32, 64 x four forms) is compiled for the block size the test mirror (mlp_programs.mlp_block_cap)
+expects, read from the kernel's launch bounds in libmpe_b200.so; and the four entry points refuse what they can refuse
+without a device with the return codes they always had."""
+import os
+import re
+import shutil
+import subprocess
+
+import pytest
+
+from helpers import make_product_env
+from mlp_programs import PROGRAMS, mlp_block_cap
+
+pytest.importorskip("torch")
+
+# the program types of csrc/mpe_kernels.cu (make_program), as c++filt prints them
+TYPE_TAGS = {
+    "Simple<1, 1>": "simple", "Spread<2>": "simple_spread_n2", "Spread<3>": "simple_spread_n3",
+    "Spread<4>": "simple_spread_n4", "Spread<5>": "simple_spread_n5", "Spread<6>": "simple_spread_n6",
+    "Tag<3, 1, 2>": "simple_tag", "Tag<1, 1, 2>": "simple_tag_1v1", "Tag<2, 1, 2>": "simple_tag_2v1",
+    "Tag<4, 2, 2>": "simple_tag_4v2", "Tag<6, 2, 3>": "simple_tag_6v2", "Adversary<1, 2, 2>": "simple_adversary",
+    "Adversary<1, 3, 3>": "simple_adversary_n4", "Push<1, 1, 2>": "simple_push",
+    "SpeakerListener": "simple_speaker_listener", "Reference": "simple_reference", "Crypto": "simple_crypto",
+}
+# kernel name -> (episodes, categorical)
+FORMS = {"rollout": (False, False), "episode": (True, False), "categorical": (False, True),
+         "categorical_episode": (True, True)}
+
+
+def cuobjdump():
+    """cuobjdump of the toolkit whose nvcc builds the library (the Makefile's NVCC, else nvcc on PATH)"""
+    nvcc = shutil.which(os.environ.get("NVCC", "nvcc"))
+    for d in ([os.path.dirname(os.path.realpath(nvcc))] if nvcc else []) + \
+            [os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin")]:
+        if os.access(os.path.join(d, "cuobjdump"), os.X_OK):
+            return os.path.join(d, "cuobjdump")
+    pytest.skip("no CUDA toolkit (cuobjdump) to read the library with")
+
+
+def max_threads_per_kernel(lib_path):
+    """mangled kernel name -> EIATTR_MAX_THREADS (x) of its .nv.info section in `cuobjdump -elf`"""
+    text = subprocess.run([cuobjdump(), "-elf", lib_path], capture_output=True, text=True, check=True).stdout
+    out, cur, attr = {}, None, False
+    for ln in text.splitlines():
+        if ln.startswith("."):
+            cur = ln[len(".nv.info."):] if ln.startswith(".nv.info.") else None
+            attr = False
+        elif cur and "Attribute:" in ln:
+            attr = ln.split()[-1] == "EIATTR_MAX_THREADS"
+        elif cur and attr and ln.strip().startswith("Value:"):
+            out[cur] = int(ln.split()[1], 16)
+            attr = False
+    return out
+
+
+def test_launch_bounds_are_the_mirrored_caps():
+    from multiagent_particle_envs_b200 import _lib
+    threads = max_threads_per_kernel(_lib.LIB_PATH)
+    names = list(threads)
+    demangled = subprocess.run(["c++filt"], input="\n".join(names), capture_output=True, text=True,
+                               check=True).stdout.split("\n")
+    seen = {}
+    for mangled, nm in zip(names, demangled):
+        m = re.match(r"void mpe::mpe_policy_mlp_(rollout|episode|categorical|categorical_episode)_kernel<mpe::(.+), "
+                     r"(\d+)>\(", nm)
+        if m:
+            key = (TYPE_TAGS[m.group(2)], int(m.group(3))) + FORMS[m.group(1)]
+            seen[key] = threads[mangled]
+    assert len(seen) == 136 and {k[0] for k in seen} == set(PROGRAMS)
+    want = {(tag, H, e, c): 32 * mlp_block_cap(tag, H, e, c) for tag, H, e, c in seen}
+    assert seen == want
+
+
+# ---- return codes without a device ---------------------------------------------------------------------------------
+ENTRY_POINTS = ("mpe_rollout_policy_mlp", "mpe_rollout_policy_mlp_categorical", "mpe_rollout_policy_mlp_episodes",
+                "mpe_rollout_policy_mlp_categorical_episodes")
+BAD_ARG, NO_DEVICE = -1, -5
+
+
+def _call(name, handle, steps=4, weights=True):
+    """`name` with aligned dummy pointers (every probe returns before one is used), H = 32, `steps` steps (the episode
+    length in the episode forms, of one episode) and null weight arrays unless `weights`"""
+    from multiagent_particle_envs_b200 import _lib
+    lib = _lib.load()
+    argtypes = _lib._SIGNATURES[name][1]
+    per_agent = _lib.ptr_array([256] * _lib.MPE_MAX_AGENTS)
+    args = [256 if t is _lib._P else per_agent if t is _lib._PP else 1 if t.__name__ == "c_int" else 0 for t in argtypes]
+    args[0], args[-1] = handle, None
+    args[5:11] = [per_agent if weights else None] * 6
+    args[11], args[12] = 32, steps
+    return getattr(lib, name)(*args)
+
+
+def test_entry_point_return_codes_without_a_device():
+    """the single-episode forms refuse a negative n_steps and null weight arrays before they ask for the device; the
+    episode forms ask for the device first"""
+    shapes = make_product_env("simple_spread_n3", num_envs=64).world.native_shapes()   # device-less handle
+    handle = shapes.handle          # `shapes` owns it: the handle stays live while the test holds `shapes`
+    for name in ENTRY_POINTS:
+        episodes = name.endswith("_episodes")
+        assert _call(name, None) == BAD_ARG, name
+        assert _call(name, handle, steps=-1) == (NO_DEVICE if episodes else BAD_ARG), name
+        assert _call(name, handle, weights=False) == (NO_DEVICE if episodes else BAD_ARG), name
+        assert _call(name, handle) == NO_DEVICE, name

@@ -7,10 +7,9 @@ import re
 import numpy as np
 import pytest
 
-import mlp_helpers
 from helpers import make_product_env
 from mlp_categorical_helpers import bounds, categorical_pick, log_softmax_at, one_hot
-from mlp_comm_helpers import gumbel_noise, segment_softmax
+from mlp_helpers import EXPLORE_TAG, gumbel_noise, philox4x32_10, segment_softmax, uniform_from_bits
 
 torch = pytest.importorskip("torch")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -45,17 +44,33 @@ def test_log_probability_model_is_scipy_log_softmax(segs):
     np.testing.assert_allclose(log_softmax_at(z, k, segs), want, rtol=0, atol=1e-12)
 
 
+def _five_logit_noise(seed, epoch, world_index, t, agent, n_agents):
+    """the five movement logits' Gumbel noise: u_0..u_3 = words 0-3 of block 0, u_4 = word 0 of block 1, counter
+    (world index low, high, epoch, EXPLORE_TAG | ((t * A + i) * 2 + b)), key (seed low, high)"""
+    gw = np.asarray(world_index, dtype=np.uint64)
+    key = (seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF)
+    word3 = EXPLORE_TAG | ((t * n_agents + agent) * 2)
+    ctr = np.stack([gw & np.uint64(0xFFFFFFFF), gw >> np.uint64(32), np.full_like(gw, epoch & 0xFFFFFFFF),
+                    np.full_like(gw, word3)], -1)
+    block0 = philox4x32_10(ctr, key)
+    ctr[:, 3] = word3 | 1
+    block1 = philox4x32_10(ctr, key)
+    u = uniform_from_bits(np.concatenate([block0, block1[:, :1]], 1)).astype(np.float64)
+    return -np.log(-np.log(u))
+
+
 @pytest.mark.parametrize("segs,stride", [([5], 2), ([3], 2), ([5, 10], 4), ([5, 3], 2)])
 def test_gumbel_argmax_model_is_the_argmax_of_the_gumbel_softmax_sample(segs, stride):
     """categorical_pick(z + g) per sub-space is the arg-max of segment_softmax(z + g), the default mode's sample, with g
-    the exploration stream of mlp_comm_helpers.gumbel_noise (which for five logits is mlp_helpers.gumbel_noise)"""
+    the exploration stream of mlp_helpers.gumbel_noise (for five logits: words 0-3 of Philox block 0 and word 0 of block
+    1, written out below)"""
     n, A = 4096, 3
     rng = np.random.RandomState(2)
     z = rng.randn(n, sum(segs))
     for t, i in ((0, 0), (7, 2)):
         g = gumbel_noise(99, 3, np.arange(n) + 10 ** 6, t, i, A, n_logits=sum(segs), stride=stride)
         if segs == [5]:
-            np.testing.assert_array_equal(g, mlp_helpers.gumbel_noise(99, 3, np.arange(n) + 10 ** 6, t, i, A))
+            np.testing.assert_array_equal(g, _five_logit_noise(99, 3, np.arange(n) + 10 ** 6, t, i, A))
         k = categorical_pick(z + g, segs)
         sample = segment_softmax(z + g, segs)
         for s, (a, b) in enumerate(bounds(segs)):

@@ -6,12 +6,11 @@ import itertools
 import numpy as np
 import pytest
 
-import helpers
 from helpers import make_product_env
-import mlp_comm_helpers
 import mlp_helpers
-from mlp_comm_helpers import gumbel_noise, mlp_block_cap, segment_softmax
-from mlp_helpers import EXPLORE_TAG, philox4x32_10, softmax, tf32_rna, tf32_tie, uniform_from_bits
+from mlp_helpers import (EXPLORE_TAG, explain_tf32_mismatches, gumbel_noise, philox4x32_10, segment_softmax, softmax,
+                         tf32_rna, tf32_tie, uniform_from_bits)
+from mlp_programs import mlp_register_rule
 
 torch = pytest.importorskip("torch")
 
@@ -116,8 +115,8 @@ def test_segmented_accounting_accepts_a_unit_on_a_tf32_midpoint_rounded_the_othe
     want = _actions(obs, params, segs)
     got = _actions(obs, params, segs, h1_override=(5, 0, 1.0))
     assert np.abs(got - want)[5].max() > 1e-4 and np.abs(got - want)[np.arange(32) != 5].max() == 0
-    assert mlp_comm_helpers.explain_tf32_mismatches(got, obs, params, segments=segs) == 1
-    assert mlp_comm_helpers.explain_tf32_mismatches(want, obs, params, segments=segs) == 0
+    assert explain_tf32_mismatches(got, obs, params, segments=segs) == 1
+    assert explain_tf32_mismatches(want, obs, params, segments=segs) == 0
 
 
 def test_segmented_accounting_rejects_one_softmax_over_movement_and_utterance():
@@ -125,26 +124,27 @@ def test_segmented_accounting_rejects_one_softmax_over_movement_and_utterance():
     segs = [5, 10]
     obs, params = _dyadic_actor(np.random.RandomState(2))
     right = _actions(obs, params, segs)
-    assert mlp_comm_helpers.explain_tf32_mismatches(right, obs, params, segments=segs) == 0
+    assert explain_tf32_mismatches(right, obs, params, segments=segs) == 0
     joint = _actions(obs, params, None)
     assert np.abs(joint - right).max() > 1e-2
     with pytest.raises(AssertionError, match="not TF32 rounding flips"):
-        mlp_comm_helpers.explain_tf32_mismatches(joint, obs, params, segments=segs)
+        explain_tf32_mismatches(joint, obs, params, segments=segs)
     # and the unsegmented accounting does not take the segmented actions either
     with pytest.raises(AssertionError, match="not TF32 rounding flips"):
-        mlp_comm_helpers.explain_tf32_mismatches(right, obs, params)
+        explain_tf32_mismatches(right, obs, params)
 
 
 def test_block_cap_for_longer_action_vectors():
-    """the cap mirror with the largest action vector: helpers.mlp_block_cap's answers for 5-entry vectors (simple,
-    spread N=3, tag 3+1), 12 warps for simple_reference's 15-entry vectors at H = 64"""
+    """the general register rule with the largest action vector: 16 warps, or 12 at H = 64 for four or more agents, for
+    5-entry vectors (simple, spread N=3, tag 3+1), 12 warps for simple_reference's 15-entry vectors at H = 64"""
     for H, A in itertools.product((32, 64), (1, 2, 3, 4)):
-        assert mlp_block_cap(H, A) == mlp_block_cap(H, A, 5) == helpers.mlp_block_cap(H, A)
-    assert [mlp_block_cap(64, 1), mlp_block_cap(64, 3), mlp_block_cap(64, 4), mlp_block_cap(32, 4)] == [16, 16, 12, 16]
+        assert mlp_register_rule(H, A) == mlp_register_rule(H, A, 5) == (12 if (H == 64 and A >= 4) else 16)
+    assert [mlp_register_rule(64, 1), mlp_register_rule(64, 3), mlp_register_rule(64, 4), mlp_register_rule(32, 4)] == \
+        [16, 16, 12, 16]
     # simple_speaker_listener (3, 5), simple_crypto (4), simple_adversary / simple_push (5), simple_reference (15)
-    assert [mlp_block_cap(64, 2, 5), mlp_block_cap(64, 3, 4), mlp_block_cap(64, 3, 5), mlp_block_cap(64, 2, 15)] == \
-        [16, 16, 16, 12]
-    assert mlp_block_cap(32, 2, 15) == 16
+    assert [mlp_register_rule(64, 2, 5), mlp_register_rule(64, 3, 4), mlp_register_rule(64, 3, 5),
+            mlp_register_rule(64, 2, 15)] == [16, 16, 16, 12]
+    assert mlp_register_rule(32, 2, 15) == 16
 
 
 def _generic_actor(rng, od=18, H=64):
@@ -155,8 +155,8 @@ def _generic_actor(rng, od=18, H=64):
 
 
 def test_accounting_without_segments_is_the_five_logit_accounting():
-    """with one sub-space the accounting explains exactly the rows mlp_helpers.explain_tf32_mismatches explains, and
-    rejects what it rejects: rows moved by a rounding flip, by an unexplainable nudge and by a wrong, renormalised logit"""
+    """with one sub-space, given as [5] or as None, the accounting explains the same rows and rejects the same rows:
+    rows moved by a rounding flip, by an unexplainable nudge and by a wrong, renormalised logit"""
     obs, params = _generic_actor(np.random.RandomState(5))
     z = mlp_helpers.actor_logits(obs, *params)
     got = softmax(z)
@@ -166,11 +166,11 @@ def test_accounting_without_segments_is_the_five_logit_accounting():
     h1 = tf32_rna(np.maximum(tf32_rna(obs) @ tf32_rna(W1).T + b1, 0).astype(f32))
     h2 = tf32_rna(np.maximum(h1 @ tf32_rna(W2).T + b2, 0).astype(f32))
     fp32 = softmax((h2 @ tf32_rna(W3).T + b3).astype(np.float64))
-    n_ref = mlp_helpers.explain_tf32_mismatches(fp32, obs, params)
+    n_ref = explain_tf32_mismatches(fp32, obs, params)
     assert n_ref > 0
     for acts, n in ((got, 0), (fp32, n_ref)):
-        assert mlp_comm_helpers.explain_tf32_mismatches(acts, obs, params) == n
-        assert mlp_comm_helpers.explain_tf32_mismatches(acts, obs, params, segments=[5]) == n
+        assert explain_tf32_mismatches(acts, obs, params) == n
+        assert explain_tf32_mismatches(acts, obs, params, segments=[5]) == n
     nudged = got.copy()
     nudged[31, 4] += 1e-4
     wrong = got.copy()
@@ -179,6 +179,6 @@ def test_accounting_without_segments_is_the_five_logit_accounting():
     wrong[40] = softmax(zz)
     for acts in (nudged, wrong):
         with pytest.raises(AssertionError, match="not TF32 rounding flips"):
-            mlp_helpers.explain_tf32_mismatches(acts, obs, params)
+            explain_tf32_mismatches(acts, obs, params)
         with pytest.raises(AssertionError, match="not TF32 rounding flips"):
-            mlp_comm_helpers.explain_tf32_mismatches(acts, obs, params, segments=[5])
+            explain_tf32_mismatches(acts, obs, params, segments=[5])

@@ -11,36 +11,17 @@ import pytest
 from helpers import device_sms, launch_shape, make_product_env, regime_size
 from mlp_categorical_helpers import (bounds, categorical_pick, explain_categorical_mismatches, log_softmax_at,
                                      one_hot_torch)
-from mlp_comm_helpers import gumbel_noise, segment_softmax
-from mlp_helpers import actor_logits
-from mlp_variant_helpers import SMEM_OPTIN_BYTES, mlp_register_cap, mlp_smem_bytes
-from test_gpu_mlp_comm_policy import as_sequential, make_policies
-from test_gpu_mlp_episodes import EPISODE_REGISTER_WARPS, PROGRAMS, make_program_env, state, twins
+from mlp_helpers import actor_logits, gumbel_noise, segment_softmax
+from mlp_programs import PROGRAMS, as_sequential, make_policies, make_program_env, mlp_block_cap, state, twins
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
-
-# (tag, H, episode form) -> warps per block of the categorical kernel where the default kernel's cap of the same form
-# would spill: the MlpCategoricalRegisterWarps specialisations in csrc/mpe_kernels.cu
-CATEGORICAL_REGISTER_WARPS = {
-    ("simple_spread_n3", 64, False): 12, ("simple_push", 64, False): 12, ("simple_push", 64, True): 12,
-    ("simple_crypto", 64, True): 12, ("simple_spread_n4", 64, True): 8,
-}
 
 # Against the unrounded float64 actor a log-probability is not held to the probabilities' 5e-3 (LOOSE_MAX of
 # tests/test_gpu_mlp_policy.py): it moves with the logits, by up to 2 max |dz| per sub-space, and measures up to 8e-3 at
 # H = 32.  The bound is computed per row from the TF32 model's logit error instead.
 LOGP_FLIP_SLACK = 1e-3
 RECORDS = dict(record_actions=True, per_step_rewards=True, record_observations=True, record_log_probs=True)
-
-
-def categorical_cap(tag, H, obs_dims, act_dims, episodes=False):
-    """mlp_block_warps<P, H, episodes, true>: the categorical register cap lowered to what fits in shared memory"""
-    default = EPISODE_REGISTER_WARPS.get((tag, H)) if episodes else None
-    cap = CATEGORICAL_REGISTER_WARPS.get((tag, H, episodes), default or mlp_register_cap(tag, H, obs_dims, act_dims))
-    while mlp_smem_bytes(H, obs_dims, act_dims, cap) > SMEM_OPTIN_BYTES:
-        cap -= 1
-    return cap
 
 
 def segments_of(env):
@@ -53,8 +34,7 @@ def stride_of(act_dims):
 
 
 def size(tag, H, wpb, base=None, episodes=False):
-    shapes = make_program_env(tag, num_envs=1).world.native_shapes()
-    cap = categorical_cap(tag, H, list(shapes.obs_dims), list(shapes.act_dims), episodes)
+    cap = mlp_block_cap(tag, H, episodes, categorical=True)
     sms = device_sms()
     n = regime_size("mlp", sms, min(wpb, cap), cap=cap, base=base)
     assert launch_shape("mlp", n, sms, cap)[0] == min(wpb, cap)

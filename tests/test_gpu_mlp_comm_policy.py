@@ -8,8 +8,8 @@ import numpy as np
 import pytest
 
 from helpers import descriptor, make_product_env
-from mlp_comm_helpers import explain_tf32_mismatches, gumbel_noise, mlp_block_cap, segment_softmax
-from mlp_helpers import actor_logits, tf32_tie
+from mlp_helpers import actor_logits, explain_tf32_mismatches, gumbel_noise, segment_softmax
+from mlp_programs import LOOSE_MAX, TIGHT_ATOL, as_sequential, make_policies, mlp_block_cap
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -17,7 +17,7 @@ torch = pytest.importorskip("torch")
 COMM_TAGS = ("simple_speaker_listener", "simple_reference", "simple_crypto", "simple_adversary", "simple_push")
 
 # Every (scenario, H) instantiation at three launch shapes (helpers.launch_shape "mlp": ceil(warps / SMs) warps per
-# block, capped at mlp_comm_helpers.mlp_block_cap -- 12 for simple_reference at H = 64, else 16):
+# block, capped at mlp_programs.mlp_block_cap -- 12 for simple_reference at H = 64, else 16):
 #   "one"  a ragged size with 1-warp blocks
 #   "mid"  5-warp blocks with a partial last block and a partial last warp
 #   "full" 65 536 worlds plus a ragged tail at the full cap, partial last block and warp
@@ -26,9 +26,6 @@ CASES = [(tag, shape, T, H) for tag in COMM_TAGS for H in (32, 64) for shape, T 
 MLP_PARAMS = [c + (e,) for c in CASES for e in ((False, True) if c[1] != "full" else (c[3] == 64,))]
 MLP_SIZES = {"one": dict(wpb=1, base=2048), "mid": dict(wpb=5), "full": dict(wpb=16, base=65536)}
 
-TIGHT_ATOL = 1e-5
-# the bound of tests/test_gpu_mlp_policy.py: TF32 operands against the unrounded float64 actor
-LOOSE_MAX = 5e-3
 SEGMENT_SUM_ATOL = 2e-6
 
 
@@ -42,10 +39,10 @@ def explore_stride(act_dims):
     return 2 if max(act_dims) <= 8 else 4
 
 
-def mlp_size(shape, H, n_agents, act_dims):
+def mlp_size(tag, shape, H):
     """the batch size of a CASES shape on this device, checked against the launch rule it is meant to exercise"""
     from helpers import device_sms, launch_shape, regime_size
-    sms, cap = device_sms(), mlp_block_cap(H, n_agents, max(act_dims))
+    sms, cap = device_sms(), mlp_block_cap(tag, H)
     kw = dict(MLP_SIZES[shape])
     wpb = min(kw.pop("wpb"), cap)
     n = regime_size("mlp", sms, wpb, cap=cap, **kw)
@@ -54,32 +51,6 @@ def mlp_size(shape, H, n_agents, act_dims):
     assert shape != "one" or got[0] == 1
     assert shape != "full" or (n >= 65536 and wpb == cap)
     return n
-
-
-def make_policies(obs_dims, act_dims, H, seed=3):
-    """seeded actors; every third weight on a TF32 rounding tie, so a rounding mode other than ties-away fails"""
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    ties = lambda W: torch.as_tensor(tf32_tie(W.cpu().numpy(), 3), device="cuda")   # noqa: E731
-    pols = []
-    for od, ad in zip(obs_dims, act_dims):
-        r = lambda *s: torch.randn(*s, device="cuda", generator=g)   # noqa: E731
-        pols.append((ties(r(H, od) * 1.5 / od ** 0.5), r(H) * 0.3, ties(r(H, H) * 1.5 / H ** 0.5), r(H) * 0.3,
-                     ties(r(ad, H) * 1.5 / H ** 0.5), r(ad) * 0.2))
-    return pols
-
-
-def as_sequential(pols):
-    mods = []
-    for W1, b1, W2, b2, W3, b3 in pols:
-        H = W1.shape[0]
-        m = torch.nn.Sequential(torch.nn.Linear(W1.shape[1], H), torch.nn.ReLU(), torch.nn.Linear(H, H), torch.nn.ReLU(),
-                                torch.nn.Linear(H, W3.shape[0])).cuda()
-        with torch.no_grad():
-            for lin, W, b in ((m[0], W1, b1), (m[2], W2, b2), (m[4], W3, b3)):
-                lin.weight.copy_(W)
-                lin.bias.copy_(b)
-        mods.append(m)
-    return mods
 
 
 def twin_envs(tag, n, seed=9, **kw):
@@ -110,7 +81,7 @@ def test_comm_rollout_parity_records_and_numerics(tag, shape, T, H, explore):
     shapes = make_product_env(tag, num_envs=1).world.native_shapes()
     A, act_dims, segs = shapes.n_agents, list(shapes.act_dims), segments(tag)
     assert [sum(s) for s in segs] == act_dims
-    n = mlp_size(shape, H, A, act_dims)
+    n = mlp_size(tag, shape, H)
     env_a, env_b, obs_b = twin_envs(tag, n)
     na, nb = env_a.world.native, env_b.world.native
     desc = descriptor(tag)

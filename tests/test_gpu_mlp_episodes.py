@@ -11,51 +11,13 @@ for, at both hidden widths, with and without exploration, at a ragged launch sha
 worlds plus a tail at the block cap; then reseeding, sharding, the device epoch and the interface."""
 import pytest
 
-from helpers import CONFIGS, device_sms, launch_shape, make_product_env, regime_size
-from mlp_variant_helpers import PROGRAMS as VARIANT_PROGRAMS
-from mlp_variant_helpers import SMEM_OPTIN_BYTES, make_variant_env, mlp_register_cap, mlp_smem_bytes
-from test_gpu_mlp_comm_policy import as_sequential, make_policies
+from helpers import device_sms, launch_shape, make_product_env, regime_size
+from mlp_programs import PROGRAMS, as_sequential, make_policies, make_program_env, mlp_block_cap, state, twins
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
 
-# the 17 programs mpe_policy_mlp_rollout_kernel is built for (MlpBuilt), tag -> (scenario name, scenario kwargs)
-PROGRAMS = {**{t: s for t, s in CONFIGS.items() if t != "simple_world_comm"}, **VARIANT_PROGRAMS}
-assert len(PROGRAMS) == 17
-
-# (tag, H) -> warps per block of the episode kernel where the rollout kernel's cap would spill: the
-# MlpEpisodeRegisterWarps specialisations in csrc/mpe_kernels.cu
-EPISODE_REGISTER_WARPS = {
-    ("simple_spread_n3", 64): 12, ("simple_speaker_listener", 64): 12, ("simple_adversary", 64): 12,
-    ("simple_reference", 64): 8, ("simple_tag_4v2", 64): 8,
-}
-
 RECORDS = dict(record_actions=True, per_step_rewards=True, record_observations=True)
-
-
-def make_program_env(tag, **kw):
-    return make_variant_env(tag, **kw) if tag in VARIANT_PROGRAMS else make_product_env(tag, **kw)
-
-
-def episode_cap(tag, H, obs_dims, act_dims):
-    """mlp_block_warps<P, H, true>: the episode form's register cap lowered to what fits in shared memory"""
-    cap = EPISODE_REGISTER_WARPS.get((tag, H), mlp_register_cap(tag, H, obs_dims, act_dims))
-    while mlp_smem_bytes(H, obs_dims, act_dims, cap) > SMEM_OPTIN_BYTES:
-        cap -= 1
-    return cap
-
-
-def twins(tag, n, seed=9, **kw):
-    a = make_program_env(tag, num_envs=n, seed=seed, **kw)
-    b = make_program_env(tag, num_envs=n, seed=seed, **kw)
-    a.reset()
-    b.reset()
-    return a, b
-
-
-def state(env):
-    nw = env.world.native
-    return [nw.agent_pv.clone(), nw.lm_p.clone(), nw.comm.clone(), nw.goal.clone()]
 
 
 def assert_same_state(a, b):
@@ -105,8 +67,7 @@ def assert_matches_loop(env_a, env_b, pols, E, L, seed):
 
 def mid_size(tag, H):
     """min(5, cap)-warp blocks of the episode kernel with a partial last block and a partial last warp"""
-    nw = make_program_env(tag, num_envs=1).world.native_shapes()
-    cap = episode_cap(tag, H, list(nw.obs_dims), list(nw.act_dims))
+    cap = mlp_block_cap(tag, H, episodes=True)
     return regime_size("mlp", device_sms(), min(5, cap), cap=cap)
 
 
@@ -127,8 +88,7 @@ def test_episodes_equal_the_loop(tag, H, E, L, explore):
 def test_episodes_equal_the_loop_at_the_block_cap(tag, H):
     """65 536 worlds plus a ragged tail, in blocks at the episode kernel's cap with a partial last block and warp"""
     sms = device_sms()
-    shapes = make_program_env(tag, num_envs=1).world.native_shapes()
-    cap = episode_cap(tag, H, list(shapes.obs_dims), list(shapes.act_dims))
+    cap = mlp_block_cap(tag, H, episodes=True)
     n = regime_size("mlp", sms, cap, cap=cap, base=65536)
     assert launch_shape("mlp", n, sms, cap)[0] == cap and n > 65536
     env_a, env_b = twins(tag, n)

@@ -29,10 +29,11 @@ TIGHT_ATOL = 1e-5
 LOOSE_MAX = 5e-3
 
 
-def mlp_size(tag, shape, H, n_agents):
+def mlp_size(tag, shape, H):
     """the batch size of a CASES shape on this device, checked against the launch rule it is meant to exercise"""
-    from helpers import device_sms, launch_shape, mlp_block_cap, regime_size
-    sms, cap = device_sms(), mlp_block_cap(H, n_agents)
+    from helpers import device_sms, launch_shape, regime_size
+    from mlp_programs import mlp_block_cap
+    sms, cap = device_sms(), mlp_block_cap(tag, H)
     kw = dict(MLP_SIZES[shape])
     wpb = min(kw.pop("wpb"), cap)
     n = regime_size("mlp", sms, wpb, cap=cap, **kw)
@@ -87,7 +88,7 @@ def test_mlp_rollout_parity_records_and_numerics(tag, shape, T, H, explore):
     every step's rewards and the reward sums bit for bit; (2) obs_record[i][t] is the twin's observation before step t,
     bit for bit; (3) every action matches the float64 actor (+ the NumPy Gumbel noise when exploring) to 1e-5 unless
     the row is a TF32 rounding flip, and the unrounded float64 actor to LOOSE_MAX."""
-    n = mlp_size(tag, shape, H, len(make_product_env(tag, num_envs=1).world.agents))
+    n = mlp_size(tag, shape, H)
     env_a, env_b, obs_b = twin_envs(tag, n)
     na, nb = env_a.world.native, env_b.world.native
     pols = make_policies(na.obs_dims, H)

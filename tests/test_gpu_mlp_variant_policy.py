@@ -9,16 +9,15 @@ import numpy as np
 import pytest
 
 from helpers import device_sms, launch_shape, regime_size
-from mlp_comm_helpers import explain_tf32_mismatches, gumbel_noise
-from mlp_helpers import actor_logits, softmax
-from mlp_variant_helpers import PROGRAMS, make_variant_env, mlp_variant_cap
-from test_gpu_mlp_comm_policy import LOOSE_MAX, TIGHT_ATOL, as_sequential, make_policies
+from mlp_helpers import actor_logits, explain_tf32_mismatches, gumbel_noise, softmax
+from mlp_programs import LOOSE_MAX, TIGHT_ATOL, as_sequential, make_policies, make_variant_env, mlp_block_cap
+from mlp_programs import VARIANT_PROGRAMS as PROGRAMS
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
 
 TAGS = tuple(PROGRAMS)
-# Every (program, H) at the launch shapes of test_gpu_mlp_comm_policy.py, with the cap of mlp_variant_cap:
+# Every (program, H) at the launch shapes of test_gpu_mlp_comm_policy.py, with the cap of mlp_block_cap:
 #   "one"  a ragged size with 1-warp blocks
 #   "mid"  min(5, cap)-warp blocks with a partial last block and a partial last warp
 #   "full" 65 536 worlds plus a ragged tail at the cap, partial last block and warp
@@ -28,14 +27,9 @@ MLP_PARAMS = [c + (e,) for c in CASES for e in ((False, True) if c[1] != "full" 
 MLP_SIZES = {"one": dict(wpb=1, base=2048), "mid": dict(wpb=5), "full": dict(wpb=16, base=65536)}
 
 
-def shapes_of(tag):
-    s = make_variant_env(tag, num_envs=1).world.native_shapes()
-    return list(s.obs_dims), list(s.act_dims)
-
-
 def mlp_size(tag, shape, H):
     """the batch size of a CASES shape on this device, checked against the launch rule it is meant to exercise"""
-    sms, cap = device_sms(), mlp_variant_cap(tag, H, *shapes_of(tag))
+    sms, cap = device_sms(), mlp_block_cap(tag, H)
     kw = dict(MLP_SIZES[shape])
     wpb = min(kw.pop("wpb"), cap)
     n = regime_size("mlp", sms, wpb, cap=cap, **kw)
@@ -100,11 +94,11 @@ def test_variant_rollout_parity_records_and_numerics(tag, shape, T, H, explore):
 @pytest.mark.parametrize("tag", TAGS)
 @pytest.mark.parametrize("H", [32, 64])
 def test_launched_block_size_is_the_mirrored_cap(tag, H, tmp_path):
-    """the kernel's block and grid at the "full" size, read from a CUDA trace of the launch, are mlp_variant_cap's: the
+    """the kernel's block and grid at the "full" size, read from a CUDA trace of the launch, are mlp_block_cap's: the
     mirror the other tests size their batches with is checked against the library, not against itself"""
     from torch.profiler import ProfilerActivity, profile
     n = mlp_size(tag, "full", H)
-    cap = mlp_variant_cap(tag, H, *shapes_of(tag))
+    cap = mlp_block_cap(tag, H)
     env = make_variant_env(tag, num_envs=n, seed=9)
     env.reset()
     nw = env.world.native
