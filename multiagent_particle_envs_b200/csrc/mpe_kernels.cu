@@ -105,6 +105,18 @@ __device__ __forceinline__ void physics(const DevDesc &d, typename P::W &w, cons
 }
 
 
+// _set_action's movement force (environment.py:173-181) from the movement probabilities p1..p4.  The force starts at
+// +0: 0 + (-0) is +0, so the addition is part of the result's bits.  sens is taken by reference so that it is read
+// after the additions, the order the callers' instruction schedules were tuned with.
+__device__ __forceinline__ float2 movement_force(float p1, float p2, float p3, float p4, const float &sens) {
+    float x = 0.0f, y = 0.0f;                                           // :145
+    x += p1 - p2;                                                       // :174
+    y += p3 - p4;                                                       // :175
+    // explicit multiplies: must not be contracted into the force accumulation, or the fused
+    // step would round differently from set_action -> world_step
+    return make_float2(__fmul_rn(x, sens), __fmul_rn(y, sens));        // :178-181
+}
+
 // MultiAgentEnv._set_action (environment.py:144-192) for this lane's world, from the warp's staged action tiles
 // (s_act = the warp's staging base; tile i starts at Shape<P>::act_off(i))
 template <class P, bool ALLOW_FORCE_DISCRETE = true>
@@ -116,7 +128,7 @@ __device__ __forceinline__ void decode_rows(const float *s_act, int lane, const 
         constexpr int OFF = Shape<P>::act_off(i);
         const float *row = s_act + OFF + lane * Tile<AD>::kStride;
         int off = 0;
-        float x = 0.0f, y = 0.0f;                                       // :145
+        float2 u = make_float2(0.0f, 0.0f);                             // immovable: no force
         if constexpr (P::movable(i)) {
             float p0 = row[0], p1 = row[1], p2 = row[2], p3 = row[3], p4 = row[4];
             if (ALLOW_FORCE_DISCRETE && (flags & MPE_FLAG_FORCE_DISCRETE_ACTION)) {   // :169-172 (first arg-max)
@@ -129,16 +141,11 @@ __device__ __forceinline__ void decode_rows(const float *s_act, int lane, const 
                 p1 = best == 1 ? 1.0f : 0.0f; p2 = best == 2 ? 1.0f : 0.0f;
                 p3 = best == 3 ? 1.0f : 0.0f; p4 = best == 4 ? 1.0f : 0.0f;
             }
-            x += p1 - p2;                                               // :174
-            y += p3 - p4;                                               // :175
-            // explicit multiplies: must not be contracted into the force accumulation, or the fused
-            // step would round differently from set_action -> world_step
-            x = __fmul_rn(x, d.a_sens[i]);                              // :178-181
-            y = __fmul_rn(y, d.a_sens[i]);
+            u = movement_force(p1, p2, p3, p4, d.a_sens[i]);
             off = 5;
         }
-        ux[i] = x;
-        uy[i] = y;
+        ux[i] = u.x;
+        uy[i] = u.y;
         if constexpr (i < P::NS) {                                      // :183-190 speakers come first
 #pragma unroll
             for (int q = 0; q < P::DIMC; ++q) cact[i * P::DIMC + q] = row[off + q];
@@ -146,14 +153,94 @@ __device__ __forceinline__ void decode_rows(const float *s_act, int lane, const 
     });
 }
 
+// The warp's tile in a persistent rollout: worlds [w0, w0 + rows) of the launch's range [begin, end), one per lane.
+// Lanes past the range (in the batch's last, partial tile) are inactive: they shadow world w0 and never store.  n is the
+// kernel's copy of StepArgs::n, read at entry: a read of a.n after memory-clobbering inline asm (cp.async)
+// would be a second load.
+struct WarpTile {
+    int lane, rows;
+    bool active;
+    int64_t n, w0, wi;
+};
+__device__ __forceinline__ WarpTile warp_tile(int lane, int64_t n, int64_t w0, int64_t end) {
+    const int rows = (end - w0) < 32 ? static_cast<int>(end - w0) : 32;
+    const bool active = lane < rows;
+    return {lane, rows, active, n, w0, w0 + (active ? lane : 0)};
+}
+
+// this lane's world from HBM into registers: positions and velocities, landmarks, the utterances, the goals
+template <class P>
+__device__ __forceinline__ void load_world(const StepArgs &a, const WarpTile &wt, typename P::W &w) {
+    const int64_t n = wt.n, wi = wt.wi;
+#pragma unroll
+    for (int i = 0; i < P::A; ++i) {
+        const float4 v = a.pv[i * n + wi];
+        w.px[i] = v.x; w.py[i] = v.y; w.vx[i] = v.z; w.vy[i] = v.w;
+    }
+#pragma unroll
+    for (int l = 0; l < P::L; ++l) {
+        const float2 v = a.lm[l * n + wi];
+        w.lx[l] = v.x; w.ly[l] = v.y;
+    }
+#pragma unroll
+    for (int q = 0; q < Shape<P>::kNC; ++q) w.c[q] = a.comm[q * n + wi];
+#pragma unroll
+    for (int q = 0; q < P::G; ++q) w.g[q] = a.goal[q * n + wi];
+}
+
+// the state a rollout changes back to HBM (active lanes only): the movable agents' positions and velocities (every
+// agent's with ALL_AGENTS, after a reset has moved the immovable ones too), then the utterances
+template <class P, bool ALL_AGENTS = false>
+__device__ __forceinline__ void store_world(const StepArgs &a, const typename P::W &w, const WarpTile &wt) {
+    const int64_t n = wt.n, wi = wt.wi;
+#pragma unroll
+    for (int i = 0; i < P::A; ++i)
+        if (ALL_AGENTS || P::movable(i)) a.pv[i * n + wi] = make_float4(w.px[i], w.py[i], w.vx[i], w.vy[i]);
+#pragma unroll
+    for (int q = 0; q < Shape<P>::kNC; ++q) a.comm[q * n + wi] = w.c[q];
+}
+
+// one rollout step's rewards (scenario.reward, summed over the agents with MPE_FLAG_SHARED_REWARD as the fused step
+// does), added to the running returns in step order and written to the optional record ra.rew_steps[tg][A][n]
+template <class P, class Args>
+__device__ __forceinline__ void rollout_rewards(const Args &ra, const typename P::W &w, float (&rsum)[P::A], int tg,
+                                                const WarpTile &wt) {
+    float rew[P::A];
+    P::reward(ra.s.d, w, rew, nullptr);
+    if (ra.s.flags & MPE_FLAG_SHARED_REWARD) {
+        float sum = 0.0f;
+#pragma unroll
+        for (int i = 0; i < P::A; ++i) sum += rew[i];
+#pragma unroll
+        for (int i = 0; i < P::A; ++i) rew[i] = sum;
+    }
+#pragma unroll
+    for (int i = 0; i < P::A; ++i) rsum[i] = __fadd_rn(rsum[i], rew[i]);
+    if (ra.rew_steps != nullptr && wt.active) {
+#pragma unroll
+        for (int i = 0; i < P::A; ++i) ra.rew_steps[(static_cast<int64_t>(tg) * P::A + i) * wt.n + wt.wi] = rew[i];
+    }
+}
+
+// one agent's observation rows of the warp's tile, staged in shared memory at `tile` (ObsTile<OD> pitch), to g: as
+// coalesced 16-byte stores (LDS.128 -> STG.128) if the tile is whole and g aligned, else row by row
+template <int OD>
+__device__ __forceinline__ void store_obs_rows(float *g, const float *tile, int lane, int rows, bool active) {
+    if (rows == 32 && (reinterpret_cast<uintptr_t>(g) & 15u) == 0) {
+        obs_tile_store<OD>(g, tile, lane);
+    } else if (active) {
+#pragma unroll
+        for (int k = 0; k < OD; ++k) g[lane * OD + k] = tile[lane * ObsTile<OD>::kPitch + k];
+    }
+}
+
 // observation rows of one 32-world tile: full warps write each agent's rows into the warp's observation slot and
 // stream them out as coalesced 16-byte stores (not a TMA bulk store: the warp would have to stay resident until the
 // copy engine has read its shared memory); the batch's last, partial warp writes its rows straight to global memory.
 template <class P>
-__device__ __forceinline__ void write_observations(const StepArgs &a, const DevDesc &d, const typename P::W &w, float *s_warp,
+__device__ __forceinline__ void write_observations(const StepArgs &a, const DevDesc &d, const typename P::W &w, float *slot,
                                                    int lane, int rows, bool active, int64_t w0, int64_t wi) {
     constexpr int A = P::A;
-    float *slot = s_warp + Shape<P>::obs_base();
     if (rows == 32) {
         static_for<A>([&](auto ic) {
             constexpr int i = decltype(ic)::value;
@@ -170,6 +257,22 @@ __device__ __forceinline__ void write_observations(const StepArgs &a, const DevD
             RowWriter o{a.obs[i] + wi * P::obs_dim(i)};
             P::template observe<i>(d, w, o);
         });
+    }
+}
+
+// the end of a rollout: the final state's observations (through the observation slot), then the returns rsum (RETURNS:
+// the episode forms write theirs per episode) and done = 0 (done_callback is None, environment.py:132-135)
+template <class P, bool RETURNS = true>
+__device__ __forceinline__ void finish_rollout(const StepArgs &a, typename P::W &w, float *slot, const WarpTile &wt,
+                                               const float (&rsum)[P::A]) {
+    P::prepare(a.d, w);
+    write_observations<P>(a, a.d, w, slot, wt.lane, wt.rows, wt.active, wt.w0, wt.wi);
+    if (wt.active) {
+#pragma unroll
+        for (int i = 0; i < P::A; ++i) {
+            if constexpr (RETURNS) a.rew[i * wt.n + wt.wi] = rsum[i];
+            a.done[i * wt.n + wt.wi] = 0;
+        }
     }
 }
 
@@ -369,7 +472,7 @@ __global__ void __launch_bounds__(DENSE ? 128 : kMaxThreads, DENSE ? 6 : 1) mpe_
         for (int i = 0; i < A; ++i) rew[i] = s;
     }
     if (!(a.flags & (kFlagPdlEarly | kFlagPdlAfterLoads | kFlagPdlAtExit | kFlagPdlAfterIssue))) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi);
+    write_observations<P>(a, d, w, s_warp + Shape<P>::obs_base(), lane, rows, active, w0, wi);
     if (active) {
 #pragma unroll
         for (int i = 0; i < A; ++i) {
@@ -401,7 +504,7 @@ struct RolloutArgs {
 
 template <class P>
 __global__ void __launch_bounds__(kMaxThreads, 1) mpe_rollout_kernel(const __grid_constant__ RolloutArgs ra) {
-    constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
+    constexpr int A = P::A, NC = Shape<P>::kNC;
     const StepArgs &a = ra.s;
     extern __shared__ __align__(16) float smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -409,9 +512,8 @@ __global__ void __launch_bounds__(kMaxThreads, 1) mpe_rollout_kernel(const __gri
     const int64_t end = a.begin + a.count;
     const int64_t w0 = a.begin + (static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + warp) * 32;
     if (w0 >= end) return;
-    const int rows = (end - w0) < 32 ? static_cast<int>(end - w0) : 32;
-    const bool active = lane < rows;
-    const int64_t wi = w0 + (active ? lane : 0);
+    const WarpTile wt = warp_tile(lane, n, w0, end);
+    const int rows = wt.rows;
     float *s_warp = smem + warp * Shape<P>::kRolloutWarpFloats;
     const DevDesc &d = a.d;
     uintptr_t bits = 0;
@@ -438,24 +540,7 @@ __global__ void __launch_bounds__(kMaxThreads, 1) mpe_rollout_kernel(const __gri
     cp_async_commit();
 
     typename P::W w;
-#pragma unroll
-    for (int i = 0; i < A; ++i) {
-        const float4 v = a.pv[i * n + wi];
-        w.px[i] = v.x; w.py[i] = v.y; w.vx[i] = v.z; w.vy[i] = v.w;
-    }
-#pragma unroll
-    for (int l = 0; l < L; ++l) {
-        const float2 v = a.lm[l * n + wi];
-        w.lx[l] = v.x; w.ly[l] = v.y;
-    }
-    if constexpr (NC > 0) {   // only matters for T == 0; every step overwrites it (update_agent_state)
-#pragma unroll
-        for (int q = 0; q < NC; ++q) w.c[q] = a.comm[q * n + wi];
-    }
-    if constexpr (P::G > 0) {
-#pragma unroll
-        for (int q = 0; q < P::G; ++q) w.g[q] = a.goal[q * n + wi];
-    }
+    load_world<P>(a, wt, w);   // the utterances only matter for T == 0: every step overwrites them
 
     float rsum[A];
 #pragma unroll
@@ -474,39 +559,11 @@ __global__ void __launch_bounds__(kMaxThreads, 1) mpe_rollout_kernel(const __gri
         physics<P>(d, w, ux, uy);
 #pragma unroll
         for (int q = 0; q < NC; ++q) w.c[q] = cact[q];
-        float rew[A];
-        P::reward(d, w, rew, nullptr);
-        if (a.flags & MPE_FLAG_SHARED_REWARD) {
-            float sum = 0.0f;
-#pragma unroll
-            for (int i = 0; i < A; ++i) sum += rew[i];
-#pragma unroll
-            for (int i = 0; i < A; ++i) rew[i] = sum;
-        }
-#pragma unroll
-        for (int i = 0; i < A; ++i) rsum[i] = __fadd_rn(rsum[i], rew[i]);
-        if (ra.rew_steps != nullptr && active) {
-#pragma unroll
-            for (int i = 0; i < A; ++i) ra.rew_steps[(static_cast<int64_t>(t) * A + i) * n + wi] = rew[i];
-        }
+        rollout_rewards<P>(ra, w, rsum, t, wt);
     }
     cp_async_wait_all();
-    if (active) {
-#pragma unroll
-        for (int i = 0; i < A; ++i)
-            if (P::movable(i)) a.pv[i * n + wi] = make_float4(w.px[i], w.py[i], w.vx[i], w.vy[i]);
-#pragma unroll
-        for (int q = 0; q < NC; ++q) a.comm[q * n + wi] = w.c[q];
-    }
-    P::prepare(d, w);
-    write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi);
-    if (active) {
-#pragma unroll
-        for (int i = 0; i < A; ++i) {
-            a.rew[i * n + wi] = rsum[i];
-            a.done[i * n + wi] = 0;
-        }
-    }
+    if (wt.active) store_world<P>(a, w, wt);
+    finish_rollout<P>(a, w, s_warp + Shape<P>::obs_base(), wt, rsum);
 }
 
 
@@ -605,17 +662,13 @@ __device__ __forceinline__ float2 policy_agent(const DevDesc &d, const typename 
 #pragma unroll
         for (int c = 0; c < 5; ++c) record[c] = pr[c];
     }
-    // _set_action (environment.py:173-181), the arithmetic of decode_rows
-    float x = 0.0f, y = 0.0f;
-    x += pr[1] - pr[2];
-    y += pr[3] - pr[4];
-    return make_float2(__fmul_rn(x, d.a_sens[I]), __fmul_rn(y, d.a_sens[I]));
+    return movement_force(pr[1], pr[2], pr[3], pr[4], d.a_sens[I]);   // _set_action, as decode_rows
 }
 
 template <class P, int H>
 __global__ void __launch_bounds__(128) mpe_policy_rollout_kernel(const __grid_constant__ PolicyArgs pa) {
     static_assert(P::NS == 0 && H % 4 == 0, "policy rollout: silent agents, hidden width a multiple of 4");
-    constexpr int A = P::A, L = P::L;
+    constexpr int A = P::A;
     using PS = PolicyShape<P, H>;
     const StepArgs &a = pa.s;
     extern __shared__ __align__(16) float smem[];
@@ -637,27 +690,12 @@ __global__ void __launch_bounds__(128) mpe_policy_rollout_kernel(const __grid_co
     const int64_t end = a.begin + a.count;
     const int64_t w0 = a.begin + (static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + warp) * 32;
     if (w0 >= end) return;
-    const int rows = (end - w0) < 32 ? static_cast<int>(end - w0) : 32;
-    const bool active = lane < rows;
-    const int64_t wi = w0 + (active ? lane : 0);
+    const WarpTile wt = warp_tile(lane, n, w0, end);
     float *s_warp = smem + PS::kWeightFloats + warp * Shape<P>::kWarpFloats;
     const DevDesc &d = a.d;
 
     typename P::W w;
-#pragma unroll
-    for (int i = 0; i < A; ++i) {
-        const float4 v = a.pv[i * n + wi];
-        w.px[i] = v.x; w.py[i] = v.y; w.vx[i] = v.z; w.vy[i] = v.w;
-    }
-#pragma unroll
-    for (int l = 0; l < L; ++l) {
-        const float2 v = a.lm[l * n + wi];
-        w.lx[l] = v.x; w.ly[l] = v.y;
-    }
-    if constexpr (P::G > 0) {
-#pragma unroll
-        for (int q = 0; q < P::G; ++q) w.g[q] = a.goal[q * n + wi];
-    }
+    load_world<P>(a, wt, w);
 
     float rsum[A];
 #pragma unroll
@@ -669,42 +707,16 @@ __global__ void __launch_bounds__(128) mpe_policy_rollout_kernel(const __grid_co
         static_for<A>([&](auto ic) {
             constexpr int i = decltype(ic)::value;
             const float2 u = policy_agent<P, H, i>(d, w, s_w + PolicyShape<P, H>::agent_off(i),
-                                                   (pa.act_rec[i] != nullptr && active)
-                                                       ? pa.act_rec[i] + (static_cast<int64_t>(t) * n + wi) * 5 : nullptr);
+                                                   (pa.act_rec[i] != nullptr && wt.active)
+                                                       ? pa.act_rec[i] + (static_cast<int64_t>(t) * n + wt.wi) * 5 : nullptr);
             ux[i] = u.x;
             uy[i] = u.y;
         });
         physics<P>(d, w, ux, uy);
-        float rew[A];
-        P::reward(d, w, rew, nullptr);
-        if (a.flags & MPE_FLAG_SHARED_REWARD) {
-            float sum = 0.0f;
-#pragma unroll
-            for (int i = 0; i < A; ++i) sum += rew[i];
-#pragma unroll
-            for (int i = 0; i < A; ++i) rew[i] = sum;
-        }
-#pragma unroll
-        for (int i = 0; i < A; ++i) rsum[i] = __fadd_rn(rsum[i], rew[i]);
-        if (pa.rew_steps != nullptr && active) {
-#pragma unroll
-            for (int i = 0; i < A; ++i) pa.rew_steps[(static_cast<int64_t>(t) * A + i) * n + wi] = rew[i];
-        }
+        rollout_rewards<P>(pa, w, rsum, t, wt);
     }
-    if (active) {
-#pragma unroll
-        for (int i = 0; i < A; ++i)
-            if (P::movable(i)) a.pv[i * n + wi] = make_float4(w.px[i], w.py[i], w.vx[i], w.vy[i]);
-    }
-    P::prepare(d, w);
-    write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi);
-    if (active) {
-#pragma unroll
-        for (int i = 0; i < A; ++i) {
-            a.rew[i * n + wi] = rsum[i];
-            a.done[i * n + wi] = 0;
-        }
-    }
+    if (wt.active) store_world<P>(a, w, wt);
+    finish_rollout<P>(a, w, s_warp + Shape<P>::obs_base(), wt, rsum);
 }
 
 template <class P>
@@ -1039,15 +1051,8 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
         P::template observe<I>(d, w, o);                   // scenario.observation(agent I) -> this lane's tile row
     }
     __syncwarp();
-    if (pa.obs_rec[I] != nullptr) {                        // the observation the actor sees at step t
-        float *g = pa.obs_rec[I] + (static_cast<int64_t>(t) * n + w0) * OD;
-        if (rows == 32 && (reinterpret_cast<uintptr_t>(g) & 15u) == 0) {
-            obs_tile_store<OD>(g, tile, lane);             // LDS.128 -> STG.128, as the fused step's observations
-        } else if (active) {
-#pragma unroll
-            for (int k = 0; k < OD; ++k) g[lane * OD + k] = tile[lane * PITCH + k];
-        }
-    }
+    if (pa.obs_rec[I] != nullptr)                          // the observation the actor sees at step t
+        store_obs_rows<OD>(pa.obs_rec[I] + (static_cast<int64_t>(t) * n + w0) * OD, tile, lane, rows, active);
     const int gq = lane >> 2, tq = lane & 3;
     // ---- layer 1: [32 x K1] . [K1 x H] + b1 ----
     float h[2][NT][4];
@@ -1187,10 +1192,7 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
         for (int q = 0; q < COMM; ++q) cact[I * P::DIMC + q] = pr[MOVE + q];
     }
     if constexpr (MOVE > 0) {
-        float x = 0.0f, y = 0.0f;
-        x += pr[1] - pr[2];
-        y += pr[3] - pr[4];
-        return make_float2(__fmul_rn(x, d.a_sens[I]), __fmul_rn(y, d.a_sens[I]));
+        return movement_force(pr[1], pr[2], pr[3], pr[4], d.a_sens[I]);
     } else {
         return make_float2(0.0f, 0.0f);                    // immovable: no force, and physics<P> never moves it
     }
@@ -1308,13 +1310,7 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
                         P::template observe<i>(d, w, o);
                     }
                     __syncwarp();
-                    float *g = ea->final_obs[i] + (static_cast<int64_t>(e) * n + w0) * OD;
-                    if (rows == 32 && (reinterpret_cast<uintptr_t>(g) & 15u) == 0) {
-                        obs_tile_store<OD>(g, s_warp, lane);
-                    } else if (active) {
-#pragma unroll
-                        for (int k = 0; k < OD; ++k) g[lane * OD + k] = s_warp[lane * ObsTile<OD>::kPitch + k];
-                    }
+                    store_obs_rows<OD>(ea->final_obs[i] + (static_cast<int64_t>(e) * n + w0) * OD, s_warp, lane, rows, active);
                     __syncwarp();
                 });
             }
@@ -1344,9 +1340,7 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
     }
     P::prepare(d, w);
     __syncwarp();                  // every lane has read its logits before the tile is reused
-    // write_observations addresses the observation slot at obs_base(): shift the base so that the slot is this warp's
-    // observation tile
-    write_observations<P>(a, d, w, s_warp - Shape<P>::obs_base(), lane, rows, active, w0, wi);
+    write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi);   // the slot is this warp's observation tile
     if (active) {
 #pragma unroll
         for (int i = 0; i < A; ++i) {
@@ -1969,6 +1963,29 @@ static int fill_actions(mpe_handle h, StepArgs &a, const float *const *act_n) {
     return MPE_OK;
 }
 
+// The persistent (multi-step) kernels: one launch covers the whole batch and writes no info
+static int fill_persistent(mpe_handle h, StepArgs &a, void *pv, const void *lm, float *comm, const int32_t *goal,
+                           float *const *obs_n, float *rew, uint8_t *done, uint32_t flags) {
+    int r = fill_state(h, a, pv, lm, comm, goal);
+    if (r) return r;
+    r = fill_outputs(h, a, obs_n, rew, done, nullptr);
+    if (r) return r;
+    a.flags = flags;
+    a.d = h->dev;
+    a.n = h->n;
+    a.begin = 0;
+    a.count = h->n;
+    return MPE_OK;
+}
+
+// `warps` warps (one per 32 worlds) in blocks of wpb; dynamic shared memory = fixed bytes + per-warp bytes x wpb
+static int launch_persistent(mpe_handle h, const void *fn, int64_t warps, int64_t wpb, size_t fixed_smem, size_t warp_smem,
+                             void *args, void *stream, const char *what) {
+    void *params[] = {args};
+    return launch_kernel(h, fn, (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb), fixed_smem + warp_smem * wpb, stream,
+                         params, false, what);
+}
+
 extern "C" int mpe_set_action(mpe_handle h, const float *const *act_n, float *u, float *c, uint32_t flags, void *stream) {
     if (!h || !ok8(u)) return MPE_ERR_BAD_ARG;
     if (h->prog->NS * h->prog->DIMC > 0 && !ok4(c)) return MPE_ERR_BAD_ARG;
@@ -2031,27 +2048,17 @@ extern "C" int mpe_rollout(mpe_handle h, void *pv, const void *lm, float *comm, 
     if (rew_steps != nullptr && !ok4(rew_steps)) return MPE_ERR_BAD_ARG;
     NvtxRange range("mpe_rollout");
     RolloutArgs ra{};
-    StepArgs &a = ra.s;
-    int r = fill_state(h, a, pv, lm, comm, goal);
+    int r = fill_persistent(h, ra.s, pv, lm, comm, goal, obs_n, rew_sum, done, flags);
     if (r) return r;
-    r = fill_actions(h, a, act_seq);
+    r = fill_actions(h, ra.s, act_seq);
     if (r) return r;
-    r = fill_outputs(h, a, obs_n, rew_sum, done, nullptr);
-    if (r) return r;
-    a.info = nullptr;
-    a.flags = flags;
-    a.d = h->dev;
-    a.n = h->n;
-    a.begin = 0;
-    a.count = h->n;
     ra.T = n_steps;
     ra.rew_steps = rew_steps;
     const int64_t warps = (h->n + 31) / 32;
     int wpb = warps <= 4LL * h->sms ? 1 : (warps <= 64LL * h->sms ? 2 : 4);
     if (wpb > max_warps_per_block(h->prog->rollout_smem)) wpb = max_warps_per_block(h->prog->rollout_smem);
-    void *params[] = {&ra};
-    return launch_kernel(h, reinterpret_cast<const void *>(h->prog->rollout_fn), (warps + wpb - 1) / wpb, 32 * wpb,
-                         static_cast<size_t>(h->prog->rollout_smem) * wpb, stream, params, false, "cudaLaunchKernelExC(rollout)");
+    return launch_persistent(h, reinterpret_cast<const void *>(h->prog->rollout_fn), warps, wpb, 0, h->prog->rollout_smem, &ra,
+                             stream, "cudaLaunchKernelExC(rollout)");
 }
 
 extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
@@ -2067,10 +2074,7 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
     if (rew_steps != nullptr && !ok4(rew_steps)) return MPE_ERR_BAD_ARG;
     NvtxRange range("mpe_rollout_policy");
     PolicyArgs pa{};
-    StepArgs &a = pa.s;
-    int r = fill_state(h, a, pv, lm, comm, goal);
-    if (r) return r;
-    r = fill_outputs(h, a, obs_n, rew_sum, done, nullptr);
+    int r = fill_persistent(h, pa.s, pv, lm, comm, goal, obs_n, rew_sum, done, flags);
     if (r) return r;
     for (int i = 0; i < h->prog->A; ++i) {
         if (!ok16(w1_n[i]) || !ok16(b1_n[i]) || !ok16(w2_n[i]) || !ok4(b2_n[i])) return MPE_ERR_BAD_ARG;
@@ -2078,20 +2082,13 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
         pa.act_rec[i] = act_record_n ? act_record_n[i] : nullptr;
         if (pa.act_rec[i] != nullptr && !ok4(pa.act_rec[i])) return MPE_ERR_BAD_ARG;
     }
-    a.info = nullptr;
-    a.flags = flags;
-    a.d = h->dev;
-    a.n = h->n;
-    a.begin = 0;
-    a.count = h->n;
     pa.T = n_steps;
     pa.rew_steps = rew_steps;
     const int64_t warps = (h->n + 31) / 32;
     const int wpb = warps <= 16LL * h->sms ? 1 : (warps <= 64LL * h->sms ? 2 : 4);
-    void *params[] = {&pa};
-    const size_t smem = static_cast<size_t>(h->prog->policy_weight_floats[k]) * 4 + static_cast<size_t>(h->prog->smem_bytes) * wpb;
-    return launch_kernel(h, reinterpret_cast<const void *>(h->prog->policy_fn[k]), (warps + wpb - 1) / wpb, 32 * wpb, smem,
-                         stream, params, false, "cudaLaunchKernelExC(rollout_policy)");
+    return launch_persistent(h, reinterpret_cast<const void *>(h->prog->policy_fn[k]), warps, wpb,
+                             static_cast<size_t>(h->prog->policy_weight_floats[k]) * 4, h->prog->smem_bytes, &pa, stream,
+                             "cudaLaunchKernelExC(rollout_policy)");
 }
 
 // The arguments of the four two-hidden-layer rollout entry points, filled by name (several neighbours share a type).
@@ -2150,10 +2147,7 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     }
     MlpEpisodeArgs ea{};
     MlpPolicyArgs &pa = ea.p;
-    StepArgs &a = pa.s;
-    int r = fill_state(h, a, c.pv, c.lm, c.comm, c.goal);
-    if (r) return r;
-    r = fill_outputs(h, a, c.obs_n, c.rew, c.done, nullptr);
+    int r = fill_persistent(h, pa.s, c.pv, c.lm, c.comm, c.goal, c.obs_n, c.rew, c.done, c.flags);
     if (r) return r;
     for (int i = 0; i < h->prog->A; ++i) {
         for (int j = 0; j < 6; ++j)
@@ -2166,12 +2160,6 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
         ea.final_obs[i] = c.final_obs_record_n ? c.final_obs_record_n[i] : nullptr;
         if (c.final_obs_record_n != nullptr && !ok16(ea.final_obs[i])) return MPE_ERR_BAD_ARG;   // every agent's, or none
     }
-    a.info = nullptr;
-    a.flags = c.flags;
-    a.d = h->dev;
-    a.n = h->n;
-    a.begin = 0;
-    a.count = h->n;
     pa.T = c.T;
     pa.explore = c.explore ? 1 : 0;
     pa.seed = c.explore_seed;
@@ -2191,10 +2179,9 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
     if (wpb > h->prog->mlp[c.form][k].warps) wpb = h->prog->mlp[c.form][k].warps;
-    void *params[] = {form_args[c.form]};
-    const size_t smem = (static_cast<size_t>(h->prog->mlp_weight_floats[k]) + static_cast<size_t>(h->prog->mlp_warp_floats[k]) * wpb) * 4;
-    return launch_kernel(h, h->prog->mlp[c.form][k].fn, (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb), smem, c.stream,
-                         params, false, kName[c.form][1]);
+    return launch_persistent(h, h->prog->mlp[c.form][k].fn, warps, wpb, static_cast<size_t>(h->prog->mlp_weight_floats[k]) * 4,
+                             static_cast<size_t>(h->prog->mlp_warp_floats[k]) * 4, form_args[c.form], c.stream,
+                             kName[c.form][1]);
 }
 
 extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
@@ -2423,21 +2410,14 @@ static int reset_impl(mpe_handle h, void *pv, void *lm, float *comm, int32_t *go
     a.seed = seed; a.world_offset = world_offset; a.epoch = epoch; a.epoch_dev = epoch_dev;
     a.landmark_range = reset_landmark_range(p->scenario);
     a.goal_mod = p->L > 0 ? p->L : 1;
-    int prev = 0;
-    CUDA_TRY(cudaGetDevice(&prev));
-    if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
-    const unsigned blocks = static_cast<unsigned>((h->n + 255) / 256);
-    reset_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess && epoch_dev) {
-        bump_epoch_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(epoch_dev);
-        e = cudaGetLastError();
-        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    void *params[] = {&a};
+    r = launch_kernel(h, reinterpret_cast<const void *>(reset_kernel), (h->n + 255) / 256, 256, 0, stream, params, false,
+                      "reset_kernel");
+    if (r == MPE_OK && epoch_dev) {   // the device epoch advances after this reset has read it
+        void *bump[] = {&epoch_dev};
+        r = launch_kernel(h, reinterpret_cast<const void *>(bump_epoch_kernel), 1, 1, 0, stream, bump, false, "reset_kernel");
     }
-    if (prev != h->device) cudaSetDevice(prev);
-    if (e != cudaSuccess) return cuda_fail(e, "reset_kernel");
-    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
-    return MPE_OK;
+    return r;
 }
 
 extern "C" int mpe_reset(mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal, const uint8_t *mask,

@@ -6,7 +6,16 @@ loads / stores, exact-image vs padded tile streaming) are all in the binary, so 
 full warp executes roughly half of them (spread N=3: 664 executed per warp in ncu vs 1252 static).
 
     python tools/sass_stats.py > profiles/r1_static_resources.md
+
+`--compare OTHER.so` instead compares this library's kernels with OTHER's, function by function: which exist in only
+one of them, which have different SASS, and which changed registers or stack; it exits with 1 if anything differs.
+"Different SASS" compares the instruction text (opcode, operands and the address/encoding line cuobjdump prints with
+it), not the separate control-word line (stall counts, yield, barriers, operand reuse), so two builds that differ
+only in scheduling control bits count as the same.
+
+    python tools/sass_stats.py --compare /path/to/parent/libmpe_b200.so
 """
+import argparse
 import collections
 import os
 import re
@@ -22,8 +31,9 @@ def demangle(names):
     return dict(zip(names, out))
 
 
-def main():
-    res = subprocess.run(["cuobjdump", "-res-usage", LIB], capture_output=True, text=True).stdout
+def resource_usage(lib):
+    """{mangled name: (registers, stack bytes)} from `cuobjdump -res-usage`."""
+    res = subprocess.run(["cuobjdump", "-res-usage", lib], capture_output=True, text=True, check=True).stdout
     usage = {}
     cur = None
     for ln in res.splitlines():
@@ -35,6 +45,50 @@ def main():
         if m and cur:
             usage[cur] = (int(m.group(1)), int(m.group(2)))
             cur = None
+    return usage
+
+
+def sass_text(lib):
+    """{mangled name: the function's SASS instruction lines} from `cuobjdump -sass`."""
+    sass = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
+    funcs = {}
+    cur = None
+    for ln in sass.splitlines():
+        m = re.match(r"\s*Function : (\S+)", ln)
+        if m:
+            cur = funcs.setdefault(m.group(1), [])
+            continue
+        if cur is not None and re.match(r"\s*/\*[0-9a-f]{4,}\*/", ln):
+            cur.append(ln.strip())
+    return funcs
+
+
+def compare(other):
+    a_sass, b_sass = sass_text(LIB), sass_text(other)
+    a_use, b_use = resource_usage(LIB), resource_usage(other)
+    names = demangle(sorted(set(a_sass) | set(b_sass) | set(a_use) | set(b_use)))
+    print("this: %s (%d functions)\nother: %s (%d functions)" % (LIB, len(a_sass), other, len(b_sass)))
+    only_a = sorted(names[k] for k in set(a_sass) - set(b_sass))
+    only_b = sorted(names[k] for k in set(b_sass) - set(a_sass))
+    differ = sorted(names[k] for k in set(a_sass) & set(b_sass) if a_sass[k] != b_sass[k])
+    usage = sorted((names[k], b_use[k], a_use[k]) for k in set(a_use) & set(b_use) if a_use[k] != b_use[k])
+    print("\nonly in this library: %d" % len(only_a))
+    for nm in only_a:
+        print("  " + nm)
+    print("\nonly in the other library: %d" % len(only_b))
+    for nm in only_b:
+        print("  " + nm)
+    print("\ndifferent SASS: %d of %d" % (len(differ), len(set(a_sass) & set(b_sass))))
+    for nm in differ:
+        print("  " + nm)
+    print("\nREG / STACK changed (other -> this): %d" % len(usage))
+    for nm, (rb, sb), (ra, sa) in usage:
+        print("  %s: REG %d -> %d, STACK %d -> %d" % (nm, rb, ra, sb, sa))
+    return 1 if only_a or only_b or differ or usage else 0
+
+
+def main():
+    usage = resource_usage(LIB)
     sass = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True).stdout
     mix = {}
     cur = None
@@ -93,4 +147,7 @@ def main():
 
 
 if __name__ == "__main__":
-    sys.exit(main())
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--compare", metavar="OTHER.so", help="compare every kernel's SASS and REG / STACK with OTHER.so")
+    args = ap.parse_args()
+    sys.exit(compare(args.compare) if args.compare else main())
