@@ -308,6 +308,36 @@ MPE_API int mpe_rollout_policy_mlp_categorical_episodes(
     int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n, uint8_t *done_dev,
     uint32_t flags, void *stream);
 
+/* MAPPO's MLP actor (MLPBase with layer_N = 1 and a categorical ACTLayer head), hidden width 64 only:
+ *     [LN(obs_dim_i)] -> Linear(obs_dim_i, 64) -> act -> LN(64) -> Linear(64, 64) -> act -> LN(64) -> Linear(64, act_dim_i)
+ * with act = ReLU, or tanh (tanhf) if net_flags & 2; the input LayerNorm only if net_flags & 1.  Every LayerNorm uses
+ * ln_eps.  w1_n .. b3_n are the FOLDED network: each LayerNorm's affine (gamma, beta) moved into the Linear after it,
+ *     W' = W diag(gamma),   b' = b + W beta
+ * (LN(obs) into W1, b1; the first hidden LN into W2, b2; the second into W3, b3), so the kernel normalises without
+ * parameters: (x - mu) * rsqrt(var + ln_eps), mu and var two-pass fp32 statistics over the row, before the TF32
+ * rounding of the next GEMM's operand.  Observation records and final observations hold the raw observations.
+ * Everything else -- the parameters, records, sampling, log-probabilities, episode semantics and refusals -- is that of
+ * mpe_rollout_policy_mlp_categorical[_episodes], with two more refusals: hidden != 64 (MPE_ERR_UNSUPPORTED, with the
+ * scenario, before any pointer) and bits of net_flags above 1 or an ln_eps that is negative or not finite
+ * (MPE_ERR_BAD_ARG, after the flags). */
+MPE_API int mpe_rollout_policy_mappo(mpe_handle h, void *agent_pv_dev, const void *lm_p_dev, float *comm_dev,
+                                     const int32_t *goal_dev, const float *const *w1_n, const float *const *b1_n,
+                                     const float *const *w2_n, const float *const *b2_n, const float *const *w3_n,
+                                     const float *const *b3_n, int32_t hidden, int32_t n_steps, int32_t explore,
+                                     uint64_t explore_seed, uint64_t explore_epoch, uint64_t world_offset,
+                                     float *const *obs_n_dev, float *rew_sum_dev, float *rew_steps_dev,
+                                     float *logp_steps_dev, int32_t *const *act_index_record_n,
+                                     float *const *obs_record_n, uint32_t net_flags, float ln_eps, uint8_t *done_dev,
+                                     uint32_t flags, void *stream);
+MPE_API int mpe_rollout_policy_mappo_episodes(
+    mpe_handle h, void *agent_pv_dev, void *lm_p_dev, float *comm_dev, int32_t *goal_dev, const float *const *w1_n,
+    const float *const *b1_n, const float *const *w2_n, const float *const *b2_n, const float *const *w3_n,
+    const float *const *b3_n, int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
+    uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset,
+    float *const *obs_n_dev, float *ep_rew_dev, float *rew_steps_dev, float *logp_steps_dev,
+    int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n,
+    uint32_t net_flags, float ln_eps, uint8_t *done_dev, uint32_t flags, void *stream);
+
 /* Same step for a caller that holds HOST buffers (what the reference's callers hold):
  * act_n_host[i] -> (async H2D into act_n_dev[i]) -> mpe_step -> (async D2H) obs_n_host[i],
  * rew_host, done_host, all ordered on `stream`.  Host buffers should be pinned for the copies

@@ -26,6 +26,10 @@ FLAG_HOST_SLAB = 8
 
 ERR_UNSUPPORTED = -3
 
+# net_flags of mpe_rollout_policy_mappo[_episodes]
+MAPPO_FEATURE_NORM = 1
+MAPPO_TANH = 2
+
 
 class MpeDesc(ctypes.Structure):
     """mirror of `struct mpe_desc` (include/mpe_b200.h)"""
@@ -102,6 +106,15 @@ _SIGNATURES = {
                                                                    ctypes.c_int32, ctypes.c_uint64, ctypes.c_uint64,
                                                                    ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, _PP,
                                                                    _P, _P, _P, _PP, _PP, _PP, _P, ctypes.c_uint32, _P]),
+    "mpe_rollout_policy_mappo": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _PP, _PP, _PP, ctypes.c_int32,
+                                                ctypes.c_int32, ctypes.c_int32, ctypes.c_uint64, ctypes.c_uint64,
+                                                ctypes.c_uint64, _PP, _P, _P, _P, _PP, _PP, ctypes.c_uint32, ctypes.c_float,
+                                                _P, ctypes.c_uint32, _P]),
+    "mpe_rollout_policy_mappo_episodes": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _PP, _PP, _PP, ctypes.c_int32,
+                                                         ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_uint64,
+                                                         ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64,
+                                                         ctypes.c_uint64, _PP, _P, _P, _P, _PP, _PP, _PP, ctypes.c_uint32,
+                                                         ctypes.c_float, _P, ctypes.c_uint32, _P]),
     "mpe_step_host": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _P, _P, _P, _PP, _P, _P, _P,
                                      ctypes.c_uint32, _P]),
     "mpe_strerror": (ctypes.c_char_p, [ctypes.c_int]),

@@ -877,6 +877,24 @@ struct MlpCategoricalEpisodeArgs {
 };
 static_assert(sizeof(MlpCategoricalEpisodeArgs) <= 4096, "kernel parameter space");
 
+// MAPPO's MLP actor (MAPPO, MLPBase with layer_N = 1 and its categorical ACTLayer head), categorical form only, H = 64:
+//     [LN(obs_dim_i)] -> Linear(obs_dim_i, 64) -> act -> LN(64) -> Linear(64, 64) -> act -> LN(64) -> Linear(64, act_dim_i)
+// act is ReLU or tanh.  Every LayerNorm's affine (gamma, beta) is folded into the Linear after it on the host
+// (W' = W diag(gamma), b' = b + W beta), so w1..b3 are the folded network and the kernel applies parameter-free
+// normalisation (x - mu) * rsqrt(var + eps) with two-pass fp32 statistics (mlp_agent).
+enum : uint32_t { kMappoFeatureNorm = 1u, kMappoTanh = 2u };
+struct MlpMappoArgs {
+    MlpCategoricalArgs c;
+    float eps;                      // of every LayerNorm
+    uint32_t net_flags;             // kMappoFeatureNorm: the input LayerNorm; kMappoTanh: tanh instead of ReLU
+};
+struct MlpMappoEpisodeArgs {
+    MlpCategoricalEpisodeArgs c;
+    float eps;
+    uint32_t net_flags;
+};
+static_assert(sizeof(MlpMappoEpisodeArgs) <= 4096, "kernel parameter space");
+
 template <class P, int H>
 struct MlpShape {
     static constexpr int NT = H / 8;                                   // n-tiles of a hidden layer (= its k-tiles)
@@ -934,10 +952,12 @@ template <> struct MlpRegisterException<Spread<3>, 64> : MlpException<kFormE | k
 template <> struct MlpRegisterException<Push<1, 1, 2>, 64> : MlpException<kFormC | kFormCE, 12> {};       // 8 at 128
 template <> struct MlpRegisterException<Crypto, 64> : MlpException<kFormCE, 12> {};                       // 16 at 128
 template <> struct MlpRegisterException<Spread<4>, 64> : MlpException<kFormCE, 8> {};                     // 8 at 168
+template <class P, int H>
+__host__ __device__ constexpr int mlp_register_rule() { return (H == 64 && (P::A >= 4 || mlp_max_act_dim<P>() > 8)) ? 12 : 16; }
 template <class P, int H, int FORM>
 __host__ __device__ constexpr int mlp_register_warps() {
     using X = MlpRegisterException<P, H>;
-    return (X::forms >> FORM & 1) ? X::warps : ((H == 64 && (P::A >= 4 || mlp_max_act_dim<P>() > 8)) ? 12 : 16);
+    return (X::forms >> FORM & 1) ? X::warps : mlp_register_rule<P, H>();
 }
 constexpr int kMlpSmemBytes = 232448;
 template <class P, int H>
@@ -947,6 +967,24 @@ __host__ __device__ constexpr int mlp_smem_warps() {
 template <class P, int H, bool EPISODES = false, bool CATEGORICAL = false>
 __host__ __device__ constexpr int mlp_block_warps() {
     constexpr int r = mlp_register_warps<P, H, EPISODES | CATEGORICAL << 1>(), s = mlp_smem_warps<P, H>();
+    return r < s ? r : s;
+}
+// The MAPPO actor's kernels (mpe_policy_mappo[_episode]_kernel, categorical, H = 64): the same shapes and shared-memory
+// limit, the general rule of H = 64 above, and their own exceptions, by the categorical forms' masks (kFormC: one
+// episode, kFormCE: episodes) -- the three LayerNorms keep a second 32-register m-tile of h2 next to h1 (see mlp_agent)
+template <class P> struct MappoRegisterException : MlpException<0, 0> {};
+template <> struct MappoRegisterException<Spread<2>> : MlpException<kFormC | kFormCE, 12> {};           // 16, 24 bytes of stack at 128
+template <> struct MappoRegisterException<Spread<3>> : MlpException<kFormC | kFormCE, 12> {};           // 32, 32 at 128
+template <> struct MappoRegisterException<Spread<6>> : MlpException<kFormC | kFormCE, 8> {};            // 64, 56 at 168
+template <> struct MappoRegisterException<Tag<1, 1, 2>> : MlpException<kFormC | kFormCE, 12> {};        // 16, 24 at 128
+template <> struct MappoRegisterException<Tag<2, 1, 2>> : MlpException<kFormC | kFormCE, 12> {};        // 56, 56 at 128
+template <> struct MappoRegisterException<SpeakerListener> : MlpException<kFormC | kFormCE, 12> {};     // 16, 16 at 128
+template <> struct MappoRegisterException<Adversary<1, 2, 2>> : MlpException<kFormC | kFormCE, 12> {};  // 32, 40 at 128
+template <> struct MappoRegisterException<Crypto> : MlpException<kFormC, 12> {};                        // 8 at 128
+template <class P, bool EPISODES>
+__host__ __device__ constexpr int mappo_block_warps() {
+    using X = MappoRegisterException<P>;
+    constexpr int r = (X::forms >> (EPISODES | 2) & 1) ? X::warps : mlp_register_rule<P, 64>(), s = mlp_smem_warps<P, 64>();
     return r < s ? r : s;
 }
 // the two programs whose weights fill most of the 227 KB
@@ -990,6 +1028,50 @@ __device__ __forceinline__ void relu_tf32_frag(uint32_t (&a)[4], const float (&c
     a[3] = to_tf32(fmaxf(c[3], 0.0f));   // row g+8, k = 2q+1
 }
 
+// MAPPO's hidden layer: the accumulators of one m-tile (NT n-tiles) -> act (tanhf, or ReLU) -> LayerNorm without affine
+// -> TF32 A fragments of the next layer, in relu_tf32_frag's order.  A row's NT * 8 units are 2 per n-tile in each of
+// the 4 lanes of a quad (rows g: elements 0, 1; g + 8: 2, 3), so its sums are a local sum and __shfl_xor over 1 and 2.
+// Two-pass fp32 statistics as torch takes them: mu = sum(x) / H, then var = sum((x - mu)^2) / H; the normalised value
+// (x - mu) * rsqrt(var + eps) is rounded to TF32 only then.
+template <int NT>
+__device__ __forceinline__ void act_norm_tf32_frags(uint32_t (&a)[NT][4], float (&c)[NT][4], bool tanh_act, float eps) {
+    constexpr float kInvH = 1.0f / (NT * 8);      // H = 8 NT, a power of two: exact
+    if (tanh_act) {
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) c[nt][j] = tanhf(c[nt][j]);
+    } else {
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) c[nt][j] = fmaxf(c[nt][j], 0.0f);
+    }
+    float s0 = 0.0f, s1 = 0.0f;
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) { s0 += c[nt][0] + c[nt][1]; s1 += c[nt][2] + c[nt][3]; }
+    s0 += __shfl_xor_sync(0xffffffffu, s0, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+    s0 += __shfl_xor_sync(0xffffffffu, s0, 2); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+    const float m0 = s0 * kInvH, m1 = s1 * kInvH;
+    float v0 = 0.0f, v1 = 0.0f;
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+        const float d0 = c[nt][0] - m0, d1 = c[nt][1] - m0, d2 = c[nt][2] - m1, d3 = c[nt][3] - m1;
+        v0 += d0 * d0 + d1 * d1;
+        v1 += d2 * d2 + d3 * d3;
+    }
+    v0 += __shfl_xor_sync(0xffffffffu, v0, 1); v1 += __shfl_xor_sync(0xffffffffu, v1, 1);
+    v0 += __shfl_xor_sync(0xffffffffu, v0, 2); v1 += __shfl_xor_sync(0xffffffffu, v1, 2);
+    const float r0 = rsqrtf(v0 * kInvH + eps), r1 = rsqrtf(v1 * kInvH + eps);
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+        a[nt][0] = to_tf32((c[nt][0] - m0) * r0);   // row g,   k = 2q
+        a[nt][1] = to_tf32((c[nt][2] - m1) * r1);   // row g+8, k = 2q
+        a[nt][2] = to_tf32((c[nt][1] - m0) * r0);   // row g,   k = 2q+1
+        a[nt][3] = to_tf32((c[nt][3] - m1) * r1);   // row g+8, k = 2q+1
+    }
+}
+
 // pr[B, B + K) = softmax(z[B, B + K)): one action sub-space.  The operation order is the one of every other softmax
 // here (the max is exact in any order; the sum runs from the first entry to the last).
 template <int B, int K, int N>
@@ -1031,12 +1113,18 @@ __device__ __forceinline__ float categorical_segment(const float (&zs)[N], const
 // (Gumbel-)softmax per sub-space -> decoded (u.x, u.y), and a speaker's utterance into cact[I * dim_c ...].  Called by
 // all 32 lanes (mma.sync is warp-collective).  t indexes the records.  The exploration noise is keyed by (pa.epoch, t),
 // and in the episode form (EPISODES) by (epoch, step) = (pa.epoch + e, t - e * T) in episode e.  The categorical form
-// (CATEGORICAL) applies one-hot vectors instead of the softmax and writes the records of cr.
-template <class P, int H, int I, bool EPISODES = false, bool CATEGORICAL = false>
+// (CATEGORICAL) applies one-hot vectors instead of the softmax and writes the records of cr.  MAPPO evaluates MAPPO's
+// actor (MlpMappoArgs) with the same GEMMs: after the observation record, the input LayerNorm (net_flags &
+// kMappoFeatureNorm) normalises each lane's tile row in place; act_norm_tf32_frags replaces relu_tf32_frag; and since
+// the second LayerNorm needs a whole row of h2, layers 2 and 3 run one m-tile at a time (h2 of 16 rows in 32 fp32
+// registers, W2's B fragments read once per m-tile).
+template <class P, int H, int I, bool EPISODES = false, bool CATEGORICAL = false, bool MAPPO = false>
 __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typename P::W &w, const float *__restrict__ Wsm,
                                             float *s_warp, int lane, int t, int rows, bool active, int64_t w0, int64_t wi,
                                             float *cact, int step = 0, uint64_t epoch = 0,
-                                            const MlpCategoricalRecords *cr = nullptr) {
+                                            const MlpCategoricalRecords *cr = nullptr, float ln_eps = 0.0f,
+                                            uint32_t net_flags = 0) {
+    static_assert(!MAPPO || (CATEGORICAL && H == 64), "the MAPPO actor: categorical form, H = 64");
     using S = MlpShape<P, H>;
     constexpr int OD = P::obs_dim(I), KT1 = S::kt1(I), NT = S::NT, PITCH = ObsTile<OD>::kPitch;
     constexpr int AD = P::act_dim(I), NO = S::nout(I) / 8;
@@ -1053,6 +1141,23 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
     __syncwarp();
     if (pa.obs_rec[I] != nullptr)                          // the observation the actor sees at step t
         store_obs_rows<OD>(pa.obs_rec[I] + (static_cast<int64_t>(t) * n + w0) * OD, tile, lane, rows, active);
+    if constexpr (MAPPO) {
+        if (net_flags & kMappoFeatureNorm) {               // the record holds the raw observation; the actor sees it normalised
+            __syncwarp();                                  // every lane has streamed the tile
+            float *row = tile + lane * PITCH;              // odd pitch: conflict-free
+            float s = 0.0f;
+#pragma unroll
+            for (int c = 0; c < OD; ++c) s += row[c];
+            const float mu = s / static_cast<float>(OD);
+            float v = 0.0f;
+#pragma unroll
+            for (int c = 0; c < OD; ++c) { const float dc = row[c] - mu; v += dc * dc; }
+            const float rstd = rsqrtf(v / static_cast<float>(OD) + ln_eps);
+#pragma unroll
+            for (int c = 0; c < OD; ++c) row[c] = (row[c] - mu) * rstd;
+            __syncwarp();
+        }
+    }
     const int gq = lane >> 2, tq = lane & 3;
     // ---- layer 1: [32 x K1] . [K1 x H] + b1 ----
     float h[2][NT][4];
@@ -1086,10 +1191,15 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
         }
     }
     uint32_t x1[2][NT][4];
+    if constexpr (MAPPO) {
 #pragma unroll
-    for (int mt = 0; mt < 2; ++mt)
+        for (int mt = 0; mt < 2; ++mt) act_norm_tf32_frags<NT>(x1[mt], h[mt], net_flags & kMappoTanh, ln_eps);
+    } else {
 #pragma unroll
-        for (int nt = 0; nt < NT; ++nt) relu_tf32_frag(x1[mt][nt], h[mt][nt]);
+        for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) relu_tf32_frag(x1[mt][nt], h[mt][nt]);
+    }
     // ---- layers 2 and 3, one 8-unit tile of h2 at a time: logits += relu(x1 . W2^T[:, tile] + b2[tile]) . W3^T[tile, :]
     const float *W2 = Wsm + S::w2_off(I), *W3 = Wsm + S::w3_off(I), *B2 = Wsm + S::b2_off(I), *B3 = Wsm + S::b3_off(I);
     float lg[2][NO][4];
@@ -1099,6 +1209,30 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt) { lg[mt][ot][0] = b.x; lg[mt][ot][1] = b.y; lg[mt][ot][2] = b.x; lg[mt][ot][3] = b.y; }
     }
+    if constexpr (MAPPO) {   // ---- MAPPO: per m-tile, h2 = x1 . W2^T + b2 whole, act + LayerNorm, then logits += x2 . W3^T
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+            float c[NT][4];
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+                const float2 bb = *reinterpret_cast<const float2 *>(B2 + nt * 8 + 2 * tq);
+                c[nt][0] = bb.x; c[nt][1] = bb.y; c[nt][2] = bb.x; c[nt][3] = bb.y;
+#pragma unroll
+                for (int kt = 0; kt < NT; ++kt)
+                    mma_tf32(c[nt], x1[mt][kt], *reinterpret_cast<const float2 *>(W2 + ((kt * NT + nt) * 32 + lane) * 2));
+            }
+            uint32_t x2[NT][4];
+            act_norm_tf32_frags<NT>(x2, c, net_flags & kMappoTanh, ln_eps);
+#pragma unroll
+            for (int ot = 0; ot < NO; ++ot)
+#pragma unroll
+                for (int kt = 0; kt < NT; ++kt)
+                    mma_tf32(lg[mt][ot], x2[kt], *reinterpret_cast<const float2 *>(W3 + ((kt * NO + ot) * 32 + lane) * 2));
+            // a memory barrier for the compiler: it would otherwise keep all of W2's and W3's B fragments (up to 160
+            // registers) live from the first m-tile to the second instead of reading them again
+            __syncwarp();
+        }
+    } else {
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
         float c[2][4];
@@ -1121,6 +1255,7 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
                 mma_tf32(lg[mt][ot], x2, b3);
             }
         }
+    }
     }
     // ---- logits back to their lane (row r = world w0 + r) ----
 #pragma unroll
@@ -1198,16 +1333,17 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
     }
 }
 
-// the body of both forms; ea is null in the single-episode form (EPISODES = false), cr unless CATEGORICAL
-template <class P, int H, bool EPISODES, bool CATEGORICAL = false>
+// the body of both forms; ea is null in the single-episode form (EPISODES = false), cr unless CATEGORICAL; ln_eps and
+// net_flags are MAPPO's (MlpMappoArgs)
+template <class P, int H, bool EPISODES, bool CATEGORICAL = false, bool MAPPO = false>
 __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEpisodeArgs *ea,
-                                            const MlpCategoricalRecords *cr = nullptr) {
+                                            const MlpCategoricalRecords *cr = nullptr, float ln_eps = 0.0f,
+                                            uint32_t net_flags = 0) {
     static_assert(H == 32 || H == 64, "MLP policy rollout: hidden width 32 or 64");
     constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     using S = MlpShape<P, H>;
-    static_assert(mlp_block_warps<P, H, EPISODES, CATEGORICAL>() >= 1 &&
-                  (S::kWeightFloats + mlp_block_warps<P, H, EPISODES, CATEGORICAL>() * S::kWarpFloats) * 4 <= kMlpSmemBytes,
-                  "one block fits an SM");
+    constexpr int kWarps = MAPPO ? mappo_block_warps<P, EPISODES>() : mlp_block_warps<P, H, EPISODES, CATEGORICAL>();
+    static_assert(kWarps >= 1 && (S::kWeightFloats + kWarps * S::kWarpFloats) * 4 <= kMlpSmemBytes, "one block fits an SM");
     const StepArgs &a = pa.s;
     extern __shared__ __align__(16) float smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1270,8 +1406,9 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
             P::prepare(d, w);
             static_for<A>([&](auto ic) {
                 constexpr int i = decltype(ic)::value;
-                const float2 u = mlp_agent<P, H, i, EPISODES, CATEGORICAL>(pa, w, smem + S::agent_off(i), s_warp, lane, tg,
-                                                                           rows, active, w0, wi, cact, t, pa.epoch + e, cr);
+                const float2 u = mlp_agent<P, H, i, EPISODES, CATEGORICAL, MAPPO>(pa, w, smem + S::agent_off(i), s_warp, lane,
+                                                                                  tg, rows, active, w0, wi, cact, t,
+                                                                                  pa.epoch + e, cr, ln_eps, net_flags);
                 ux[i] = u.x;
                 uy[i] = u.y;
             });
@@ -1371,6 +1508,18 @@ template <class P, int H>
 __global__ void __launch_bounds__(mlp_block_warps<P, H, true, true>() * 32)
     mpe_policy_mlp_categorical_episode_kernel(const __grid_constant__ MlpCategoricalEpisodeArgs ca) {
     mlp_rollout<P, H, true, true>(ca.e.p, &ca.e, &ca.c);
+}
+
+template <class P>
+__global__ void __launch_bounds__(mappo_block_warps<P, false>() * 32)
+    mpe_policy_mappo_kernel(const __grid_constant__ MlpMappoArgs ma) {
+    mlp_rollout<P, 64, false, true, true>(ma.c.p, nullptr, &ma.c.c, ma.eps, ma.net_flags);
+}
+
+template <class P>
+__global__ void __launch_bounds__(mappo_block_warps<P, true>() * 32)
+    mpe_policy_mappo_episode_kernel(const __grid_constant__ MlpMappoEpisodeArgs ma) {
+    mlp_rollout<P, 64, true, true, true>(ma.c.e.p, &ma.c.e, &ma.c.c, ma.eps, ma.net_flags);
 }
 
 // ---- generic program for user scenarios (MPE_SCN_CUSTOM) ------------------------------------------
@@ -1558,6 +1707,7 @@ struct Program {
     // the same with the two-hidden-layer actor on the tensor cores, by form (episodes | categorical << 1) and H = 32 / 64:
     // the kernel and its warps per block at most (mlp_block_warps)
     struct { const void *fn; int warps; } mlp[kMlpForms][2];
+    struct { const void *fn; int warps; } mappo[2];   // MAPPO's actor (H = 64, categorical), one episode / episodes
     int mlp_weight_floats[2], mlp_warp_floats[2];
     int mlp_explore_stride;           // Philox blocks per (step, agent) of its exploration noise
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
@@ -1601,6 +1751,8 @@ static Program make_program() {
     if constexpr (MlpBuilt<P>::value) {
         set_mlp<P, 32>(p, 0);
         set_mlp<P, 64>(p, 1);
+        p.mappo[0] = {reinterpret_cast<const void *>(mpe_policy_mappo_kernel<P>), mappo_block_warps<P, false>()};
+        p.mappo[1] = {reinterpret_cast<const void *>(mpe_policy_mappo_episode_kernel<P>), mappo_block_warps<P, true>()};
         p.mlp_explore_stride = mlp_explore_stride<P>();
     }
     p.smem_bytes = Shape<P>::kWarpBytes;  // per warp
@@ -1738,6 +1890,10 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
                 if (prog->mlp[f][k].fn)
                     CUDA_TRY(cudaFuncSetAttribute(prog->mlp[f][k].fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                   (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp[f][k].warps) * 4));
+        for (int e = 0; e < 2; ++e)
+            if (prog->mappo[e].fn)
+                CUDA_TRY(cudaFuncSetAttribute(prog->mappo[e].fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (prog->mlp_weight_floats[1] + prog->mlp_warp_floats[1] * prog->mappo[e].warps) * 4));
         if (prog->rollout_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->rollout_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->rollout_smem * max_warps_per_block(prog->rollout_smem)));
@@ -2093,9 +2249,12 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
 
 // The arguments of the four two-hidden-layer rollout entry points, filled by name (several neighbours share a type).
 // form: episodes | categorical << 1.  T is the episode length (n_steps in the single-episode forms); a record the form
-// does not have is null.
+// does not have is null.  mappo: MAPPO's actor (categorical forms, H = 64) with net_flags and ln_eps (MlpMappoArgs).
 struct MlpCall {
     int form;
+    bool mappo;
+    uint32_t net_flags;
+    float ln_eps;
     void *pv;
     const void *lm;                   // writable in the episode forms: every episode end redraws them
     float *comm;
@@ -2119,6 +2278,9 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
         {"mpe_rollout_policy_mlp_episodes", "cudaLaunchKernelExC(rollout_policy_mlp_episodes)"},
         {"mpe_rollout_policy_mlp_categorical", "cudaLaunchKernelExC(rollout_policy_mlp_categorical)"},
         {"mpe_rollout_policy_mlp_categorical_episodes", "cudaLaunchKernelExC(rollout_policy_mlp_categorical_episodes)"}};
+    static const char *const kMappoName[2][2] = {
+        {"mpe_rollout_policy_mappo", "cudaLaunchKernelExC(rollout_policy_mappo)"},
+        {"mpe_rollout_policy_mappo_episodes", "cudaLaunchKernelExC(rollout_policy_mappo_episodes)"}};
     const bool episodes = c.form & 1, categorical = c.form & 2;
     const bool no_weights = !c.w[0] || !c.w[1] || !c.w[2] || !c.w[3] || !c.w[4] || !c.w[5];
     // the single-episode forms refuse a negative n_steps and null weight arrays before anything else, the episode forms
@@ -2127,7 +2289,11 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     if (h->device < 0) return MPE_ERR_NO_DEVICE;
     const int k = c.hidden == 32 ? 0 : (c.hidden == 64 ? 1 : -1);
     if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || h->prog->mlp[c.form][k].fn == nullptr) return MPE_ERR_UNSUPPORTED;
+    if (c.mappo && (k != 1 || h->prog->mappo[episodes].fn == nullptr)) return MPE_ERR_UNSUPPORTED;   // H = 64 only
     if (c.flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
+    // unknown network flags, or an eps that is negative, NaN or infinite
+    if (c.mappo && ((c.net_flags & ~(kMappoFeatureNorm | kMappoTanh)) || !(c.ln_eps >= 0.0f && c.ln_eps <= 3.4e38f)))
+        return MPE_ERR_BAD_ARG;
     // records are indexed by the global step e * episode_length + t, an int
     if (episodes && (c.T < 1 || c.episodes < 1 || static_cast<int64_t>(c.T) * c.episodes > 0x7fffffffLL))
         return MPE_ERR_BAD_ARG;
@@ -2135,7 +2301,7 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     if (c.explore && static_cast<int64_t>(c.T) * h->prog->A * h->prog->mlp_explore_stride > static_cast<int64_t>(kExploreTag))
         return MPE_ERR_BAD_ARG;
     if (no_weights || (c.rew_steps != nullptr && !ok4(c.rew_steps))) return MPE_ERR_BAD_ARG;
-    NvtxRange range(kName[c.form][0]);
+    NvtxRange range(c.mappo ? kMappoName[episodes][0] : kName[c.form][0]);
     MlpCategoricalRecords cr{};
     if (categorical) {
         if (c.logp_steps != nullptr && !ok4(c.logp_steps)) return MPE_ERR_BAD_ARG;
@@ -2173,15 +2339,20 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     ea.reset_epoch = c.reset_epoch;
     MlpCategoricalArgs ca{pa, cr};
     MlpCategoricalEpisodeArgs cea{ea, cr};
+    MlpMappoArgs ma{ca, c.ln_eps, c.net_flags};
+    MlpMappoEpisodeArgs mea{cea, c.ln_eps, c.net_flags};
     void *const form_args[kMlpForms] = {&pa, &ea, &ca, &cea};
+    void *const args = c.mappo ? (episodes ? static_cast<void *>(&mea) : static_cast<void *>(&ma)) : form_args[c.form];
+    const void *const fn = c.mappo ? h->prog->mappo[episodes].fn : h->prog->mlp[c.form][k].fn;
+    const int cap = c.mappo ? h->prog->mappo[episodes].warps : h->prog->mlp[c.form][k].warps;
     // every block stages all agents' weights once, so blocks are as large as possible while every SM still gets work
     const int64_t warps = (h->n + 31) / 32;
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
-    if (wpb > h->prog->mlp[c.form][k].warps) wpb = h->prog->mlp[c.form][k].warps;
-    return launch_persistent(h, h->prog->mlp[c.form][k].fn, warps, wpb, static_cast<size_t>(h->prog->mlp_weight_floats[k]) * 4,
-                             static_cast<size_t>(h->prog->mlp_warp_floats[k]) * 4, form_args[c.form], c.stream,
-                             kName[c.form][1]);
+    if (wpb > cap) wpb = cap;
+    return launch_persistent(h, fn, warps, wpb, static_cast<size_t>(h->prog->mlp_weight_floats[k]) * 4,
+                             static_cast<size_t>(h->prog->mlp_warp_floats[k]) * 4, args, c.stream,
+                             c.mappo ? kMappoName[episodes][1] : kName[c.form][1]);
 }
 
 extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
@@ -2256,6 +2427,46 @@ extern "C" int mpe_rollout_policy_mlp_categorical_episodes(
     c.form = 3; c.T = episode_length; c.episodes = n_episodes; c.rew = ep_rew;
     c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
     c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
+    return rollout_policy_mlp(h, c);
+}
+
+extern "C" int mpe_rollout_policy_mappo(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
+                                        const float *const *w1_n, const float *const *b1_n, const float *const *w2_n,
+                                        const float *const *b2_n, const float *const *w3_n, const float *const *b3_n,
+                                        int32_t hidden, int32_t n_steps, int32_t explore, uint64_t explore_seed,
+                                        uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n, float *rew_sum,
+                                        float *rew_steps, float *logp_steps, int32_t *const *act_index_record_n,
+                                        float *const *obs_record_n, uint32_t net_flags, float ln_eps, uint8_t *done,
+                                        uint32_t flags, void *stream) {
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.w[0] = w1_n; c.w[1] = b1_n; c.w[2] = w2_n; c.w[3] = b2_n; c.w[4] = w3_n; c.w[5] = b3_n;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = 2; c.T = n_steps; c.episodes = 1; c.rew = rew_sum;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    c.mappo = true; c.net_flags = net_flags; c.ln_eps = ln_eps;
+    return rollout_policy_mlp(h, c);
+}
+
+extern "C" int mpe_rollout_policy_mappo_episodes(
+    mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal, const float *const *w1_n, const float *const *b1_n,
+    const float *const *w2_n, const float *const *b2_n, const float *const *w3_n, const float *const *b3_n, int32_t hidden,
+    int32_t episode_length, int32_t n_episodes, int32_t explore, uint64_t explore_seed, uint64_t explore_epoch,
+    uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew, float *rew_steps,
+    float *logp_steps, int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n,
+    uint32_t net_flags, float ln_eps, uint8_t *done, uint32_t flags, void *stream) {
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.w[0] = w1_n; c.w[1] = b1_n; c.w[2] = w2_n; c.w[3] = b2_n; c.w[4] = w3_n; c.w[5] = b3_n;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = 3; c.T = episode_length; c.episodes = n_episodes; c.rew = ep_rew;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
+    c.mappo = true; c.net_flags = net_flags; c.ln_eps = ln_eps;
     return rollout_policy_mlp(h, c);
 }
 

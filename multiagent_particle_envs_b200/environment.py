@@ -294,8 +294,18 @@ class MultiAgentEnv(_Env):
         log_softmax(logits)[k] on the logits the kernel acted with (Categorical(logits).log_prob(k), the behaviour
         policy's term of PPO's ratio), else None.  Returns, observations, episode_length and both epochs behave as in
         the default mode.  An unknown action_mode, or record_log_probs in the default mode, raises ValueError; the
-        one-hidden-layer actor raises NotImplementedError.  Actors with LayerNorm or tanh layers (MAPPO's default MLP)
-        are not this network and are refused."""
+        one-hidden-layer actor raises NotImplementedError.
+
+        MAPPO's MLP actor (mpe_rollout_policy_mappo, action_mode="categorical" only): policies[i] is an
+        `nn.Sequential([LayerNorm(obs_dim_i)], Linear(obs_dim_i, 64), Act, LayerNorm(64), Linear(64, 64), Act,
+        LayerNorm(64), Linear(64, act_dim_i))` -- MAPPO's MLPBase (layer_N = 1, the optional input LayerNorm being
+        use_feature_normalization) and its categorical head -- with Act = ReLU() or Tanh(), the same everywhere, and one
+        LayerNorm eps for all.  One module object may serve all agents (share_policy).  Any policy with a LayerNorm takes
+        this path, and mappo_actor_params checks the layer list (ValueError).  Each LayerNorm's affine is folded into the
+        next Linear (float64, then float32); the kernel normalises with fp32 statistics and TF32 GEMM operands.  Records,
+        extras, sampling, log-probabilities and episodes are those of the categorical mode above; observation records and
+        final observations hold the raw observations (before the input LayerNorm).  action_mode="softmax" and a hidden
+        width other than 64 raise NotImplementedError.  GRU actors are not supported."""
         import torch
         world = self.world
         if action_mode not in ("softmax", "categorical"):
@@ -312,6 +322,15 @@ class MultiAgentEnv(_Env):
                                            or int(n_steps) % int(episode_length) != 0):
             raise ValueError("rollout_policy: n_steps (%d) must be a positive multiple of episode_length (%d)"
                              % (int(n_steps), int(episode_length)))
+        if any(_has_layer_norm(p) for p in policies):
+            if action_mode != "categorical":
+                raise NotImplementedError("rollout_policy: MAPPO's actor (LayerNorm layers) has action_mode='categorical' "
+                                          "only")
+            if _mappo_hidden_widths(policies) - {MAPPO_HIDDEN}:
+                raise NotImplementedError("rollout_policy: MAPPO's actor is built for hidden width %d only; got %s"
+                                          % (MAPPO_HIDDEN, sorted(_mappo_hidden_widths(policies))))
+            return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
+                                            explore_seed, episode_length, True, record_log_probs, mappo=True)
         if any(_has_two_hidden_layers(p) for p in policies):
             return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
                                             explore_seed, episode_length, action_mode == "categorical", record_log_probs)
@@ -357,13 +376,19 @@ class MultiAgentEnv(_Env):
         return list(out.obs), list(out.rew_list), list(out.done_list), info_n, {"actions": actions, "rewards": rew_steps}
 
     def _rollout_policy_mlp(self, policies, n_steps, record_actions, per_step_rewards, record_observations, explore_seed,
-                            episode_length=None, categorical=False, record_log_probs=False):
+                            episode_length=None, categorical=False, record_log_probs=False, mappo=False):
         import torch
         world = self.world
         nw = world.bind()
         N, T = nw.n_env, int(n_steps)
         nw.require_mlp_actor()   # a program without the kernel is refused as such, before its heads are checked
-        params, hidden = mlp_actor_params(policies, nw.obs_dims, nw.act_dims)
+        if mappo:
+            params, tanh, feature_norm, eps = mappo_actor_params(policies, nw.obs_dims, nw.act_dims)
+            hidden = MAPPO_HIDDEN
+            net = ((_lib.MAPPO_FEATURE_NORM if feature_norm else 0) | (_lib.MAPPO_TANH if tanh else 0), eps)
+        else:
+            params, hidden = mlp_actor_params(policies, nw.obs_dims, nw.act_dims)
+            net = None
         keep = [[t.detach().to(device=nw.device, dtype=torch.float32).contiguous() for t in p] for p in params]
         w_ptrs = [_lib.ptr_array([keep[i][j].data_ptr() for i in range(self.n)]) for j in range(6)]
         out = nw.out if self.reuse_buffers else nw.new_outputs()
@@ -390,7 +415,8 @@ class MultiAgentEnv(_Env):
         nw.rollout_policy_mlp(w_ptrs, hidden, T, out, self._flags(), episode_length=episode_length, categorical=categorical,
                               rew_steps=rew_steps, act_rec_ptrs=act_ptrs, obs_rec_ptrs=obs_ptrs,
                               final_obs_ptrs=_lib.ptr_array([o.data_ptr() for o in final]) if final is not None else None,
-                              logp_steps=log_probs, ep_rew=ep_rew, explore_seed=seed, explore_epoch=self.explore_epoch)
+                              logp_steps=log_probs, ep_rew=ep_rew, explore_seed=seed, explore_epoch=self.explore_epoch,
+                              mappo=net)
         if episode_length is None:
             reward_n = list(out.rew_list)
         else:
@@ -715,3 +741,93 @@ def mlp_actor_params(policies, obs_dims, act_dims=None):
                                 ", ".join(str(list(s)) for s in got)))
         params.append(tuple(ts))
     return params, hidden
+
+
+# ---- MAPPO's MLP actor (MLPBase with layer_N = 1 and a categorical ACTLayer head) ----------------------------------
+MAPPO_HIDDEN = 64
+_MAPPO_SHAPE = ("nn.Sequential([LayerNorm(obs_dim)], Linear(obs_dim, 64), Act, LayerNorm(64), Linear(64, 64), Act, "
+                "LayerNorm(64), Linear(64, act_dim)) with Act = ReLU() or Tanh()")
+
+
+def _has_layer_norm(pol):
+    """does this policy ask for MAPPO's actor?  (A module with a LayerNorm; mappo_actor_params checks the rest.)"""
+    import torch
+    return isinstance(pol, torch.nn.Module) and any(isinstance(m, torch.nn.LayerNorm) for m in pol.modules())
+
+
+def _mappo_hidden_widths(policies):
+    """the output width of every MAPPO policy's first Linear layer (what the kernel's H would be)"""
+    import torch
+    out = set()
+    for pol in policies:
+        lin = [m for m in pol.modules() if isinstance(m, torch.nn.Linear)] if isinstance(pol, torch.nn.Module) else []
+        if lin:
+            out.add(int(lin[0].out_features))
+    return out
+
+
+def mappo_actor_params(policies, obs_dims, act_dims=None):
+    """MAPPO's actor -> (params, tanh, feature_norm, eps), or ValueError.  Every policy must be an nn.Sequential whose
+    layers are exactly
+        [LayerNorm(obs_dim_i)], Linear(obs_dim_i, 64), Act, LayerNorm(64), Linear(64, 64), Act, LayerNorm(64),
+        Linear(64, act_dim_i)
+    with Act = ReLU() or Tanh(), the same in both places and for all agents; the input LayerNorm (MAPPO's
+    use_feature_normalization) for all agents or none; every LayerNorm with elementwise_affine=True and one eps for all;
+    every Linear with a bias.  One module object may serve several agents (MAPPO's share_policy).  act_dims None means 5
+    for every agent.
+
+    params[i] = (W1', b1', W2', b2', W3', b3') in float64, torch's Linear layout: the network with each LayerNorm's
+    affine folded into the Linear after it, W' = W diag(gamma), b' = b + W beta, so that the kernel needs only the
+    parameter-free (x - mu) * rsqrt(var + eps).  No device is needed."""
+    import torch
+    nn = torch.nn
+    if act_dims is None:
+        act_dims = [5] * len(obs_dims)
+    if len(policies) != len(obs_dims):
+        raise ValueError("expected %d policies, got %d" % (len(obs_dims), len(policies)))
+    H = MAPPO_HIDDEN
+    params, acts, feature_norms, eps = [], set(), set(), set()
+    for i, pol in enumerate(policies):
+        layers = [m for m in pol.modules() if not list(m.children())] if isinstance(pol, nn.Module) else []
+        names = " -> ".join(type(m).__name__ for m in layers)
+        fn = len(layers) == 8 and type(layers[0]) is nn.LayerNorm
+        body = layers[1:] if fn else layers
+        ok = (isinstance(pol, nn.Sequential) and len(body) == 7
+              and all(type(body[k]) is nn.Linear for k in (0, 3, 6))
+              and all(type(body[k]) is nn.LayerNorm for k in (2, 5))
+              and type(body[1]) in (nn.ReLU, nn.Tanh) and type(body[4]) is type(body[1]))
+        if not ok:
+            raise ValueError("policy %d must be %s; got %s (%s)" % (i, _MAPPO_SHAPE, type(pol).__name__, names))
+        lins, norms = (body[0], body[3], body[6]), ((layers[0] if fn else None), body[2], body[5])
+        if any(ln is not None and ln.weight is None for ln in norms):
+            raise ValueError("policy %d: every LayerNorm needs elementwise_affine=True" % i)
+        if any(lin.bias is None for lin in lins):
+            raise ValueError("policy %d: every Linear layer needs a bias" % i)
+        od, ad = obs_dims[i], act_dims[i]
+        want = ((H, od), (H, H), (ad, H))
+        got = tuple(tuple(lin.weight.shape) for lin in lins)
+        ln_want = ((od,), (H,), (H,))
+        ln_got = tuple(None if ln is None else tuple(ln.normalized_shape) for ln in norms)
+        if got != want or any(g is not None and g != w for g, w in zip(ln_got, ln_want)):
+            raise ValueError("policy %d: expected Linear weights %s and LayerNorm shapes %s (hidden width %d only); got "
+                             "%s and %s" % (i, list(want), list(ln_want), H, list(got), list(ln_got)))
+        acts.add(type(body[1]))
+        feature_norms.add(fn)
+        eps.update(float(ln.eps) for ln in norms if ln is not None)
+        p = []
+        for lin, ln in zip(lins, norms):
+            W, b = lin.weight.detach().to(torch.float64), lin.bias.detach().to(torch.float64)
+            if ln is not None:
+                g = ln.weight.detach().to(torch.float64)
+                beta = ln.bias.detach().to(torch.float64) if ln.bias is not None else torch.zeros_like(g)
+                W, b = W * g, b + W @ beta
+            p += [W, b]
+        params.append(tuple(p))
+    if len(acts) != 1:
+        raise ValueError("every policy must use the same activation (ReLU or Tanh); got %s"
+                         % sorted(a.__name__ for a in acts))
+    if len(feature_norms) != 1:
+        raise ValueError("the input LayerNorm (feature normalisation) must be on for every policy or for none")
+    if len(eps) != 1:
+        raise ValueError("every LayerNorm must have the same eps; got %s" % sorted(eps))
+    return params, acts.pop() is nn.Tanh, feature_norms.pop(), eps.pop()

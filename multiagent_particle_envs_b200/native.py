@@ -284,7 +284,7 @@ class NativeWorld(ShapeHandle):
 
     def rollout_policy_mlp(self, w_ptrs, hidden, n_steps, out=None, flags=0, *, episode_length=None, categorical=False,
                            rew_steps=None, act_rec_ptrs=None, obs_rec_ptrs=None, final_obs_ptrs=None, logp_steps=None,
-                           ep_rew=None, explore_seed=None, explore_epoch=0):
+                           ep_rew=None, explore_seed=None, explore_epoch=0, mappo=None):
         """n_steps fused steps in ONE launch with every agent's two-hidden-layer actor evaluated on the tensor cores
         (mpe_rollout_policy_mlp); w_ptrs: the six pointer arrays (W1, b1, W2, b2, W3, b3), one device pointer per
         agent each.  explore_seed (not None) switches the Gumbel-softmax sampling on.
@@ -297,9 +297,14 @@ class NativeWorld(ShapeHandle):
         the reset that `reset()` would draw, inside the kernel.  The resets use the epochs `reset()` would use next, and
         self.epoch (and the device epoch, if enabled) advances by the number of episodes.  ep_rew: float32 [episodes, A,
         N] CUDA tensor receiving each episode's returns; out.obs receives the observations of the state after the last
-        reset; final_obs_ptrs: one [episodes, N, obs_dim_i] record per agent of each episode's last observation."""
+        reset; final_obs_ptrs: one [episodes, N, obs_dim_i] record per agent of each episode's last observation.
+
+        mappo=(net_flags, eps) (mpe_rollout_policy_mappo[_episodes], categorical only): MAPPO's actor, w_ptrs holding
+        its folded network (environment.mappo_actor_params); net_flags is _lib.MAPPO_FEATURE_NORM | _lib.MAPPO_TANH."""
         out = out or self.out
         episodes = episode_length is not None
+        if mappo is not None and not categorical:
+            raise ValueError("rollout_policy_mlp: the MAPPO actor has the categorical form only")
         if episodes and self.torch.cuda.is_current_stream_capturing():
             raise RuntimeError("rollout_policy with episode_length cannot be captured in a CUDA graph: the reset epoch "
                                "is a launch argument")
@@ -308,18 +313,23 @@ class NativeWorld(ShapeHandle):
         explore_args = (int(explore), int(explore_seed) if explore else 0, int(explore_epoch))
         rew_ptr = rew_steps.data_ptr() if rew_steps is not None else None
         logp = (logp_steps.data_ptr() if logp_steps is not None else None,) if categorical else ()
-        name = "mpe_rollout_policy_mlp" + ("_categorical" if categorical else "") + ("_episodes" if episodes else "")
+        if mappo is not None:
+            name = "mpe_rollout_policy_mappo" + ("_episodes" if episodes else "")
+            net = (int(mappo[0]), float(mappo[1]))
+        else:
+            name = "mpe_rollout_policy_mlp" + ("_categorical" if categorical else "") + ("_episodes" if episodes else "")
+            net = ()
         if episodes:
             epoch = int(self._epoch_dev.item()) if self._epoch_dev is not None else self.epoch
             n_episodes = int(n_steps) // int(episode_length)
             rc = getattr(self.lib, name)(self.handle, pv, lm, comm, goal, *w_ptrs, int(hidden), int(episode_length),
                                          n_episodes, *explore_args, self.seed, epoch, self.world_offset, out.obs_ptrs,
                                          ep_rew.data_ptr(), rew_ptr, *logp, act_rec_ptrs, obs_rec_ptrs, final_obs_ptrs,
-                                         out.done_ptr, flags, self._stream())
+                                         *net, out.done_ptr, flags, self._stream())
         else:
             rc = getattr(self.lib, name)(self.handle, pv, lm, comm, goal, *w_ptrs, int(hidden), int(n_steps), *explore_args,
                                          self.world_offset, out.obs_ptrs, out.rew_ptr, rew_ptr, *logp, act_rec_ptrs,
-                                         obs_rec_ptrs, out.done_ptr, flags, self._stream())
+                                         obs_rec_ptrs, *net, out.done_ptr, flags, self._stream())
         check(rc, name)
         if episodes:
             self.epoch = epoch + n_episodes

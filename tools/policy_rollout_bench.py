@@ -7,6 +7,10 @@
       --categorical: policy-gradient actions (action_mode="categorical", --layers 3 only): the one-hot vector of the
       arg-max of the logits (--explore: of the Gumbel-perturbed logits) per sub-space, recording the indices and the
       log-probabilities;
+      --actor mappo: MAPPO's actor ([LayerNorm] - Linear - Act - LayerNorm - Linear - Act - LayerNorm - Linear, H = 64,
+      mpe_rollout_policy_mappo), --categorical and --layers 3 implied; --tanh for Act = Tanh (else ReLU),
+      --feature-norm for the input LayerNorm.  The MADDPG categorical kernel is timed in the same run
+      ("maddpg_in_kernel"), so the cost of the LayerNorms and the tanh shows;
   (b) the same actors as torch modules + env.step, all captured in one CUDA graph (rollout.GraphedRollout); with
       --categorical the graphed policy takes argmax(logits - log(-log u)) per sub-space, its one_hot and
       log_softmax(logits).gather(k) for the log-probabilities.
@@ -58,7 +62,15 @@ def main():
     ap.add_argument("--explore", action="store_true", help="Gumbel-softmax exploration (--layers 3)")
     ap.add_argument("--categorical", action="store_true",
                     help="one-hot arg-max actions with index and log-probability records (--layers 3)")
+    ap.add_argument("--actor", choices=("maddpg", "mappo"), default="maddpg",
+                    help="mappo: MAPPO's LayerNorm actor (implies --layers 3 --categorical)")
+    ap.add_argument("--tanh", action="store_true", help="MAPPO's actor with Tanh instead of ReLU")
+    ap.add_argument("--feature-norm", action="store_true", help="MAPPO's actor with the input LayerNorm")
     args = ap.parse_args()
+    if args.actor == "mappo":
+        args.layers, args.categorical = 3, True
+    elif args.tanh or args.feature_norm:
+        ap.error("--tanh and --feature-norm need --actor mappo")
     try:
         skw = {k: int(v) for k, v in (kv.split("=", 1) for kv in args.scenario_kwargs)}
     except ValueError:
@@ -84,26 +96,43 @@ def main():
     else:
         mods = [torch.nn.Sequential(torch.nn.Linear(od, H), torch.nn.ReLU(), torch.nn.Linear(H, H), torch.nn.ReLU(),
                                     torch.nn.Linear(H, ad)).to(dev) for od, ad in zip(nw.obs_dims, nw.act_dims)]
+    maddpg_mods = None
+    if args.actor == "mappo":
+        nn = torch.nn
+        Act = nn.Tanh if args.tanh else nn.ReLU
+        maddpg_mods = mods
+        mods = [nn.Sequential(*(([nn.LayerNorm(od)] if args.feature_norm else []) +
+                                [nn.Linear(od, H), Act(), nn.LayerNorm(H), nn.Linear(H, H), Act(), nn.LayerNorm(H),
+                                 nn.Linear(H, ad)])).to(dev) for od, ad in zip(nw.obs_dims, nw.act_dims)]
     segs = sub_spaces(env.world) if args.layers == 3 else [[5]] * len(nw.obs_dims)
     res = {"config": {"scenario": args.scenario, "scenario_kwargs": skw, "n_env": n, "T": T, "hidden": H}}
     if args.layers == 3:
         res["config"].update(layers=3, explore=args.explore, categorical=args.categorical,
                              torch_float32_matmul_precision=torch.get_float32_matmul_precision())
+    if args.actor == "mappo":
+        res["config"].update(actor="mappo", tanh=args.tanh, feature_norm=args.feature_norm)
     kw = {"explore_seed": 1} if args.explore else {}
     if args.categorical:
         kw.update(action_mode="categorical", record_actions=True, record_log_probs=True)
     # (a) in-kernel actors
-    for _ in range(2):
-        env.rollout_policy(mods, T, **kw)
-    torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(args.reps):
-        env.rollout_policy(mods, T, **kw)
-    e1.record()
-    torch.cuda.synchronize()
-    sec = e0.elapsed_time(e1) / 1e3 / (args.reps * T)
+
+    def time_in_kernel(ms):
+        for _ in range(2):
+            env.rollout_policy(ms, T, **kw)
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(args.reps):
+            env.rollout_policy(ms, T, **kw)
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / 1e3 / (args.reps * T)
+
+    sec = time_in_kernel(mods)
     res["in_kernel"] = {"us_per_step": 1e6 * sec, "env_steps_per_sec": n / sec}
+    if maddpg_mods is not None:   # the MADDPG categorical kernel on the same env, same sizes
+        sec_m = time_in_kernel(maddpg_mods)
+        res["maddpg_in_kernel"] = {"us_per_step": 1e6 * sec_m, "env_steps_per_sec": n / sec_m}
     if args.layers == 3:
         flops = actor_flops_per_step(nw.obs_dims, nw.act_dims, H, n)
         res["in_kernel"].update(actor_flop_per_step=flops, actor_tflops=flops / sec / 1e12)

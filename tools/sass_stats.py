@@ -141,6 +141,20 @@ def main():
         print("|---|---|---|---|---|---|---|---|---|")
         for r in sorted(mlp):
             print("| " + " | ".join(str(x) for x in r) + " |")
+    mappo = []
+    for mangled, (reg, stack) in usage.items():
+        m = re.match(r"void mpe::mpe_policy_mappo(_episode)?_kernel<mpe::(.+?)\s*>\(", names[mangled])
+        if m:
+            c = mix.get(mangled, {})
+            mappo.append((m.group(2), "episodes" if m.group(1) else "one episode", reg, stack, c["total"], c["HMMA"],
+                          c["LDS"], c["MUFU"]))
+    if mappo:
+        print("\n## Closed-loop rollout with MAPPO's LayerNorm actor (`mpe_policy_mappo_kernel`, "
+              "`mpe_policy_mappo_episode_kernel`, categorical, H = 64)\n")
+        print("| program | form | regs | stack | instr | HMMA | LDS | MUFU |")
+        print("|---|---|---|---|---|---|---|---|")
+        for r in sorted(mappo):
+            print("| " + " | ".join(str(x) for x in r) + " |")
     other = [(names[k], v) for k, v in usage.items() if "mpe_kernel" not in names[k] or ", 0, " not in names[k]]
     spills = [n for n, (r, s) in other if s]
     print("\nOther kernels with a non-zero stack frame: %s" % (", ".join("`%s`" % s for s in spills) or "none"))
