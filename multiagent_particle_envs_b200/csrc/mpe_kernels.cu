@@ -927,31 +927,36 @@ struct MlpShape {
 //    (ptxas -v): then 12, or 8 where 168 spills too.  At H = 64 every program with four or more agents (their state
 //    next to the 64 registers of h1) and simple_reference (two 8-column logit tiles and 20 comm floats next to h1)
 //    take 12; the exceptions below are the rest.  The episode form adds the reset draw and the episode-end stores, the
-//    categorical form the arg-max, the log-probability and the index stores, so an exception names the forms it holds
-//    for.
+//    categorical form the arg-max, the log-probability and the index stores, and MAPPO's actor a second 32-register
+//    m-tile of h2 next to h1 for its LayerNorms (see mlp_agent), so an exception names the forms it holds for.
 //  - shared memory (mlp_smem_warps): the weights plus kWarpFloats per warp within the 227 KB a block may opt in to on
 //    H100.  Below the register limit only for tag 6+2 at H = 64 (212 KB of weights, 3 warps).
-// The forms, indexed by episodes | categorical << 1, and the masks an exception lists them by
-enum : int { kMlpForms = 4, kFormS = 1, kFormE = 2, kFormC = 4, kFormCE = 8, kFormAll = 15 };
+// The forms, indexed by episodes | kind << 1 with kind 0 for softmax actions, 1 for categorical ones and 2 for MAPPO's
+// actor (categorical records, H = 64 only), and the masks an exception lists them by
+enum : int { kMlpForms = 6, kFormS = 1, kFormE = 2, kFormC = 4, kFormCE = 8, kFormM = 16, kFormME = 32, kFormAll = 63 };
 template <int FORMS, int WARPS>
 struct MlpException { static constexpr int forms = FORMS, warps = WARPS; };
-// One exception per (program, H), so that no kernel matches two: a second one would redefine the specialisation
+// One exception per (program, H), so that no kernel matches two: a second one would redefine the specialisation.  The
+// stack ptxas -v showed without it, by form: MADDPG's (S, E, C, CE), then MAPPO's (M, ME)
 template <class P, int H> struct MlpRegisterException : MlpException<0, 0> {};
-template <> struct MlpRegisterException<Spread<2>, 64> : MlpException<kFormAll, 12> {};                   // 8 bytes of stack at 128
-template <> struct MlpRegisterException<Tag<1, 1, 2>, 64> : MlpException<kFormAll, 12> {};                // 8 at 128
-template <> struct MlpRegisterException<Tag<2, 1, 2>, 64> : MlpException<kFormAll, 12> {};                // 8 at 128
-template <> struct MlpRegisterException<Spread<6>, 64> : MlpException<kFormAll, 8> {};                    // 16 at 168
-template <> struct MlpRegisterException<Spread<6>, 32> : MlpException<kFormAll, 12> {};                   // 48 at 128
-template <> struct MlpRegisterException<Tag<4, 2, 2>, 32> : MlpException<kFormAll, 12> {};                // 16 at 128
-template <> struct MlpRegisterException<Tag<6, 2, 3>, 32> : MlpException<kFormAll, 8> {};                 // 64 at 128, 8 at 168
-template <> struct MlpRegisterException<SpeakerListener, 64> : MlpException<kFormE | kFormCE, 12> {};     // 8 at 128
-template <> struct MlpRegisterException<Adversary<1, 2, 2>, 64> : MlpException<kFormE | kFormCE, 12> {};  // 16 at 128
-template <> struct MlpRegisterException<Reference, 64> : MlpException<kFormE | kFormCE, 8> {};            // 8 at 168
-template <> struct MlpRegisterException<Tag<4, 2, 2>, 64> : MlpException<kFormE | kFormCE, 8> {};         // 8 at 168
-template <> struct MlpRegisterException<Spread<3>, 64> : MlpException<kFormE | kFormC | kFormCE, 12> {};  // 8 at 128
-template <> struct MlpRegisterException<Push<1, 1, 2>, 64> : MlpException<kFormC | kFormCE, 12> {};       // 8 at 128
-template <> struct MlpRegisterException<Crypto, 64> : MlpException<kFormCE, 12> {};                       // 16 at 128
-template <> struct MlpRegisterException<Spread<4>, 64> : MlpException<kFormCE, 8> {};                     // 8 at 168
+template <> struct MlpRegisterException<Spread<2>, 64> : MlpException<kFormAll, 12> {};      // 8 bytes at 128; M, ME 16, 24 at 128
+template <> struct MlpRegisterException<Tag<1, 1, 2>, 64> : MlpException<kFormAll, 12> {};   // 8 at 128; M, ME 16, 24 at 128
+template <> struct MlpRegisterException<Tag<2, 1, 2>, 64> : MlpException<kFormAll, 12> {};   // 8 at 128; M, ME 56, 56 at 128
+template <> struct MlpRegisterException<Spread<6>, 64> : MlpException<kFormAll, 8> {};       // 16 at 168; M, ME 64, 56 at 168
+template <> struct MlpRegisterException<Spread<6>, 32> : MlpException<kFormAll, 12> {};      // 48 at 128
+template <> struct MlpRegisterException<Tag<4, 2, 2>, 32> : MlpException<kFormAll, 12> {};   // 16 at 128
+template <> struct MlpRegisterException<Tag<6, 2, 3>, 32> : MlpException<kFormAll, 8> {};    // 64 at 128, 8 at 168
+template <> struct MlpRegisterException<SpeakerListener, 64>
+    : MlpException<kFormE | kFormCE | kFormM | kFormME, 12> {};                                 // 8 at 128; M, ME 16, 16 at 128
+template <> struct MlpRegisterException<Adversary<1, 2, 2>, 64>
+    : MlpException<kFormE | kFormCE | kFormM | kFormME, 12> {};                                 // 16 at 128; M, ME 32, 40 at 128
+template <> struct MlpRegisterException<Reference, 64> : MlpException<kFormE | kFormCE, 8> {};             // 8 at 168
+template <> struct MlpRegisterException<Tag<4, 2, 2>, 64> : MlpException<kFormE | kFormCE, 8> {};          // 8 at 168
+template <> struct MlpRegisterException<Spread<3>, 64>
+    : MlpException<kFormE | kFormC | kFormCE | kFormM | kFormME, 12> {};                        // 8 at 128; M, ME 32, 32 at 128
+template <> struct MlpRegisterException<Push<1, 1, 2>, 64> : MlpException<kFormC | kFormCE, 12> {};        // 8 at 128
+template <> struct MlpRegisterException<Crypto, 64> : MlpException<kFormCE | kFormM, 12> {};               // 16 at 128; M 8 at 128
+template <> struct MlpRegisterException<Spread<4>, 64> : MlpException<kFormCE, 8> {};                      // 8 at 168
 template <class P, int H>
 __host__ __device__ constexpr int mlp_register_rule() { return (H == 64 && (P::A >= 4 || mlp_max_act_dim<P>() > 8)) ? 12 : 16; }
 template <class P, int H, int FORM>
@@ -964,27 +969,9 @@ template <class P, int H>
 __host__ __device__ constexpr int mlp_smem_warps() {
     return (kMlpSmemBytes / 4 - MlpShape<P, H>::kWeightFloats) / MlpShape<P, H>::kWarpFloats;
 }
-template <class P, int H, bool EPISODES = false, bool CATEGORICAL = false>
+template <class P, int H, int FORM>
 __host__ __device__ constexpr int mlp_block_warps() {
-    constexpr int r = mlp_register_warps<P, H, EPISODES | CATEGORICAL << 1>(), s = mlp_smem_warps<P, H>();
-    return r < s ? r : s;
-}
-// The MAPPO actor's kernels (mpe_policy_mappo[_episode]_kernel, categorical, H = 64): the same shapes and shared-memory
-// limit, the general rule of H = 64 above, and their own exceptions, by the categorical forms' masks (kFormC: one
-// episode, kFormCE: episodes) -- the three LayerNorms keep a second 32-register m-tile of h2 next to h1 (see mlp_agent)
-template <class P> struct MappoRegisterException : MlpException<0, 0> {};
-template <> struct MappoRegisterException<Spread<2>> : MlpException<kFormC | kFormCE, 12> {};           // 16, 24 bytes of stack at 128
-template <> struct MappoRegisterException<Spread<3>> : MlpException<kFormC | kFormCE, 12> {};           // 32, 32 at 128
-template <> struct MappoRegisterException<Spread<6>> : MlpException<kFormC | kFormCE, 8> {};            // 64, 56 at 168
-template <> struct MappoRegisterException<Tag<1, 1, 2>> : MlpException<kFormC | kFormCE, 12> {};        // 16, 24 at 128
-template <> struct MappoRegisterException<Tag<2, 1, 2>> : MlpException<kFormC | kFormCE, 12> {};        // 56, 56 at 128
-template <> struct MappoRegisterException<SpeakerListener> : MlpException<kFormC | kFormCE, 12> {};     // 16, 16 at 128
-template <> struct MappoRegisterException<Adversary<1, 2, 2>> : MlpException<kFormC | kFormCE, 12> {};  // 32, 40 at 128
-template <> struct MappoRegisterException<Crypto> : MlpException<kFormC, 12> {};                        // 8 at 128
-template <class P, bool EPISODES>
-__host__ __device__ constexpr int mappo_block_warps() {
-    using X = MappoRegisterException<P>;
-    constexpr int r = (X::forms >> (EPISODES | 2) & 1) ? X::warps : mlp_register_rule<P, 64>(), s = mlp_smem_warps<P, 64>();
+    constexpr int r = mlp_register_warps<P, H, FORM>(), s = mlp_smem_warps<P, H>();
     return r < s ? r : s;
 }
 // the two programs whose weights fill most of the 227 KB
@@ -1342,7 +1329,7 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
     static_assert(H == 32 || H == 64, "MLP policy rollout: hidden width 32 or 64");
     constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     using S = MlpShape<P, H>;
-    constexpr int kWarps = MAPPO ? mappo_block_warps<P, EPISODES>() : mlp_block_warps<P, H, EPISODES, CATEGORICAL>();
+    constexpr int kWarps = mlp_block_warps<P, H, EPISODES | (MAPPO ? 2 : CATEGORICAL) << 1>();
     static_assert(kWarps >= 1 && (S::kWeightFloats + kWarps * S::kWarpFloats) * 4 <= kMlpSmemBytes, "one block fits an SM");
     const StepArgs &a = pa.s;
     extern __shared__ __align__(16) float smem[];
@@ -1488,36 +1475,36 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
 }
 
 template <class P, int H>
-__global__ void __launch_bounds__(mlp_block_warps<P, H>() * 32) mpe_policy_mlp_rollout_kernel(const __grid_constant__ MlpPolicyArgs pa) {
+__global__ void __launch_bounds__(mlp_block_warps<P, H, 0>() * 32) mpe_policy_mlp_rollout_kernel(const __grid_constant__ MlpPolicyArgs pa) {
     mlp_rollout<P, H, false>(pa, nullptr);
 }
 
 template <class P, int H>
-__global__ void __launch_bounds__(mlp_block_warps<P, H, true>() * 32)
+__global__ void __launch_bounds__(mlp_block_warps<P, H, 1>() * 32)
     mpe_policy_mlp_episode_kernel(const __grid_constant__ MlpEpisodeArgs ea) {
     mlp_rollout<P, H, true>(ea.p, &ea);
 }
 
 template <class P, int H>
-__global__ void __launch_bounds__(mlp_block_warps<P, H, false, true>() * 32)
+__global__ void __launch_bounds__(mlp_block_warps<P, H, 2>() * 32)
     mpe_policy_mlp_categorical_kernel(const __grid_constant__ MlpCategoricalArgs ca) {
     mlp_rollout<P, H, false, true>(ca.p, nullptr, &ca.c);
 }
 
 template <class P, int H>
-__global__ void __launch_bounds__(mlp_block_warps<P, H, true, true>() * 32)
+__global__ void __launch_bounds__(mlp_block_warps<P, H, 3>() * 32)
     mpe_policy_mlp_categorical_episode_kernel(const __grid_constant__ MlpCategoricalEpisodeArgs ca) {
     mlp_rollout<P, H, true, true>(ca.e.p, &ca.e, &ca.c);
 }
 
 template <class P>
-__global__ void __launch_bounds__(mappo_block_warps<P, false>() * 32)
+__global__ void __launch_bounds__(mlp_block_warps<P, 64, 4>() * 32)
     mpe_policy_mappo_kernel(const __grid_constant__ MlpMappoArgs ma) {
     mlp_rollout<P, 64, false, true, true>(ma.c.p, nullptr, &ma.c.c, ma.eps, ma.net_flags);
 }
 
 template <class P>
-__global__ void __launch_bounds__(mappo_block_warps<P, true>() * 32)
+__global__ void __launch_bounds__(mlp_block_warps<P, 64, 5>() * 32)
     mpe_policy_mappo_episode_kernel(const __grid_constant__ MlpMappoEpisodeArgs ma) {
     mlp_rollout<P, 64, true, true, true>(ma.c.e.p, &ma.c.e, &ma.c.c, ma.eps, ma.net_flags);
 }
@@ -1704,10 +1691,9 @@ struct Program {
     KernelFn hot_dense_fn;   // the same compiled for 80 registers (large batches of programs that fit without spilling)
     void (*policy_fn[2])(PolicyArgs);  // K-step closed-loop rollout, hidden width 32 / 64 (null: not built for this program)
     int policy_weight_floats[2];
-    // the same with the two-hidden-layer actor on the tensor cores, by form (episodes | categorical << 1) and H = 32 / 64:
-    // the kernel and its warps per block at most (mlp_block_warps)
+    // the same with the two-hidden-layer actor on the tensor cores, by form (episodes | kind << 1) and H = 32 / 64: the
+    // kernel and its warps per block at most (mlp_block_warps); null for MAPPO's forms at H = 32
     struct { const void *fn; int warps; } mlp[kMlpForms][2];
-    struct { const void *fn; int warps; } mappo[2];   // MAPPO's actor (H = 64, categorical), one episode / episodes
     int mlp_weight_floats[2], mlp_warp_floats[2];
     int mlp_explore_stride;           // Philox blocks per (step, agent) of its exploration noise
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
@@ -1719,11 +1705,14 @@ struct Program {
 
 template <class P, int H>
 static void set_mlp(Program &p, int k) {
-    p.mlp[0][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_rollout_kernel<P, H>), mlp_block_warps<P, H>()};
-    p.mlp[1][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_episode_kernel<P, H>), mlp_block_warps<P, H, true>()};
-    p.mlp[2][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_categorical_kernel<P, H>), mlp_block_warps<P, H, false, true>()};
-    p.mlp[3][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_categorical_episode_kernel<P, H>),
-                   mlp_block_warps<P, H, true, true>()};
+    p.mlp[0][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_rollout_kernel<P, H>), mlp_block_warps<P, H, 0>()};
+    p.mlp[1][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_episode_kernel<P, H>), mlp_block_warps<P, H, 1>()};
+    p.mlp[2][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_categorical_kernel<P, H>), mlp_block_warps<P, H, 2>()};
+    p.mlp[3][k] = {reinterpret_cast<const void *>(mpe_policy_mlp_categorical_episode_kernel<P, H>), mlp_block_warps<P, H, 3>()};
+    if constexpr (H == 64) {
+        p.mlp[4][k] = {reinterpret_cast<const void *>(mpe_policy_mappo_kernel<P>), mlp_block_warps<P, H, 4>()};
+        p.mlp[5][k] = {reinterpret_cast<const void *>(mpe_policy_mappo_episode_kernel<P>), mlp_block_warps<P, H, 5>()};
+    }
     p.mlp_weight_floats[k] = MlpShape<P, H>::kWeightFloats;
     p.mlp_warp_floats[k] = MlpShape<P, H>::kWarpFloats;
 }
@@ -1751,8 +1740,6 @@ static Program make_program() {
     if constexpr (MlpBuilt<P>::value) {
         set_mlp<P, 32>(p, 0);
         set_mlp<P, 64>(p, 1);
-        p.mappo[0] = {reinterpret_cast<const void *>(mpe_policy_mappo_kernel<P>), mappo_block_warps<P, false>()};
-        p.mappo[1] = {reinterpret_cast<const void *>(mpe_policy_mappo_episode_kernel<P>), mappo_block_warps<P, true>()};
         p.mlp_explore_stride = mlp_explore_stride<P>();
     }
     p.smem_bytes = Shape<P>::kWarpBytes;  // per warp
@@ -1890,10 +1877,6 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
                 if (prog->mlp[f][k].fn)
                     CUDA_TRY(cudaFuncSetAttribute(prog->mlp[f][k].fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                   (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp[f][k].warps) * 4));
-        for (int e = 0; e < 2; ++e)
-            if (prog->mappo[e].fn)
-                CUDA_TRY(cudaFuncSetAttribute(prog->mappo[e].fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (prog->mlp_weight_floats[1] + prog->mlp_warp_floats[1] * prog->mappo[e].warps) * 4));
         if (prog->rollout_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->rollout_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->rollout_smem * max_warps_per_block(prog->rollout_smem)));
@@ -2247,12 +2230,11 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
                              "cudaLaunchKernelExC(rollout_policy)");
 }
 
-// The arguments of the four two-hidden-layer rollout entry points, filled by name (several neighbours share a type).
-// form: episodes | categorical << 1.  T is the episode length (n_steps in the single-episode forms); a record the form
-// does not have is null.  mappo: MAPPO's actor (categorical forms, H = 64) with net_flags and ln_eps (MlpMappoArgs).
+// The arguments of the six two-hidden-layer rollout entry points, filled by name (several neighbours share a type).
+// form: episodes | kind << 1 (kMlpForms).  T is the episode length (n_steps in the single-episode forms); a record the
+// form does not have is null.  net_flags and ln_eps are MAPPO's (MlpMappoArgs).
 struct MlpCall {
     int form;
-    bool mappo;
     uint32_t net_flags;
     float ln_eps;
     void *pv;
@@ -2277,11 +2259,10 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
         {"mpe_rollout_policy_mlp", "cudaLaunchKernelExC(rollout_policy_mlp)"},
         {"mpe_rollout_policy_mlp_episodes", "cudaLaunchKernelExC(rollout_policy_mlp_episodes)"},
         {"mpe_rollout_policy_mlp_categorical", "cudaLaunchKernelExC(rollout_policy_mlp_categorical)"},
-        {"mpe_rollout_policy_mlp_categorical_episodes", "cudaLaunchKernelExC(rollout_policy_mlp_categorical_episodes)"}};
-    static const char *const kMappoName[2][2] = {
+        {"mpe_rollout_policy_mlp_categorical_episodes", "cudaLaunchKernelExC(rollout_policy_mlp_categorical_episodes)"},
         {"mpe_rollout_policy_mappo", "cudaLaunchKernelExC(rollout_policy_mappo)"},
         {"mpe_rollout_policy_mappo_episodes", "cudaLaunchKernelExC(rollout_policy_mappo_episodes)"}};
-    const bool episodes = c.form & 1, categorical = c.form & 2;
+    const bool episodes = c.form & 1, categorical = c.form >= 2, mappo = c.form >= 4;
     const bool no_weights = !c.w[0] || !c.w[1] || !c.w[2] || !c.w[3] || !c.w[4] || !c.w[5];
     // the single-episode forms refuse a negative n_steps and null weight arrays before anything else, the episode forms
     // after the device, program and length checks
@@ -2289,10 +2270,9 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     if (h->device < 0) return MPE_ERR_NO_DEVICE;
     const int k = c.hidden == 32 ? 0 : (c.hidden == 64 ? 1 : -1);
     if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || h->prog->mlp[c.form][k].fn == nullptr) return MPE_ERR_UNSUPPORTED;
-    if (c.mappo && (k != 1 || h->prog->mappo[episodes].fn == nullptr)) return MPE_ERR_UNSUPPORTED;   // H = 64 only
     if (c.flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
     // unknown network flags, or an eps that is negative, NaN or infinite
-    if (c.mappo && ((c.net_flags & ~(kMappoFeatureNorm | kMappoTanh)) || !(c.ln_eps >= 0.0f && c.ln_eps <= 3.4e38f)))
+    if (mappo && ((c.net_flags & ~(kMappoFeatureNorm | kMappoTanh)) || !(c.ln_eps >= 0.0f && c.ln_eps <= 3.4e38f)))
         return MPE_ERR_BAD_ARG;
     // records are indexed by the global step e * episode_length + t, an int
     if (episodes && (c.T < 1 || c.episodes < 1 || static_cast<int64_t>(c.T) * c.episodes > 0x7fffffffLL))
@@ -2301,7 +2281,7 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     if (c.explore && static_cast<int64_t>(c.T) * h->prog->A * h->prog->mlp_explore_stride > static_cast<int64_t>(kExploreTag))
         return MPE_ERR_BAD_ARG;
     if (no_weights || (c.rew_steps != nullptr && !ok4(c.rew_steps))) return MPE_ERR_BAD_ARG;
-    NvtxRange range(c.mappo ? kMappoName[episodes][0] : kName[c.form][0]);
+    NvtxRange range(kName[c.form][0]);
     MlpCategoricalRecords cr{};
     if (categorical) {
         if (c.logp_steps != nullptr && !ok4(c.logp_steps)) return MPE_ERR_BAD_ARG;
@@ -2341,18 +2321,17 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     MlpCategoricalEpisodeArgs cea{ea, cr};
     MlpMappoArgs ma{ca, c.ln_eps, c.net_flags};
     MlpMappoEpisodeArgs mea{cea, c.ln_eps, c.net_flags};
-    void *const form_args[kMlpForms] = {&pa, &ea, &ca, &cea};
-    void *const args = c.mappo ? (episodes ? static_cast<void *>(&mea) : static_cast<void *>(&ma)) : form_args[c.form];
-    const void *const fn = c.mappo ? h->prog->mappo[episodes].fn : h->prog->mlp[c.form][k].fn;
-    const int cap = c.mappo ? h->prog->mappo[episodes].warps : h->prog->mlp[c.form][k].warps;
+    void *const form_args[kMlpForms] = {&pa, &ea, &ca, &cea, &ma, &mea};
+    const void *const fn = h->prog->mlp[c.form][k].fn;
+    const int cap = h->prog->mlp[c.form][k].warps;
     // every block stages all agents' weights once, so blocks are as large as possible while every SM still gets work
     const int64_t warps = (h->n + 31) / 32;
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
     if (wpb > cap) wpb = cap;
     return launch_persistent(h, fn, warps, wpb, static_cast<size_t>(h->prog->mlp_weight_floats[k]) * 4,
-                             static_cast<size_t>(h->prog->mlp_warp_floats[k]) * 4, args, c.stream,
-                             c.mappo ? kMappoName[episodes][1] : kName[c.form][1]);
+                             static_cast<size_t>(h->prog->mlp_warp_floats[k]) * 4, form_args[c.form], c.stream,
+                             kName[c.form][1]);
 }
 
 extern "C" int mpe_rollout_policy_mlp(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
@@ -2444,9 +2423,9 @@ extern "C" int mpe_rollout_policy_mappo(mpe_handle h, void *pv, const void *lm, 
     c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
     c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
     c.done = done; c.flags = flags; c.stream = stream;
-    c.form = 2; c.T = n_steps; c.episodes = 1; c.rew = rew_sum;
+    c.form = 4; c.T = n_steps; c.episodes = 1; c.rew = rew_sum;
     c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
-    c.mappo = true; c.net_flags = net_flags; c.ln_eps = ln_eps;
+    c.net_flags = net_flags; c.ln_eps = ln_eps;
     return rollout_policy_mlp(h, c);
 }
 
@@ -2463,10 +2442,10 @@ extern "C" int mpe_rollout_policy_mappo_episodes(
     c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
     c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
     c.done = done; c.flags = flags; c.stream = stream;
-    c.form = 3; c.T = episode_length; c.episodes = n_episodes; c.rew = ep_rew;
+    c.form = 5; c.T = episode_length; c.episodes = n_episodes; c.rew = ep_rew;
     c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
     c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
-    c.mappo = true; c.net_flags = net_flags; c.ln_eps = ln_eps;
+    c.net_flags = net_flags; c.ln_eps = ln_eps;
     return rollout_policy_mlp(h, c);
 }
 

@@ -110,7 +110,7 @@ def random_actions(act_dims, n, rng, temperature=2.0, movable=None):
 #            where kLowRegVariant holds: tag with 3 to 6 agents and spread N=4 (csrc/mpe_scenarios.cuh ~l.96, ~l.173).
 #   "rollout" mpe_rollout: 1 warp per block up to 4*sms warps, 2 up to 64*sms, else 4
 #   "policy"  mpe_rollout_policy: 1 up to 16*sms warps, 2 up to 64*sms, else 4
-#   "mlp"     rollout_policy_mlp, all four forms: ceil(warps / sms) warps per block, capped at mlp_block_warps
+#   "mlp"     rollout_policy_mlp, all six forms: ceil(warps / sms) warps per block, capped at mlp_block_warps
 #            (mirrored by mlp_programs.mlp_block_cap)
 # The shared-memory caps (max_warps_per_block) never bind for the built-in scenarios at 4 warps per block.
 STEP_DENSE_TAGS = ("simple_tag", "simple_tag_2v1", "simple_tag_4v2")    # the test tags with a hot_dense_fn

@@ -7,8 +7,8 @@ import itertools
 
 import numpy as np
 
-from mlp_categorical_helpers import GUMBEL_GAP, LOGP_ATOL, bounds, categorical_pick, log_softmax_at
-from mlp_helpers import tf32_accumulation_bound, tf32_rna
+from mlp_categorical_helpers import LOGP_ATOL, _row_ok, categorical_pick, log_softmax_at
+from mlp_helpers import flip_candidates, tf32_accumulation_bound, tf32_rna
 
 H = 64
 FEATURE_NORM, TANH = 1, 2          # net_flags
@@ -99,27 +99,22 @@ def module_logits(module, obs):
         return m(torch.as_tensor(np.asarray(obs, np.float64))).numpy()
 
 
-def _row_ok(z, noise, k, logp, segments):
-    """do the logits z (one row) explain the pick k and the log-probability logp?  (ok, needed the Gumbel gap)"""
-    zp = z + noise
-    gap_used = False
-    for s, (a, b) in enumerate(bounds(segments)):
-        j = a + int(np.argmax(zp[a:b]))
-        if j != a + int(k[s]):
-            if zp[j] - zp[a + int(k[s])] > GUMBEL_GAP:
-                return False, False
-            gap_used = True
-    if logp is not None and abs(log_softmax_at(z[None], k[None], segments)[0] - logp) > LOGP_ATOL:
-        return False, False
-    return True, gap_used
-
-
 def ambiguous_groups(values, alt):
     """the ambiguous elements of one row (alt not NaN), grouped by equal value: [(index, ...), ...]"""
     groups = {}
     for j in np.where(~np.isnan(alt))[0]:
         groups.setdefault(float(values[j]), []).append(int(j))
     return [tuple(g) for g in groups.values()]
+
+
+def next_layer(model, layer_index):
+    """flip_candidates' layer after a rounded row: (rounded values, alternatives, ambiguous groups) of hidden layer
+    `layer_index`"""
+    def of(prev):
+        v, e = model.hidden(prev[None], layer_index)
+        r, alt = flip_choices(v[0], e[0])
+        return r, alt, ambiguous_groups(v[0], alt)
+    return of
 
 
 def explain_mappo_mismatches(k, logp, obs, model, segments, noise=0.0):
@@ -155,42 +150,10 @@ def explain_mappo_mismatches(k, logp, obs, model, segments, noise=0.0):
             _, alt0 = flip_choices(x0v[w], e0[w])
         else:
             alt0 = np.full(x0v.shape[1], np.nan)
-        amb0 = ambiguous_groups(x0v[w], alt0)
-        cache = {}
-
-        def layer(prev, layer_index):
-            """(rounded values, alternatives, ambiguous groups) of the layer after `prev` (a rounded row)"""
-            key = (layer_index, prev.tobytes())
-            if key not in cache:
-                v, e = model.hidden(prev[None], layer_index)
-                r, alt = flip_choices(v[0], e[0])
-                cache[key] = (r, alt, ambiguous_groups(v[0], alt))
-            return cache[key]
-
-        def flipped(r, alt, f):
-            idx = [j for group in f for j in group]
-            g = r.copy()
-            g[idx] = alt[idx]
-            return g
-
-        def candidates():                            # flip sets in order of their size, earlier layers first
-            for nflips in range(1, len(amb0) + 2 * H + 1):
-                produced = False
-                for k0 in range(min(nflips, len(amb0)) + 1):
-                    for f0 in itertools.combinations(amb0, k0):
-                        g0 = flipped(x0[w], alt0, f0)
-                        r1, alt1, amb1 = layer(g0, 0)
-                        for k1 in range(min(nflips - k0, len(amb1)) + 1):
-                            for f1 in itertools.combinations(amb1, k1):
-                                r2, alt2, amb2 = layer(flipped(r1, alt1, f1), 1)
-                                for f2 in itertools.combinations(amb2, nflips - k0 - k1):
-                                    produced = True
-                                    yield flipped(r2, alt2, f2)
-                if not produced:
-                    return
-
+        first = (x0[w], alt0, ambiguous_groups(x0v[w], alt0))
         tried, ok = 0, False
-        for g in itertools.islice(candidates(), MAPPO_MAX_COMBOS):
+        for g in itertools.islice(flip_candidates(first, [next_layer(model, 0), next_layer(model, 1)]),
+                                  MAPPO_MAX_COMBOS):
             tried += 1
             ok, _ = _row_ok(model.logits(g), noise[w], k[w], lp, segments)
             if ok:
@@ -204,34 +167,6 @@ def explain_mappo_mismatches(k, logp, obs, model, segments, noise=0.0):
                              "Gumbel gap (row, pick, model pick, logp, model logp, combinations tried): %s"
                              % (len(unexplained), bad.size, unexplained[:8]))
     return flips, gaps
-
-
-# ---- block-size cap: mappo_block_warps in csrc/mpe_kernels.cu ----------------------------------------------------------
-# MappoRegisterException: (tag, forms, warps) where the general H = 64 rule would spill, by form: "C" (one episode),
-# "CE" (episodes)
-MAPPO_REGISTER_EXCEPTIONS = [
-    ("simple_spread_n2", ("C", "CE"), 12),
-    ("simple_spread_n3", ("C", "CE"), 12),
-    ("simple_spread_n6", ("C", "CE"), 8),
-    ("simple_tag_1v1", ("C", "CE"), 12),
-    ("simple_tag_2v1", ("C", "CE"), 12),
-    ("simple_speaker_listener", ("C", "CE"), 12),
-    ("simple_adversary", ("C", "CE"), 12),
-    ("simple_crypto", ("C",), 12),
-]
-assert len({tag for tag, _, _ in MAPPO_REGISTER_EXCEPTIONS}) == len(MAPPO_REGISTER_EXCEPTIONS)
-
-
-def mappo_block_cap(tag, episodes):
-    """mappo_block_warps: the exception or the general H = 64 rule, lowered to what fits in shared memory"""
-    from mlp_programs import SMEM_OPTIN_BYTES, mlp_register_rule, mlp_smem_bytes, shapes_of
-    obs_dims, act_dims = shapes_of(tag)
-    form = "CE" if episodes else "C"
-    cap = next((w for t, forms, w in MAPPO_REGISTER_EXCEPTIONS if t == tag and form in forms),
-               mlp_register_rule(H, len(obs_dims), max(act_dims)))
-    while mlp_smem_bytes(H, obs_dims, act_dims, cap) > SMEM_OPTIN_BYTES:
-        cap -= 1
-    return cap
 
 
 def make_mappo_actors(obs_dims, act_dims, tanh, feature_norm, seed=3, eps=1e-5, device="cuda", hidden=H):

@@ -6,7 +6,8 @@ import itertools
 
 import numpy as np
 
-from mlp_helpers import TF32_MAX_COMBOS, tf32_accumulation_bound, tf32_flip_choices, tf32_rna
+from mlp_helpers import (TF32_MAX_COMBOS, flip_candidates, relu_layer, relu_next_layer, tf32_accumulation_bound,
+                         tf32_flip_choices, tf32_rna)
 
 # the fp32 error of the kernel's Gumbel term logf(-logf(u)) next to float64 -log(-log u): a few ulps of values below 17
 GUMBEL_GAP = 1e-5
@@ -65,6 +66,19 @@ def _row_ok(g, noise, k, logp, segments):
     return True, gap_used
 
 
+def split_pick_noise(z_model, z_kernel):
+    """Noise for one row of one sub-space under which the model's logits z_model and the kernel's z_kernel pick
+    different entries: the pair of entries that z_kernel - z_model moves furthest apart, D, is set D / 2 apart, and every
+    other entry far below.  Returns (noise, the kernel's pick, D / 2)."""
+    d = z_kernel - z_model
+    a, b = int(np.argmin(d)), int(np.argmax(d))
+    half = (d[b] - d[a]) / 2
+    noise = np.full(z_model.shape, -50.0)
+    noise[a] = 0.0
+    noise[b] = z_model[a] - z_model[b] - half
+    return noise, b, half
+
+
 def explain_categorical_mismatches(k, logp, obs, params, segments, noise=0.0):
     """Assert that every row whose pick k [n, n_sub] differs from the arg-max of the float64 TF32 model (+ noise), or
     whose log-probability logp [n] (None: not checked) is more than LOGP_ATOL from log_softmax of that model at k, is
@@ -75,7 +89,6 @@ def explain_categorical_mismatches(k, logp, obs, params, segments, noise=0.0):
     Returns (rows explained by a flip, rows explained by the Gumbel gap)."""
     f64 = np.float64
     W1, b1, W2, b2, W3, b3 = [np.asarray(p, dtype=np.float32) for p in params]
-    H = W1.shape[0]
     t1, t2, t3 = (tf32_rna(W).astype(f64) for W in (W1, W2, W3))
     b1, b2, b3 = (np.asarray(b, f64) for b in (b1, b2, b3))
     n = k.shape[0]
@@ -97,33 +110,9 @@ def explain_categorical_mismatches(k, logp, obs, params, segments, noise=0.0):
         if ok:
             gaps += 1
             continue
-        amb1 = list(np.where(~np.isnan(alt1[r]))[0])
-        h2_of = {}
-
-        def layer2(f1):
-            if f1 not in h2_of:
-                h = h1[w].copy()
-                h[list(f1)] = alt1[r, list(f1)]
-                r2, alt2 = tf32_flip_choices(h @ t2.T + b2, tf32_accumulation_bound(h[None], t2, b2)[0])
-                h2_of[f1] = (r2, alt2, list(np.where(~np.isnan(alt2))[0]))
-            return h2_of[f1]
-
-        def candidates():                            # flip sets in order of their size, h1 choices first
-            for nflips in range(1, len(amb1) + H + 1):
-                produced = False
-                for k1 in range(min(nflips, len(amb1)) + 1):
-                    for f1 in itertools.combinations(amb1, k1):
-                        r2, alt2, amb2 = layer2(f1)
-                        for f2 in itertools.combinations(amb2, nflips - k1):
-                            g = r2.copy()
-                            g[list(f2)] = alt2[list(f2)]
-                            produced = True
-                            yield g
-                if not produced:
-                    return
-
         tried = 0
-        for g in itertools.islice(candidates(), TF32_MAX_COMBOS):
+        for g in itertools.islice(flip_candidates(relu_layer(h1[w], alt1[r]), [relu_next_layer(t2, b2)]),
+                                  TF32_MAX_COMBOS):
             tried += 1
             ok, _ = _row_ok(g @ t3.T + b3, noise[w], k[w], lp, segments)
             if ok:

@@ -33,6 +33,15 @@ def tf32_tie(x, every=1):
     return np.where(pick, (b & np.uint32(0xFFFFE000)) | np.uint32(0x1000), b).view(np.float32)
 
 
+def dyadic_actor(rng, od=6, H=32, scale=2.0):
+    """weights and observations on a 2^-4 grid: every sum is exact and every h1 / h2 value a short dyadic number, so no
+    unit lies near a TF32 rounding boundary"""
+    q = lambda *s: (np.round(rng.randn(*s) * scale * 16) / 16).astype(np.float32)        # noqa: E731
+    params = (q(H, od) / 4, q(H) / 4, q(H, H) / 16, q(H) / 4, q(5, H) / 4, q(5) / 4)
+    obs = q(32, od)
+    return obs, params
+
+
 def philox4x32_10(ctr, key):
     """Philox4x32-10 (Salmon et al., SC'11): ctr uint32 [..., 4], key (k0, k1) -> uint32 [..., 4]"""
     M0, M1, W0, W1 = 0xD2511F53, 0xCD9E8D57, 0x9E3779B9, 0xBB67AE85
@@ -146,6 +155,57 @@ def tf32_flip_choices(pre, bound):
     return r, alt
 
 
+def flipped(r, alt, flips):
+    """the rounded row r with every unit of the groups in `flips` set to its alternative"""
+    idx = [j for group in flips for j in group]
+    g = r.copy()
+    g[idx] = alt[idx]
+    return g
+
+
+def flip_candidates(first, next_layers):
+    """The last layer's rounded row under every combination of TF32 rounding flips, in order of the number of flips,
+    earlier layers' flips first (the enumeration the explainers share).  `first` is a layer of one row: (rounded row,
+    alternatives, ambiguous groups), a group being a tuple of units that flip together.  Each of `next_layers` maps the
+    previous layer's rounded row, flips applied, to the next layer of that row, so that its values and ambiguity follow
+    the flips before it.  Stops at the first number of flips that no combination reaches, since none larger does."""
+    cache = {}
+
+    def layer(depth, prev):
+        key = (depth, prev.tobytes())
+        if key not in cache:
+            cache[key] = next_layers[depth](prev)
+        return cache[key]
+
+    def rows(depth, lay, nflips):                    # every row of the last layer reached with exactly nflips flips
+        r, alt, groups = lay
+        if depth == len(next_layers):
+            for f in itertools.combinations(groups, nflips):
+                yield flipped(r, alt, f)
+            return
+        for k in range(min(nflips, len(groups)) + 1):
+            for f in itertools.combinations(groups, k):
+                yield from rows(depth + 1, layer(depth, flipped(r, alt, f)), nflips - k)
+
+    for nflips in itertools.count(1):
+        produced = False
+        for g in rows(0, first, nflips):
+            produced = True
+            yield g
+        if not produced:
+            return
+
+
+def relu_layer(r, alt):
+    """a ReLU layer of one row for flip_candidates: every ambiguous unit flips by itself"""
+    return r, alt, [(int(j),) for j in np.where(~np.isnan(alt))[0]]
+
+
+def relu_next_layer(t, b):
+    """flip_candidates' layer after a rounded ReLU row h: relu(h . t^T + b) and its ambiguity, one row at a time"""
+    return lambda h: relu_layer(*tf32_flip_choices(h @ t.T + b, tf32_accumulation_bound(h[None], t, b)[0]))
+
+
 def explain_tf32_mismatches(actions, obs, params, noise=0.0, atol=1e-5, segments=None):
     """Assert that every row of the kernel's `actions` [n, act_dim] that differs from segment_softmax(actor_logits(obs,
     *params, tf32=True) + noise, segments) by more than atol is a TF32 rounding flip (see above): it has an ambiguous h1
@@ -154,7 +214,6 @@ def explain_tf32_mismatches(actions, obs, params, noise=0.0, atol=1e-5, segments
     TF32_MAX_COMBOS combinations per row; a row that needs more fails.  Returns the number of explained rows."""
     f64 = np.float64
     W1, b1, W2, b2, W3, b3 = [np.asarray(p, dtype=np.float32) for p in params]
-    H = W1.shape[0]
     t1, t2, t3 = (tf32_rna(W).astype(f64) for W in (W1, W2, W3))
     b1, b2, b3 = (np.asarray(b, f64) for b in (b1, b2, b3))
     got = np.asarray(actions, f64)
@@ -170,41 +229,15 @@ def explain_tf32_mismatches(actions, obs, params, noise=0.0, atol=1e-5, segments
     _, alt1 = tf32_flip_choices(p1[bad], tf32_accumulation_bound(x0[bad], t1, b1))
     unexplained = []
     for r, w in enumerate(bad):
-        amb1 = list(np.where(~np.isnan(alt1[r]))[0])
-        h2_of = {}                                   # h1 flip set -> (h2 as the model rounds it, alternatives, ambiguous)
-
-        def layer2(f1):
-            if f1 not in h2_of:
-                h = h1[w].copy()
-                h[list(f1)] = alt1[r, list(f1)]
-                r2, alt2 = tf32_flip_choices(h @ t2.T + b2, tf32_accumulation_bound(h[None], t2, b2)[0])
-                h2_of[f1] = (r2, alt2, list(np.where(~np.isnan(alt2))[0]))
-            return h2_of[f1]
-
-        def candidates():                            # flip sets in order of their size, h1 choices first
-            for nflips in range(1, len(amb1) + H + 1):
-                produced = False
-                for k1 in range(min(nflips, len(amb1)) + 1):
-                    for f1 in itertools.combinations(amb1, k1):
-                        r2, alt2, amb2 = layer2(f1)
-                        for f2 in itertools.combinations(amb2, nflips - k1):
-                            g = r2.copy()
-                            g[list(f2)] = alt2[list(f2)]
-                            produced = True
-                            yield g
-                if not produced:                     # no flip set of this size, hence none larger
-                    return
-
-        any_ambiguous = bool(amb1) or bool(layer2(())[2])
         tried, ok = 0, False
-        if any_ambiguous:
-            for g in itertools.islice(candidates(), TF32_MAX_COMBOS):
-                tried += 1
-                if (np.abs(segment_softmax(g @ t3.T + b3 + noise[w], segments) - got[w]) <= atol).all():
-                    ok = True
-                    break
-        if not ok:
-            unexplained.append((int(w), any_ambiguous, tried, float(np.abs(got[w] - want[w]).max())))
+        for g in itertools.islice(flip_candidates(relu_layer(h1[w], alt1[r]), [relu_next_layer(t2, b2)]),
+                                  TF32_MAX_COMBOS):
+            tried += 1
+            if (np.abs(segment_softmax(g @ t3.T + b3 + noise[w], segments) - got[w]) <= atol).all():
+                ok = True
+                break
+        if not ok:                                   # a row with an ambiguous unit has at least one candidate
+            unexplained.append((int(w), tried > 0, tried, float(np.abs(got[w] - want[w]).max())))
     assert not unexplained, ("%d of %d rows beyond %g are not TF32 rounding flips (row, has an ambiguous unit, "
                              "combinations tried, max |difference|): %s" % (len(unexplained), bad.size, atol,
                                                                             unexplained[:8]))

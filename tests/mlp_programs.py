@@ -46,9 +46,9 @@ def shapes_of(tag):
 # The dynamic shared memory one block may opt in to on H100 (cudaDevAttrMaxSharedMemoryPerBlockOptin)
 SMEM_OPTIN_BYTES = 232448
 
-# The forms, in the kernel's order (episodes | categorical << 1): softmax, softmax episodes, categorical, categorical
-# episodes
-FORMS = ("S", "E", "C", "CE")
+# The forms, in the kernel's order (episodes | kind << 1, kind 0 softmax, 1 categorical, 2 MAPPO's actor): softmax,
+# softmax episodes, categorical, categorical episodes, MAPPO, MAPPO episodes.  MAPPO's forms exist at H = 64 only.
+FORMS = ("S", "E", "C", "CE", "M", "ME")
 # MlpRegisterException: (tag, H, forms, warps) where the general rule would spill (12 warps leave 168 registers per
 # thread, 8 leave 255)
 REGISTER_EXCEPTIONS = [
@@ -59,13 +59,13 @@ REGISTER_EXCEPTIONS = [
     ("simple_spread_n6", 32, FORMS, 12),
     ("simple_tag_4v2", 32, FORMS, 12),
     ("simple_tag_6v2", 32, FORMS, 8),
-    ("simple_speaker_listener", 64, ("E", "CE"), 12),
-    ("simple_adversary", 64, ("E", "CE"), 12),
+    ("simple_speaker_listener", 64, ("E", "CE", "M", "ME"), 12),
+    ("simple_adversary", 64, ("E", "CE", "M", "ME"), 12),
     ("simple_reference", 64, ("E", "CE"), 8),
     ("simple_tag_4v2", 64, ("E", "CE"), 8),
-    ("simple_spread_n3", 64, ("E", "C", "CE"), 12),
+    ("simple_spread_n3", 64, ("E", "C", "CE", "M", "ME"), 12),
     ("simple_push", 64, ("C", "CE"), 12),
-    ("simple_crypto", 64, ("CE",), 12),
+    ("simple_crypto", 64, ("CE", "M"), 12),
     ("simple_spread_n4", 64, ("CE",), 8),
 ]
 # one exception per (program, H), as in the kernel, so that no kernel matches two
@@ -78,9 +78,10 @@ def mlp_register_rule(H, n_agents, max_act_dim=5):
     return 12 if (H == 64 and (n_agents >= 4 or max_act_dim > 8)) else 16
 
 
-def mlp_register_warps(tag, H, episodes=False, categorical=False):
+def mlp_register_warps(tag, H, episodes=False, categorical=False, mappo=False):
     """mlp_register_warps: the general rule, or the exception for this program, H and form"""
-    form = FORMS[int(episodes) | int(categorical) << 1]
+    assert not mappo or (categorical and H == 64), "MAPPO's actor: categorical, H = 64"
+    form = FORMS[int(episodes) | (2 if mappo else int(categorical)) << 1]
     for t, h, forms, warps in REGISTER_EXCEPTIONS:
         if (t, h) == (tag, H) and form in forms:
             return warps
@@ -105,11 +106,11 @@ def mlp_smem_bytes(H, obs_dims, act_dims, warps):
     return 4 * (weights + warps * warp)
 
 
-def mlp_block_cap(tag, H, episodes=False, categorical=False):
+def mlp_block_cap(tag, H, episodes=False, categorical=False, mappo=False):
     """mlp_block_warps: the register cap lowered to the most warps whose tiles fit in shared memory next to the
     weights"""
     obs_dims, act_dims = shapes_of(tag)
-    cap = mlp_register_warps(tag, H, episodes, categorical)
+    cap = mlp_register_warps(tag, H, episodes, categorical, mappo)
     while mlp_smem_bytes(H, obs_dims, act_dims, cap) > SMEM_OPTIN_BYTES:
         cap -= 1
     return cap

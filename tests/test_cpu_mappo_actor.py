@@ -1,20 +1,21 @@
 """CPU checks of MAPPO's actor in the in-kernel rollout (env.rollout_policy with LayerNorm policies): mappo_actor_params
 accepts exactly MAPPO's layer list and folds each LayerNorm's affine exactly; the float64 model the GPU tests judge the
-kernel by agrees with an independent torch formulation; the two C entry points are declared, bound and refuse what they
-can refuse without a device as the categorical ones do; and every one of the 34 kernels is compiled for the block size
-the test mirror expects."""
+kernel by agrees with an independent torch formulation; the flip accounting the GPU tests use explains what a TF32
+rounding flip or the Gumbel gap explains and nothing else; and the two C entry points are declared and bound.  Their
+return codes without a device and the launch bounds of their 34 kernels are checked with the other forms' in
+test_cpu_mlp_block_table.py."""
 import ctypes
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 from helpers import make_product_env
-from mappo_helpers import FEATURE_NORM, TANH, MappoModel, make_mappo_actors, mappo_block_cap, module_logits
-from mlp_programs import PROGRAMS
+from mappo_helpers import (FEATURE_NORM, TANH, MappoModel, explain_mappo_mismatches, make_mappo_actors, module_logits,
+                           next_layer)
+from mlp_categorical_helpers import GUMBEL_GAP, categorical_pick, log_softmax_at, split_pick_noise
+from mlp_helpers import flipped, tf32_rna
 
 torch = pytest.importorskip("torch")
 nn = torch.nn
@@ -143,6 +144,56 @@ def test_model_is_the_torch_float64_recipe(tanh, fn):
         np.testing.assert_allclose(model(obs), want, rtol=0, atol=1e-12)
 
 
+# ---- explain_mappo_mismatches on a synthetic actor (no GPU) -----------------------------------------------------------
+def _model_and_obs():
+    """agent 0's folded actor with the input LayerNorm, and 32 observations"""
+    params, _, _, eps = _params(pols=make_mappo_actors(OBS, ACT, False, True, device="cpu"))
+    model = MappoModel([t.to(torch.float32).numpy() for t in params[0]], (FEATURE_NORM, eps))
+    return model, np.random.RandomState(5).uniform(-2.0, 2.0, (32, 18)).astype(np.float32)
+
+
+def test_accounting_explains_a_pick_moved_by_a_tf32_flip_and_one_within_the_gumbel_gap():
+    model, obs = _model_and_obs()
+    segs = [5]
+    z = model(obs)
+    # the "kernel" rounds one ambiguous group of row 11's x2 the other way: the one that moves a pair of logits furthest
+    # apart.  x1 and x2 are evaluated one row at a time, as the accounting does
+    x0 = tf32_rna(model.input(obs)[0].astype(np.float32)).astype(np.float64)
+    r1, _, _ = next_layer(model, 0)(x0[11])
+    r2, alt2, groups = next_layer(model, 1)(r1)
+    zk = max((model.logits(flipped(r2, alt2, [g])) for g in groups), key=lambda v: np.ptp(v - z[11]))
+    noise = np.zeros_like(z)
+    noise[11], pick11, half = split_pick_noise(z[11], zk)
+    assert half > 1e-4                      # the pick moves, and by more than the Gumbel gap
+    a, b = np.argsort(z[3])[::-1][:2]       # row 3: the runner-up within the Gumbel gap of the pick
+    noise[3, b] = z[3, a] - z[3, b] - GUMBEL_GAP / 2
+    k = categorical_pick(z + noise, segs)
+    logp = log_softmax_at(z, k, segs)
+    assert explain_mappo_mismatches(k, logp, obs, model, segs, noise=noise) == (0, 0)
+    assert k[11, 0] != pick11 and k[3, 0] == a
+    k[11, 0], k[3, 0] = pick11, b
+    logp = log_softmax_at(z, k, segs)
+    logp[11] = log_softmax_at(zk[None], k[11:12], segs)[0]
+    assert explain_mappo_mismatches(k, logp, obs, model, segs, noise=noise) == (1, 1)
+
+
+def test_accounting_rejects_a_wrong_pick_and_a_wrong_log_probability():
+    model, obs = _model_and_obs()
+    segs = [5]
+    z = model(obs)
+    k = categorical_pick(z, segs)
+    logp = log_softmax_at(z, k, segs)
+    assert explain_mappo_mismatches(k, logp, obs, model, segs) == (0, 0)
+    bad = k.copy()
+    bad[7, 0] = np.argmin(z[7])             # with the model's log-probability of that pick
+    with pytest.raises(AssertionError, match="neither TF32 rounding flips of the normalised operands nor within"):
+        explain_mappo_mismatches(bad, log_softmax_at(z, bad, segs), obs, model, segs)
+    wrong = logp.copy()
+    wrong[7] += 1e-2
+    with pytest.raises(AssertionError, match=r"\(7, "):
+        explain_mappo_mismatches(k, wrong, obs, model, segs)
+
+
 def test_refusals_without_a_device():
     """the softmax mode and a hidden width other than 64 are refused before the env is bound"""
     env = make_product_env("simple_spread_n3", num_envs=64)
@@ -175,82 +226,3 @@ def test_entry_points_are_declared_exported_and_bound():
         got, want = _lib._SIGNATURES[name][1], list(_lib._SIGNATURES[base][1])
         assert got == want[:-3] + [ctypes.c_uint32, ctypes.c_float] + want[-3:], name
     assert _lib.MPE_ABI_VERSION == 1
-
-
-BAD_ARG, NO_DEVICE = -1, -5
-
-
-def _call(name, handle, steps=4, weights=True, hidden=64):
-    from multiagent_particle_envs_b200 import _lib
-    lib = _lib.load()
-    argtypes = _lib._SIGNATURES[name][1]
-    per_agent = _lib.ptr_array([256] * _lib.MPE_MAX_AGENTS)
-    args = [256 if t is _lib._P else per_agent if t is _lib._PP else 1 if t.__name__ == "c_int" else 0 for t in argtypes]
-    args[0], args[-1] = handle, None
-    args[5:11] = [per_agent if weights else None] * 6
-    args[11], args[12] = hidden, steps
-    return getattr(lib, name)(*args)
-
-
-def test_return_codes_without_a_device_are_the_categorical_ones():
-    shapes = make_product_env("simple_spread_n3", num_envs=64).world.native_shapes()   # device-less handle
-    handle = shapes.handle          # `shapes` owns it: the handle stays live while the test holds `shapes`
-    for name, base in ENTRY_POINTS.items():
-        episodes = name.endswith("_episodes")
-        for hidden in (64, 32):
-            probes = [dict(handle=None), dict(handle=handle, steps=-1), dict(handle=handle, weights=False),
-                      dict(handle=handle)]
-            want = [BAD_ARG, NO_DEVICE if episodes else BAD_ARG, NO_DEVICE if episodes else BAD_ARG, NO_DEVICE]
-            for kw, w in zip(probes, want):
-                assert _call(name, hidden=hidden, **kw) == _call(base, hidden=hidden, **kw) == w, (name, hidden, kw)
-
-
-# ---- launch bounds ----------------------------------------------------------------------------------------------------
-TYPE_TAGS = {
-    "Simple<1, 1>": "simple", "Spread<2>": "simple_spread_n2", "Spread<3>": "simple_spread_n3",
-    "Spread<4>": "simple_spread_n4", "Spread<5>": "simple_spread_n5", "Spread<6>": "simple_spread_n6",
-    "Tag<3, 1, 2>": "simple_tag", "Tag<1, 1, 2>": "simple_tag_1v1", "Tag<2, 1, 2>": "simple_tag_2v1",
-    "Tag<4, 2, 2>": "simple_tag_4v2", "Tag<6, 2, 3>": "simple_tag_6v2", "Adversary<1, 2, 2>": "simple_adversary",
-    "Adversary<1, 3, 3>": "simple_adversary_n4", "Push<1, 1, 2>": "simple_push",
-    "SpeakerListener": "simple_speaker_listener", "Reference": "simple_reference", "Crypto": "simple_crypto",
-}
-
-
-def _max_threads(lib_path):
-    """mangled kernel name -> EIATTR_MAX_THREADS of `cuobjdump -elf` (the toolkit of the nvcc that builds the library)"""
-    nvcc = shutil.which(os.environ.get("NVCC", "nvcc"))
-    tool = None
-    for d in ([os.path.dirname(os.path.realpath(nvcc))] if nvcc else []) + \
-            [os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin")]:
-        if os.access(os.path.join(d, "cuobjdump"), os.X_OK):
-            tool = os.path.join(d, "cuobjdump")
-            break
-    if tool is None:
-        pytest.skip("no CUDA toolkit (cuobjdump) to read the library with")
-    text = subprocess.run([tool, "-elf", lib_path], capture_output=True, text=True, check=True).stdout
-    out, cur, attr = {}, None, False
-    for ln in text.splitlines():
-        if ln.startswith("."):
-            cur = ln[len(".nv.info."):] if ln.startswith(".nv.info.") else None
-            attr = False
-        elif cur and "Attribute:" in ln:
-            attr = ln.split()[-1] == "EIATTR_MAX_THREADS"
-        elif cur and attr and ln.strip().startswith("Value:"):
-            out[cur] = int(ln.split()[1], 16)
-            attr = False
-    return out
-
-
-def test_launch_bounds_are_the_mirrored_caps():
-    from multiagent_particle_envs_b200 import _lib
-    threads = _max_threads(_lib.LIB_PATH)
-    names = list(threads)
-    demangled = subprocess.run(["c++filt"], input="\n".join(names), capture_output=True, text=True,
-                               check=True).stdout.split("\n")
-    seen = {}
-    for mangled, nm in zip(names, demangled):
-        m = re.match(r"void mpe::mpe_policy_mappo(_episode)?_kernel<mpe::(.+?)\s*>\(", nm)
-        if m:
-            seen[(TYPE_TAGS[m.group(2)], m.group(1) is not None)] = threads[mangled]
-    assert len(seen) == 34 and {k[0] for k in seen} == set(PROGRAMS)
-    assert seen == {(tag, e): 32 * mappo_block_cap(tag, e) for tag, e in seen}

@@ -5,7 +5,7 @@ import pytest
 
 from helpers import make_product_env
 import mlp_helpers
-from mlp_helpers import philox4x32_10, softmax, tf32_rna, tf32_rne, tf32_tie, uniform_from_bits
+from mlp_helpers import dyadic_actor, philox4x32_10, softmax, tf32_rna, tf32_rne, tf32_tie, uniform_from_bits
 
 torch = pytest.importorskip("torch")
 
@@ -120,18 +120,9 @@ def _actions(obs, params, rnd=tf32_rna, h1_override=None):
     return softmax(h2 @ rnd(W3).astype(f64).T + b3)
 
 
-def _dyadic_actor(rng, od=6, H=32, scale=2.0):
-    """weights and observations on a 2^-4 grid: every sum is exact and every h1 / h2 value a short dyadic number, so no
-    unit lies near a TF32 rounding boundary"""
-    q = lambda *s: (np.round(rng.randn(*s) * scale * 16) / 16).astype(np.float32)        # noqa: E731
-    params = (q(H, od) / 4, q(H) / 4, q(H, H) / 16, q(H) / 4, q(5, H) / 4, q(5) / 4)
-    obs = q(32, od)
-    return obs, params
-
-
 def test_accounting_accepts_a_unit_on_a_tf32_midpoint_rounded_the_other_way():
     rng = np.random.RandomState(1)
-    obs, (W1, b1, W2, b2, W3, b3) = _dyadic_actor(rng)
+    obs, (W1, b1, W2, b2, W3, b3) = dyadic_actor(rng)
     # unit 0 of row 5: pre-activation 1 + 2^-11 exactly (a TF32 tie); the model rounds it up to 1 + 2^-10, the "kernel"
     # lands a hair below the tie and rounds it down to 1
     W1 = W1.copy()
@@ -149,7 +140,7 @@ def test_accounting_accepts_a_unit_on_a_tf32_midpoint_rounded_the_other_way():
 
 
 def test_accounting_rejects_a_perturbation_without_an_ambiguous_unit():
-    obs, params = _dyadic_actor(np.random.RandomState(2))
+    obs, params = dyadic_actor(np.random.RandomState(2))
     got = _actions(obs, params)
     assert mlp_helpers.explain_tf32_mismatches(got, obs, params) == 0
     bad = got.copy()
@@ -193,7 +184,7 @@ def test_accounting_rejects_a_perturbation_in_the_last_row_of_a_tile():
 def test_accounting_rejects_round_to_nearest_even():
     """weights and observations that are exact TF32 ties: an actor that rounds them to nearest-even is not the kernel"""
     rng = np.random.RandomState(4)
-    obs, (W1, b1, W2, b2, W3, b3) = _dyadic_actor(rng)
+    obs, (W1, b1, W2, b2, W3, b3) = dyadic_actor(rng)
     params = (tf32_tie(W1 + 0.3), b1, tf32_tie(W2 + 0.1), b2, tf32_tie(W3), b3)
     obs = tf32_tie(obs + 0.7)
     assert (tf32_rna(params[0]) != tf32_rne(params[0])).mean() > 0.3

@@ -1,7 +1,7 @@
-"""CPU checks that tie the two-hidden-layer actor's host side to the built library: every one of its 136 kernels (17
-programs x H = 32, 64 x four forms) is compiled for the block size the test mirror (mlp_programs.mlp_block_cap)
-expects, read from the kernel's launch bounds in libmpe_b200.so; and the four entry points refuse what they can refuse
-without a device with the return codes they always had."""
+"""CPU checks that tie the two-hidden-layer actor's host side to the built library: every one of its 170 kernels (17
+programs x H = 32, 64 x the four MADDPG forms, and 17 programs x MAPPO's two forms at H = 64) is compiled for the block
+size the test mirror (mlp_programs.mlp_block_cap) expects, read from the kernel's launch bounds in libmpe_b200.so; and
+the six entry points refuse what they can refuse without a device with the return codes they always had."""
 import os
 import re
 import shutil
@@ -23,9 +23,10 @@ TYPE_TAGS = {
     "Adversary<1, 3, 3>": "simple_adversary_n4", "Push<1, 1, 2>": "simple_push",
     "SpeakerListener": "simple_speaker_listener", "Reference": "simple_reference", "Crypto": "simple_crypto",
 }
-# kernel name -> (episodes, categorical)
-FORMS = {"rollout": (False, False), "episode": (True, False), "categorical": (False, True),
-         "categorical_episode": (True, True)}
+# kernel name -> (episodes, categorical, mappo)
+FORMS = {"mlp_rollout": (False, False, False), "mlp_episode": (True, False, False),
+         "mlp_categorical": (False, True, False), "mlp_categorical_episode": (True, True, False),
+         "mappo": (False, True, True), "mappo_episode": (True, True, True)}
 
 
 def cuobjdump():
@@ -62,25 +63,32 @@ def test_launch_bounds_are_the_mirrored_caps():
                                check=True).stdout.split("\n")
     seen = {}
     for mangled, nm in zip(names, demangled):
-        m = re.match(r"void mpe::mpe_policy_mlp_(rollout|episode|categorical|categorical_episode)_kernel<mpe::(.+), "
-                     r"(\d+)>\(", nm)
+        m = re.match(r"void mpe::mpe_policy_(mlp_rollout|mlp_episode|mlp_categorical|mlp_categorical_episode)_kernel"
+                     r"<mpe::(.+), (\d+)>\(", nm)
         if m:
-            key = (TYPE_TAGS[m.group(2)], int(m.group(3))) + FORMS[m.group(1)]
-            seen[key] = threads[mangled]
-    assert len(seen) == 136 and {k[0] for k in seen} == set(PROGRAMS)
-    want = {(tag, H, e, c): 32 * mlp_block_cap(tag, H, e, c) for tag, H, e, c in seen}
+            seen[(TYPE_TAGS[m.group(2)], int(m.group(3))) + FORMS[m.group(1)]] = threads[mangled]
+        m = re.match(r"void mpe::mpe_policy_(mappo|mappo_episode)_kernel<mpe::(.+?)\s*>\(", nm)
+        if m:                                        # MAPPO's actor: H = 64 only
+            seen[(TYPE_TAGS[m.group(2)], 64) + FORMS[m.group(1)]] = threads[mangled]
+    assert len(seen) == 170 and {k[0] for k in seen} == set(PROGRAMS)
+    assert sum(k[4] for k in seen) == 34
+    want = {(tag, H, e, c, mp): 32 * mlp_block_cap(tag, H, e, c, mp) for tag, H, e, c, mp in seen}
     assert seen == want
 
 
 # ---- return codes without a device ---------------------------------------------------------------------------------
 ENTRY_POINTS = ("mpe_rollout_policy_mlp", "mpe_rollout_policy_mlp_categorical", "mpe_rollout_policy_mlp_episodes",
-                "mpe_rollout_policy_mlp_categorical_episodes")
+                "mpe_rollout_policy_mlp_categorical_episodes", "mpe_rollout_policy_mappo",
+                "mpe_rollout_policy_mappo_episodes")
+# MAPPO's entry points -> the categorical form whose return codes they give
+MAPPO_BASE = {"mpe_rollout_policy_mappo": "mpe_rollout_policy_mlp_categorical",
+              "mpe_rollout_policy_mappo_episodes": "mpe_rollout_policy_mlp_categorical_episodes"}
 BAD_ARG, NO_DEVICE = -1, -5
 
 
-def _call(name, handle, steps=4, weights=True):
-    """`name` with aligned dummy pointers (every probe returns before one is used), H = 32, `steps` steps (the episode
-    length in the episode forms, of one episode) and null weight arrays unless `weights`"""
+def _call(name, handle, steps=4, weights=True, hidden=32):
+    """`name` with aligned dummy pointers (every probe returns before one is used), hidden width `hidden`, `steps` steps
+    (the episode length in the episode forms, of one episode) and null weight arrays unless `weights`"""
     from multiagent_particle_envs_b200 import _lib
     lib = _lib.load()
     argtypes = _lib._SIGNATURES[name][1]
@@ -88,18 +96,23 @@ def _call(name, handle, steps=4, weights=True):
     args = [256 if t is _lib._P else per_agent if t is _lib._PP else 1 if t.__name__ == "c_int" else 0 for t in argtypes]
     args[0], args[-1] = handle, None
     args[5:11] = [per_agent if weights else None] * 6
-    args[11], args[12] = 32, steps
+    args[11], args[12] = hidden, steps
     return getattr(lib, name)(*args)
 
 
 def test_entry_point_return_codes_without_a_device():
     """the single-episode forms refuse a negative n_steps and null weight arrays before they ask for the device; the
-    episode forms ask for the device first"""
+    episode forms ask for the device first; MAPPO's entry points, at either width, answer as the categorical ones"""
     shapes = make_product_env("simple_spread_n3", num_envs=64).world.native_shapes()   # device-less handle
     handle = shapes.handle          # `shapes` owns it: the handle stays live while the test holds `shapes`
     for name in ENTRY_POINTS:
         episodes = name.endswith("_episodes")
-        assert _call(name, None) == BAD_ARG, name
-        assert _call(name, handle, steps=-1) == (NO_DEVICE if episodes else BAD_ARG), name
-        assert _call(name, handle, weights=False) == (NO_DEVICE if episodes else BAD_ARG), name
-        assert _call(name, handle) == NO_DEVICE, name
+        for hidden in (32, 64):
+            probes = [dict(handle=None), dict(handle=handle, steps=-1), dict(handle=handle, weights=False),
+                      dict(handle=handle)]
+            want = [BAD_ARG, NO_DEVICE if episodes else BAD_ARG, NO_DEVICE if episodes else BAD_ARG, NO_DEVICE]
+            for kw, w in zip(probes, want):
+                got = _call(name, hidden=hidden, **kw)
+                assert got == w, (name, hidden, kw)
+                if name in MAPPO_BASE:
+                    assert got == _call(MAPPO_BASE[name], hidden=hidden, **kw), (name, hidden, kw)

@@ -1,6 +1,7 @@
 """CPU checks of the categorical form of the two-hidden-layer actor (env.rollout_policy(..., action_mode="categorical")):
 the new C entry points are declared and bound, the NumPy models the GPU tests judge the kernel by (log-probability,
-Gumbel arg-max, one-hot replay) agree with independent formulations, and the refusals that need no device."""
+Gumbel arg-max, one-hot replay) agree with independent formulations, the flip accounting explains what a TF32 rounding
+flip or the Gumbel gap explains and nothing else, and the refusals that need no device."""
 import os
 import re
 
@@ -8,8 +9,10 @@ import numpy as np
 import pytest
 
 from helpers import make_product_env
-from mlp_categorical_helpers import bounds, categorical_pick, log_softmax_at, one_hot
-from mlp_helpers import EXPLORE_TAG, gumbel_noise, philox4x32_10, segment_softmax, uniform_from_bits
+from mlp_categorical_helpers import (GUMBEL_GAP, bounds, categorical_pick, explain_categorical_mismatches, log_softmax_at,
+                                     one_hot, split_pick_noise)
+from mlp_helpers import (EXPLORE_TAG, actor_logits, dyadic_actor, gumbel_noise, philox4x32_10, segment_softmax, tf32_rna,
+                         uniform_from_bits)
 
 torch = pytest.importorskip("torch")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -90,6 +93,60 @@ def test_ties_go_to_the_lowest_index_and_one_hot_inverts_the_pick():
     rng = np.random.RandomState(3)
     k = np.stack([rng.randint(0, 5, 100), rng.randint(0, 10, 100)], -1)
     np.testing.assert_array_equal(categorical_pick(one_hot(k, [5, 10]), [5, 10]), k)
+
+
+# ---- explain_categorical_mismatches on synthetic actors (no GPU) -----------------------------------------------------
+def _logits(obs, params, h1_override):
+    """actor_logits with one rounded h1 entry, (row, unit, value), replaced"""
+    f64 = np.float64
+    W1, b1, W2, b2, W3, b3 = params
+    h1 = tf32_rna(np.maximum(tf32_rna(obs).astype(f64) @ tf32_rna(W1).astype(f64).T + b1, 0).astype(np.float32)).astype(f64)
+    h1[h1_override[0], h1_override[1]] = h1_override[2]
+    h2 = tf32_rna(np.maximum(h1 @ tf32_rna(W2).astype(f64).T + b2, 0).astype(np.float32)).astype(f64)
+    return h2 @ tf32_rna(W3).astype(f64).T + b3
+
+
+def test_accounting_explains_a_pick_moved_by_a_tf32_flip_and_one_within_the_gumbel_gap():
+    obs, (W1, b1, W2, b2, W3, b3) = dyadic_actor(np.random.RandomState(1))
+    # unit 0: pre-activation 1 + 2^-11 exactly (a TF32 tie); the model rounds it up to 1 + 2^-10, the "kernel" rounds
+    # row 5's down to 1
+    W1, b1, W2 = W1.copy(), b1.copy(), W2.copy()
+    W1[0] = 0.0
+    b1[0] = np.float32(1 + 2 ** -11)
+    W2[:, 0] = 1.0                          # make the flip visible in the logits
+    params, segs = (W1, b1, W2, b2, W3, b3), [5]
+    z = actor_logits(obs, *params)
+    zk = _logits(obs, params, (5, 0, 1.0))
+    noise = np.zeros_like(z)
+    noise[5], pick5, half = split_pick_noise(z[5], zk[5])
+    assert half > 1e-4                      # the pick moves, and by more than the Gumbel gap
+    a, b = np.argsort(z[3])[::-1][:2]       # row 3: the runner-up within the Gumbel gap of the pick
+    noise[3, b] = z[3, a] - z[3, b] - GUMBEL_GAP / 2
+    k = categorical_pick(z + noise, segs)
+    logp = log_softmax_at(z, k, segs)
+    assert explain_categorical_mismatches(k, logp, obs, params, segs, noise=noise) == (0, 0)
+    assert k[5, 0] != pick5 and k[3, 0] == a
+    k[5, 0], k[3, 0] = pick5, b
+    logp = log_softmax_at(z, k, segs)
+    logp[5] = log_softmax_at(zk[5:6], k[5:6], segs)[0]
+    assert explain_categorical_mismatches(k, logp, obs, params, segs, noise=noise) == (1, 1)
+
+
+def test_accounting_rejects_a_wrong_pick_and_a_wrong_log_probability():
+    obs, params = dyadic_actor(np.random.RandomState(2))
+    segs = [5]
+    z = actor_logits(obs, *params)
+    k = categorical_pick(z, segs)
+    logp = log_softmax_at(z, k, segs)
+    assert explain_categorical_mismatches(k, logp, obs, params, segs) == (0, 0)
+    bad = k.copy()
+    bad[7, 0] = np.argmin(z[7])             # with the model's log-probability of that pick
+    with pytest.raises(AssertionError, match="neither TF32 rounding flips nor within the Gumbel gap"):
+        explain_categorical_mismatches(bad, log_softmax_at(z, bad, segs), obs, params, segs)
+    wrong = logp.copy()
+    wrong[7] += 1e-3
+    with pytest.raises(AssertionError, match=r"\(7, "):
+        explain_categorical_mismatches(k, wrong, obs, params, segs)
 
 
 def test_refusals_without_a_device():

@@ -8,11 +8,10 @@ import numpy as np
 import pytest
 
 from helpers import device_sms, launch_shape, make_product_env, regime_size
-from mappo_helpers import (FEATURE_NORM, TANH, MappoModel, explain_mappo_mismatches, make_mappo_actors,
-                           mappo_block_cap, module_logits)
+from mappo_helpers import FEATURE_NORM, TANH, MappoModel, explain_mappo_mismatches, make_mappo_actors, module_logits
 from mlp_categorical_helpers import bounds, log_softmax_at, one_hot_torch
 from mlp_helpers import gumbel_noise
-from mlp_programs import PROGRAMS, make_program_env, state, twins
+from mlp_programs import PROGRAMS, make_program_env, mlp_block_cap, state, twins
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -28,7 +27,7 @@ def segments_of(env):
 
 
 def size(tag, wpb, base=None, episodes=False):
-    cap = mappo_block_cap(tag, episodes)
+    cap = mlp_block_cap(tag, 64, episodes, categorical=True, mappo=True)
     sms = device_sms()
     n = regime_size("mlp", sms, min(wpb, cap), cap=cap, base=base)
     assert launch_shape("mlp", n, sms, cap)[0] == min(wpb, cap)

@@ -127,33 +127,23 @@ def main():
     print("|---|---|---|---|---|---|---|---|---|---|---|---|---|")
     for r in rows:
         print("| " + " | ".join(str(x) for x in r) + " |")
+    forms = {"mlp_rollout": "S", "mlp_episode": "E", "mlp_categorical": "C", "mlp_categorical_episode": "CE",
+             "mappo": "M", "mappo_episode": "ME"}
     mlp = []
     for mangled, (reg, stack) in usage.items():
-        m = re.match(r"void mpe::mpe_policy_mlp_(rollout|episode|categorical|categorical_episode)_kernel<mpe::(.+), (\d+)>\(",
-                     names[mangled])
+        m = re.match(r"void mpe::mpe_policy_(mlp_rollout|mlp_episode|mlp_categorical|mlp_categorical_episode|mappo|"
+                     r"mappo_episode)_kernel<mpe::(.+?)(?:, (\d+))?\s*>\(", names[mangled])
         if m:
             c = mix.get(mangled, {})
-            mlp.append((m.group(2), m.group(3), m.group(1), reg, stack, c["total"], c["HMMA"], c["LDS"], c["MUFU"]))
+            mlp.append((m.group(2), m.group(3) or "64", forms[m.group(1)], reg, stack, c["total"], c["HMMA"], c["LDS"],
+                        c["MUFU"]))
     if mlp:
-        print("\n## Closed-loop rollout with the two-hidden-layer actor (`mpe_policy_mlp_rollout_kernel`, its episode form "
-              "`mpe_policy_mlp_episode_kernel` and the categorical forms of both, TF32 mma.sync)\n")
+        print("\n## Closed-loop rollout with the two-hidden-layer actor (TF32 mma.sync), by form: S "
+              "`mpe_policy_mlp_rollout_kernel`, E its episode form `mpe_policy_mlp_episode_kernel`, C and CE the "
+              "categorical forms of both, M and ME MAPPO's LayerNorm actor `mpe_policy_mappo[_episode]_kernel` (H = 64)\n")
         print("| program | H | form | regs | stack | instr | HMMA | LDS | MUFU |")
         print("|---|---|---|---|---|---|---|---|---|")
         for r in sorted(mlp):
-            print("| " + " | ".join(str(x) for x in r) + " |")
-    mappo = []
-    for mangled, (reg, stack) in usage.items():
-        m = re.match(r"void mpe::mpe_policy_mappo(_episode)?_kernel<mpe::(.+?)\s*>\(", names[mangled])
-        if m:
-            c = mix.get(mangled, {})
-            mappo.append((m.group(2), "episodes" if m.group(1) else "one episode", reg, stack, c["total"], c["HMMA"],
-                          c["LDS"], c["MUFU"]))
-    if mappo:
-        print("\n## Closed-loop rollout with MAPPO's LayerNorm actor (`mpe_policy_mappo_kernel`, "
-              "`mpe_policy_mappo_episode_kernel`, categorical, H = 64)\n")
-        print("| program | form | regs | stack | instr | HMMA | LDS | MUFU |")
-        print("|---|---|---|---|---|---|---|---|")
-        for r in sorted(mappo):
             print("| " + " | ".join(str(x) for x in r) + " |")
     other = [(names[k], v) for k, v in usage.items() if "mpe_kernel" not in names[k] or ", 0, " not in names[k]]
     spills = [n for n, (r, s) in other if s]
