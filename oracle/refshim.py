@@ -122,9 +122,10 @@ def import_reference():
 
 
 def make_reference_env(name, n=None):
-    """Reference env for `name`; `simple_spread` accepts n (agents = landmarks = n) by building
-    the world test-side with the reference's own property assignments (simple_spread.py:15-26)
-    and reusing its generic reset_world / reward / observation (SURVEY.md 8(c) "N=6 spread")."""
+    """Reference env for `name`; `simple_spread` accepts n (agents = landmarks = n), `simple_tag` a tuple
+    (adversaries, good agents, landmarks) and `simple_adversary` n (agents; n - 1 landmarks), by building the
+    world test-side with the reference's own property assignments (e.g. simple_spread.py:15-26) and reusing
+    its generic reset_world / reward / observation (SURVEY.md 8(c) "N=6 spread")."""
     make_env, multiagent = import_reference()
     if name == "simple_spread" and n not in (None, 3):
         from multiagent.core import World, Agent, Landmark
@@ -175,6 +176,32 @@ def make_reference_env(name, n=None):
             landmark.movable = False
             landmark.size = 0.2
             landmark.boundary = False
+        scenario.reset_world(world)
+        return MultiAgentEnv(world, scenario.reset_world, scenario.reward, scenario.observation, scenario.benchmark_data)
+    if name == "simple_adversary" and n not in (None, 3):
+        # n agents (one adversary) and n - 1 landmarks, built test-side with the reference's own property assignments
+        # (simple_adversary.py:8-31); its reset_world / reward / observation / benchmark_data are generic over
+        # world.num_agents / world.agents / world.landmarks and are reused unchanged
+        from multiagent.core import World, Agent, Landmark
+        from multiagent.environment import MultiAgentEnv
+        import multiagent.scenarios as scenarios
+        scenario = scenarios.load("simple_adversary.py").Scenario()
+        world = World()
+        world.dim_c = 2
+        world.num_agents = n
+        world.agents = [Agent() for _ in range(n)]
+        for i, agent in enumerate(world.agents):
+            agent.name = "agent %d" % i
+            agent.collide = False
+            agent.silent = True
+            agent.adversary = i < 1
+            agent.size = 0.15
+        world.landmarks = [Landmark() for _ in range(n - 1)]
+        for i, landmark in enumerate(world.landmarks):
+            landmark.name = "landmark %d" % i
+            landmark.collide = False
+            landmark.movable = False
+            landmark.size = 0.08
         scenario.reset_world(world)
         return MultiAgentEnv(world, scenario.reset_world, scenario.reward, scenario.observation, scenario.benchmark_data)
     return make_env(name, benchmark=(name not in ("simple", "simple_push", "simple_reference",

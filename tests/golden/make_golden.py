@@ -11,7 +11,11 @@ some worlds start outside the arena so that tag's bound() penalty is exercised. 
 the known-answer trajectories of SURVEY.md section 8(c) (np.random.seed(0); reset; 2 steps).
 
 The fixtures pin oracle/mpe_oracle.c (tests/test_oracle_golden.py) and, through it and directly,
-the CUDA kernels (tests/test_gpu_parity.py).
+the CUDA kernels (tests/test_gpu_parity.py): the ten reference scenarios, simple_tag with forced
+discrete and with integer actions, and the entity-count variants simple_spread N = 2, 4, 5,
+simple_tag 1+1, 2+1, 4+2, 6+2 and simple_adversary with 4 agents (64 worlds x 6 steps each), whose
+worlds are built test-side with the reference's own property assignments (oracle/refshim.py).  The
+oracle pins every other seeded-world check of those programs.
 """
 import os
 import sys
@@ -218,8 +222,14 @@ def main():
     np.savez_compressed(os.path.join(HERE, "simple_tag_force_discrete.npz"), **data)
     data = run_config("simple_tag", None, 64, 8, seed=78, discrete_input=True)
     np.savez_compressed(os.path.join(HERE, "simple_tag_discrete_input.npz"), **data)
-    for counts, tag in (((1, 1, 2), "simple_tag_1v1"), ((4, 2, 2), "simple_tag_4v2"), ((6, 2, 3), "simple_tag_6v2")):
+    for counts, tag in (((1, 1, 2), "simple_tag_1v1"), ((4, 2, 2), "simple_tag_4v2"), ((6, 2, 3), "simple_tag_6v2"),
+                        ((2, 1, 2), "simple_tag_2v1")):
         data = run_config("simple_tag", counts, 64, 6, seed=80 + counts[0])     # entity-count variants
+        np.savez_compressed(os.path.join(HERE, tag + ".npz"), **data)
+    for name, n, tag, seed in (("simple_spread", 2, "simple_spread_n2", 92), ("simple_spread", 4, "simple_spread_n4", 94),
+                               ("simple_spread", 5, "simple_spread_n5", 95),
+                               ("simple_adversary", 4, "simple_adversary_n4", 104)):
+        data = run_config(name, n, 64, 6, seed=seed)
         np.savez_compressed(os.path.join(HERE, tag + ".npz"), **data)
     np.savez_compressed(os.path.join(HERE, "kat.npz"), **kat())
 

@@ -18,8 +18,11 @@ CONFIGS = {
     "simple_reference": ("simple_reference", {}),
     "simple_crypto": ("simple_crypto", {}),
 }
-# entity-count variants the reference hard-codes away (no goldens; checked against the generic oracle)
+# entity-count variants the reference hard-codes away (their goldens build the world test-side, oracle/refshim.py)
 VARIANTS = {
+    "simple_spread_n2": ("simple_spread", {"num_agents": 2}),
+    "simple_spread_n4": ("simple_spread", {"num_agents": 4}),
+    "simple_spread_n5": ("simple_spread", {"num_agents": 5}),
     "simple_tag_1v1": ("simple_tag", {"num_adversaries": 1, "num_good_agents": 1, "num_landmarks": 2}),
     "simple_tag_2v1": ("simple_tag", {"num_adversaries": 2, "num_good_agents": 1, "num_landmarks": 2}),
     "simple_tag_4v2": ("simple_tag", {"num_adversaries": 4, "num_good_agents": 2, "num_landmarks": 2}),
@@ -27,6 +30,18 @@ VARIANTS = {
     "simple_adversary_n4": ("simple_adversary", {"num_agents": 4}),
 }
 NO_BENCHMARK = ("simple", "simple_push", "simple_speaker_listener", "simple_reference")
+# every program the library compiles (csrc/mpe_kernels.cu programs()), one tag each
+PROGRAM_TAGS = list(CONFIGS) + list(VARIANTS)
+assert len(PROGRAM_TAGS) == 18
+# the program types of csrc/mpe_kernels.cu (make_program), as c++filt prints them
+TYPE_TAGS = {
+    "Simple<1, 1>": "simple", "Spread<2>": "simple_spread_n2", "Spread<3>": "simple_spread_n3",
+    "Spread<4>": "simple_spread_n4", "Spread<5>": "simple_spread_n5", "Spread<6>": "simple_spread_n6",
+    "Tag<3, 1, 2>": "simple_tag", "Tag<1, 1, 2>": "simple_tag_1v1", "Tag<2, 1, 2>": "simple_tag_2v1",
+    "Tag<4, 2, 2>": "simple_tag_4v2", "Tag<6, 2, 3>": "simple_tag_6v2", "WorldComm<4, 2, 1, 2>": "simple_world_comm",
+    "Adversary<1, 2, 2>": "simple_adversary", "Adversary<1, 3, 3>": "simple_adversary_n4", "Push<1, 1, 2>": "simple_push",
+    "SpeakerListener": "simple_speaker_listener", "Reference": "simple_reference", "Crypto": "simple_crypto",
+}
 
 
 def load_golden(tag):
@@ -113,7 +128,7 @@ def random_actions(act_dims, n, rng, temperature=2.0, movable=None):
 #   "mlp"     rollout_policy_mlp, all six forms: ceil(warps / sms) warps per block, capped at mlp_block_warps
 #            (mirrored by mlp_programs.mlp_block_cap)
 # The shared-memory caps (max_warps_per_block) never bind for the built-in scenarios at 4 warps per block.
-STEP_DENSE_TAGS = ("simple_tag", "simple_tag_2v1", "simple_tag_4v2")    # the test tags with a hot_dense_fn
+STEP_DENSE_TAGS = ("simple_tag", "simple_tag_2v1", "simple_tag_4v2", "simple_spread_n4")   # the tags with a hot_dense_fn
 
 
 def device_sms():

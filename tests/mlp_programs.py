@@ -2,17 +2,12 @@
 the GPU tests of that actor share (seeded actors, twin envs)."""
 import functools
 
-from helpers import CONFIGS, NO_BENCHMARK, VARIANTS, make_product_env
+from helpers import CONFIGS, VARIANTS, make_product_env
 
 # The entity-count variants, tag -> (scenario name, scenario kwargs)
-VARIANT_PROGRAMS = {
-    "simple_spread_n2": ("simple_spread", {"num_agents": 2}),
-    "simple_spread_n4": ("simple_spread", {"num_agents": 4}),
-    "simple_spread_n5": ("simple_spread", {"num_agents": 5}),
-    "simple_spread_n6": CONFIGS["simple_spread_n6"],
-    **{tag: VARIANTS[tag] for tag in ("simple_tag_1v1", "simple_tag_2v1", "simple_tag_4v2", "simple_tag_6v2",
-                                      "simple_adversary_n4")},
-}
+VARIANT_PROGRAMS = {tag: CONFIGS[tag] if tag in CONFIGS else VARIANTS[tag]
+                    for tag in ("simple_spread_n2", "simple_spread_n4", "simple_spread_n5", "simple_spread_n6",
+                                "simple_tag_1v1", "simple_tag_2v1", "simple_tag_4v2", "simple_tag_6v2", "simple_adversary_n4")}
 # every program mpe_policy_mlp_rollout_kernel is built for (MlpBuilt): all but simple_world_comm
 PROGRAMS = {**{t: s for t, s in CONFIGS.items() if t != "simple_world_comm"}, **VARIANT_PROGRAMS}
 assert len(PROGRAMS) == 17
@@ -24,21 +19,10 @@ TIGHT_ATOL = 1e-5
 LOOSE_MAX = 5e-3
 
 
-def make_variant_env(tag, **kw):
-    from multiagent_particle_envs_b200 import make_env
-    name, skw = VARIANT_PROGRAMS[tag]
-    kw.update(skw)
-    return make_env(name, benchmark=(name not in NO_BENCHMARK), **kw)
-
-
-def make_program_env(tag, **kw):
-    return make_variant_env(tag, **kw) if tag in VARIANT_PROGRAMS else make_product_env(tag, **kw)
-
-
 @functools.lru_cache(maxsize=None)
 def shapes_of(tag):
     """(obs_dims, act_dims) of a program, from its shape-only handle"""
-    s = make_program_env(tag, num_envs=1).world.native_shapes()
+    s = make_product_env(tag, num_envs=1).world.native_shapes()
     return tuple(s.obs_dims), tuple(s.act_dims)
 
 
@@ -147,8 +131,8 @@ def as_sequential(pols):
 
 
 def twins(tag, n, seed=9, **kw):
-    a = make_program_env(tag, num_envs=n, seed=seed, **kw)
-    b = make_program_env(tag, num_envs=n, seed=seed, **kw)
+    a = make_product_env(tag, num_envs=n, seed=seed, **kw)
+    b = make_product_env(tag, num_envs=n, seed=seed, **kw)
     a.reset()
     b.reset()
     return a, b

@@ -1,7 +1,8 @@
 """CPU checks that tie the two-hidden-layer actor's host side to the built library: every one of its 170 kernels (17
 programs x H = 32, 64 x the four MADDPG forms, and 17 programs x MAPPO's two forms at H = 64) is compiled for the block
 size the test mirror (mlp_programs.mlp_block_cap) expects, read from the kernel's launch bounds in libmpe_b200.so; and
-the six entry points refuse what they can refuse without a device with the return codes they always had."""
+the six entry points refuse what they can refuse without a device with the return codes they always had.  Also: the
+programs with step, rollout and 80-register step kernels in the library are the ones the GPU tests parametrize."""
 import os
 import re
 import shutil
@@ -9,20 +10,11 @@ import subprocess
 
 import pytest
 
-from helpers import make_product_env
+from helpers import PROGRAM_TAGS, STEP_DENSE_TAGS, TYPE_TAGS, make_product_env
 from mlp_programs import PROGRAMS, mlp_block_cap
 
 pytest.importorskip("torch")
 
-# the program types of csrc/mpe_kernels.cu (make_program), as c++filt prints them
-TYPE_TAGS = {
-    "Simple<1, 1>": "simple", "Spread<2>": "simple_spread_n2", "Spread<3>": "simple_spread_n3",
-    "Spread<4>": "simple_spread_n4", "Spread<5>": "simple_spread_n5", "Spread<6>": "simple_spread_n6",
-    "Tag<3, 1, 2>": "simple_tag", "Tag<1, 1, 2>": "simple_tag_1v1", "Tag<2, 1, 2>": "simple_tag_2v1",
-    "Tag<4, 2, 2>": "simple_tag_4v2", "Tag<6, 2, 3>": "simple_tag_6v2", "Adversary<1, 2, 2>": "simple_adversary",
-    "Adversary<1, 3, 3>": "simple_adversary_n4", "Push<1, 1, 2>": "simple_push",
-    "SpeakerListener": "simple_speaker_listener", "Reference": "simple_reference", "Crypto": "simple_crypto",
-}
 # kernel name -> (episodes, categorical, mappo)
 FORMS = {"mlp_rollout": (False, False, False), "mlp_episode": (True, False, False),
          "mlp_categorical": (False, True, False), "mlp_categorical_episode": (True, True, False),
@@ -74,6 +66,29 @@ def test_launch_bounds_are_the_mirrored_caps():
     assert sum(k[4] for k in seen) == 34
     want = {(tag, H, e, c, mp): 32 * mlp_block_cap(tag, H, e, c, mp) for tag, H, e, c, mp in seen}
     assert seen == want
+
+
+def test_every_step_program_is_in_the_test_tables():
+    """The programs with a fused step (mpe_kernel) and an open-loop rollout (mpe_rollout_kernel) in libmpe_b200.so are
+    exactly helpers.PROGRAM_TAGS, which the step, rollout and reset tests run; those with the 80-register HOT build
+    (mpe_kernel<P, kFusedStep, true, true>) are exactly helpers.STEP_DENSE_TAGS, which the oracle test runs at sizes
+    that select it.  A program or a low-register build added without a place in those tests fails here."""
+    from multiagent_particle_envs_b200 import _lib
+    names = list(max_threads_per_kernel(_lib.LIB_PATH))
+    demangled = subprocess.run(["c++filt"], input="\n".join(names), capture_output=True, text=True,
+                               check=True).stdout.split("\n")
+    step, rollout, dense = set(), set(), set()
+    for nm in demangled:
+        m = re.match(r"void mpe::mpe_kernel<mpe::(.+), (\d), (true|false), (true|false)>\(", nm)
+        if m:
+            step.add(TYPE_TAGS[m.group(1)])
+            if (m.group(2), m.group(3), m.group(4)) == ("0", "true", "true"):      # kFusedStep, HOT, DENSE
+                dense.add(TYPE_TAGS[m.group(1)])
+        m = re.match(r"void mpe::mpe_rollout_kernel<mpe::(.+?)\s*>\(", nm)
+        if m:
+            rollout.add(TYPE_TAGS[m.group(1)])
+    assert step == rollout == set(PROGRAM_TAGS)
+    assert dense == set(STEP_DENSE_TAGS)
 
 
 # ---- return codes without a device ---------------------------------------------------------------------------------

@@ -4,7 +4,7 @@ opt-in limit for the variants, computed from the shape-only handle's observation
 import pytest
 
 from helpers import make_product_env
-from mlp_programs import (SMEM_OPTIN_BYTES, make_variant_env, mlp_block_cap, mlp_register_rule, mlp_register_warps,
+from mlp_programs import (SMEM_OPTIN_BYTES, mlp_block_cap, mlp_register_rule, mlp_register_warps,
                           mlp_smem_bytes)
 from mlp_programs import VARIANT_PROGRAMS as PROGRAMS
 
@@ -27,7 +27,7 @@ def test_existing_programs_keep_their_cap(tag, H):
 @pytest.mark.parametrize("tag", list(PROGRAMS))
 @pytest.mark.parametrize("H", [32, 64])
 def test_variant_cap_fits_shared_memory(tag, H):
-    shapes = make_variant_env(tag, num_envs=64).world.native_shapes()          # device-less handle
+    shapes = make_product_env(tag, num_envs=64).world.native_shapes()          # device-less handle
     obs_dims, act_dims = list(shapes.obs_dims), list(shapes.act_dims)
     assert act_dims == [5] * len(obs_dims)
     cap = mlp_block_cap(tag, H)
@@ -43,7 +43,7 @@ def test_shared_memory_binds_only_for_the_largest_programs():
     (its registers allow 8), tag 6+2's 212 KB for 3; shared memory binds for no other (program, H)"""
     binding = {}
     for tag in PROGRAMS:
-        shapes = make_variant_env(tag, num_envs=64).world.native_shapes()
+        shapes = make_product_env(tag, num_envs=64).world.native_shapes()
         od, ad = list(shapes.obs_dims), list(shapes.act_dims)
         for H in (32, 64):
             if mlp_smem_bytes(H, od, ad, mlp_register_warps(tag, H)) > SMEM_OPTIN_BYTES:

@@ -4,7 +4,7 @@ scalar (batch-1, NumPy) convention for every scenario, benchmark_data shapes, go
 import numpy as np
 import pytest
 
-from helpers import CONFIGS, NO_BENCHMARK, load_golden, make_product_env, split_cols
+from helpers import CONFIGS, NO_BENCHMARK, PROGRAM_TAGS, load_golden, make_product_env, split_cols
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -65,32 +65,62 @@ def test_scenario_callbacks_and_env_accessors():
     assert (frames[0] != 255).any() and (frames[0] == 255).mean() > 0.5
 
 
-@pytest.mark.parametrize("tag", ["simple_tag", "simple_world_comm", "simple_speaker_listener"])
-def test_discrete_action_input(tag):
-    """env.discrete_action_input = True: integer sub-actions (environment.py:161-167, 185-187)"""
+def integer_decode_vs_oracle(tag, force_discrete):
+    """one fused step with integer sub-actions (discrete_action_input) or with probability vectors under
+    force_discrete_action, against the f64 oracle with the same flag; the batch size has a ragged last warp"""
     from oracle import Oracle
     from multiagent_particle_envs_b200 import _lib
-    n = 1024
+    from helpers import explain_flag_mismatches, random_actions
+    n = 1031
     env = make_product_env(tag, num_envs=n)
-    env.discrete_action_input = True
+    env.discrete_action_input = not force_discrete
+    env.force_discrete_action = force_discrete
     env.reset()
     nw, desc = env.world.native, env.world.descriptor()
     rng = np.random.RandomState(5)
     pv0 = nw.agent_pv.permute(1, 0, 2).cpu().numpy()
     lm0 = nw.lm_p.permute(1, 0, 2).cpu().numpy()
     goal = nw.goal.t().cpu().numpy() if nw.n_goals else None
-    ints = []
-    for i in range(desc.n_agents):
-        cols = ([rng.randint(0, 5, n)] if desc.agent_movable[i] else []) + \
-               ([rng.randint(0, desc.dim_c, n)] if not desc.agent_silent[i] else [])
-        ints.append(np.stack(cols, 1))
-    obs_n, rew_n, _, _ = env.step([torch.as_tensor(a, device="cuda") for a in ints])
-    flat = np.concatenate(ints, 1).astype(np.float64)
-    flags = _lib.FLAG_DISCRETE_ACTION_INPUT | (_lib.FLAG_SHARED_REWARD if env.shared_reward else 0)
+    if force_discrete:
+        movable = [bool(desc.agent_movable[i]) for i in range(desc.n_agents)]
+        flat = random_actions(nw.act_dims, n, rng, movable=movable).astype(np.float32)
+        acts = [torch.as_tensor(np.ascontiguousarray(a), device="cuda") for a in split_cols(flat, nw.act_dims)]
+        flags = _lib.FLAG_FORCE_DISCRETE_ACTION
+    else:
+        acts = []
+        for i in range(desc.n_agents):
+            cols = ([rng.randint(0, 5, n)] if desc.agent_movable[i] else []) + \
+                   ([rng.randint(0, desc.dim_c, n)] if not desc.agent_silent[i] else [])
+            acts.append(np.stack(cols, 1))
+        flat = np.concatenate(acts, 1).astype(np.float64)
+        acts = [torch.as_tensor(a, device="cuda") for a in acts]
+        flags = _lib.FLAG_DISCRETE_ACTION_INPUT
+    flags |= _lib.FLAG_SHARED_REWARD if env.shared_reward else 0
+    obs_n, rew_n, _, _ = env.step(acts)
     rpv, rcomm, robs, rrew, _, _ = Oracle(desc, "f64").step(pv0, lm0, np.zeros((n, desc.n_agents, desc.dim_c)), flat,
                                                             flags, goal=goal)
+    pv = nw.agent_pv.permute(1, 0, 2).cpu().numpy()
     np.testing.assert_allclose(np.concatenate([o.cpu().numpy() for o in obs_n], 1), robs, rtol=RTOL, atol=ATOL)
-    np.testing.assert_allclose(nw.agent_pv.permute(1, 0, 2).cpu().numpy(), rpv, rtol=RTOL, atol=ATOL)
+    np.testing.assert_allclose(pv, rpv, rtol=RTOL, atol=ATOL)
+    for i in range(desc.n_agents):                       # utterances are copies: exact
+        s = nw.speaker_slot(i)
+        if s >= 0 and desc.dim_c:
+            assert np.array_equal(nw.comm[s * desc.dim_c:(s + 1) * desc.dim_c].t().cpu().numpy(), rcomm[:, i])
+    explain_flag_mismatches(tag, torch.stack(rew_n, 1).cpu().numpy(), rrew, None, None, rpv, lm0,
+                            [desc.agent_size[i] for i in range(desc.n_agents)],
+                            [desc.landmark_size[l] for l in range(desc.n_landmarks)])
+
+
+@pytest.mark.parametrize("tag", PROGRAM_TAGS)
+def test_discrete_action_input(tag):
+    """env.discrete_action_input = True: integer sub-actions (environment.py:161-167, 185-187)"""
+    integer_decode_vs_oracle(tag, force_discrete=False)
+
+
+@pytest.mark.parametrize("tag", PROGRAM_TAGS)
+def test_force_discrete_action(tag):
+    """env.force_discrete_action = True: the movement vector's argmax becomes a one-hot (environment.py:169-172)"""
+    integer_decode_vs_oracle(tag, force_discrete=True)
 
 
 def test_scalar_mode_with_integer_actions():
@@ -209,20 +239,11 @@ def test_graphed_rollout_with_resets_draws_fresh_episodes_on_replay():
     assert int(nw._epoch_dev.item()) == e1 + 2
 
 
-@pytest.mark.parametrize("tag,n,T", [("simple_spread_n3", 2049, 25), ("simple_tag", 4096, 10), ("simple_world_comm", 1031, 7),
-                                     ("simple_reference", 512, 6), ("simple_speaker_listener", 100, 5),
-                                     ("simple_crypto", 333, 4), ("simple_adversary", 64, 9), ("simple", 33, 3),
-                                     ("simple_spread_n3", "2warp", 4), ("simple_tag", "4warp", 3)])
-def test_open_loop_rollout_equals_repeated_steps(tag, n, T):
-    """env.rollout (mpe_rollout: T steps in one launch, state in registers, next step's actions prefetched) is
-    bit-identical to T calls of env.step on the same actions with the rewards summed in step order -- full tiles take
-    the cp.async path, the ragged last tile the scalar one.  "2warp" / "4warp": sizes with 2- / 4-warp blocks
-    (helpers.launch_shape "rollout"), partial last block and ragged last warp"""
-    if isinstance(n, str):
-        from helpers import device_sms, regime_size
-        n = regime_size("rollout", device_sms(), int(n[0]))
+def rollout_vs_steps(tag, n, T, force_discrete=False):
+    """env.rollout on T random action steps against T env.step calls of a twin env, bit for bit"""
     env_a = make_product_env(tag, num_envs=n, seed=5)
     env_b = make_product_env(tag, num_envs=n, seed=5)
+    env_a.force_discrete_action = env_b.force_discrete_action = force_discrete
     env_a.reset()
     env_b.reset()
     na, nb = env_a.world.native, env_b.world.native
@@ -248,9 +269,35 @@ def test_open_loop_rollout_equals_repeated_steps(tag, n, T):
     assert not any(bool(d.any()) for d in done_r)
     # without the per-step record the result is the same
     env_c = make_product_env(tag, num_envs=n, seed=5)
+    env_c.force_discrete_action = force_discrete
     env_c.reset()
     obs_c, rew_c, _, _ = env_c.rollout(seqs)
     assert all(torch.equal(x, y) for x, y in zip(obs_c, obs_r)) and torch.equal(torch.stack(list(rew_c)), rew_sum)
+
+
+@pytest.mark.parametrize("tag,n,T", [("simple_spread_n3", 2049, 25), ("simple_tag", 4096, 10), ("simple_world_comm", 1031, 7),
+                                     ("simple_reference", 512, 6), ("simple_speaker_listener", 100, 5),
+                                     ("simple_crypto", 333, 4), ("simple_adversary", 64, 9), ("simple", 33, 3),
+                                     ("simple_spread_n3", "2warp", 4), ("simple_tag", "4warp", 3)]
+                         # every program: whole tiles with 16-byte aligned action rows (the cp.async path), and an odd
+                         # size (the scalar tile path, ragged last tile)
+                         + [(tag, n, 4) for tag in PROGRAM_TAGS for n in (640, 645)])
+def test_open_loop_rollout_equals_repeated_steps(tag, n, T):
+    """env.rollout (mpe_rollout: T steps in one launch, state in registers, next step's actions prefetched) is
+    bit-identical to T calls of env.step on the same actions with the rewards summed in step order -- full tiles take
+    the cp.async path, the ragged last tile the scalar one.  "2warp" / "4warp": sizes with 2- / 4-warp blocks
+    (helpers.launch_shape "rollout"), partial last block and ragged last warp"""
+    if isinstance(n, str):
+        from helpers import device_sms, regime_size
+        n = regime_size("rollout", device_sms(), int(n[0]))
+    rollout_vs_steps(tag, n, T)
+
+
+@pytest.mark.parametrize("tag", ["simple_tag", "simple_speaker_listener"])
+def test_open_loop_rollout_under_force_discrete_action(tag):
+    """with env.force_discrete_action the rollout kernel moves by the one-hot argmax of every step's movement vector
+    (utterances stay as given, environment.py:169-190), as the fused step does"""
+    rollout_vs_steps(tag, 645, 4, force_discrete=True)
 
 
 @pytest.mark.parametrize("tag,n,T,H", [("simple_spread_n3", 2049, 12, 32), ("simple_spread_n3", 1000, 8, 64),

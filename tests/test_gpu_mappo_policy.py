@@ -11,7 +11,7 @@ from helpers import device_sms, launch_shape, make_product_env, regime_size
 from mappo_helpers import FEATURE_NORM, TANH, MappoModel, explain_mappo_mismatches, make_mappo_actors, module_logits
 from mlp_categorical_helpers import bounds, log_softmax_at, one_hot_torch
 from mlp_helpers import gumbel_noise
-from mlp_programs import PROGRAMS, make_program_env, mlp_block_cap, state, twins
+from mlp_programs import PROGRAMS, mlp_block_cap, state, twins
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -185,7 +185,7 @@ def test_a_shared_policy_equals_equal_copies():
 def test_refusals_leave_state_and_epochs_unchanged():
     from multiagent_particle_envs_b200 import _lib
     from multiagent_particle_envs_b200._lib import MpeError
-    env = make_program_env("simple_spread_n3", num_envs=64, seed=9)
+    env = make_product_env("simple_spread_n3", num_envs=64, seed=9)
     env.reset()
     nw = env.world.native
     before, epoch = state(env), nw.epoch

@@ -12,7 +12,7 @@ from helpers import device_sms, launch_shape, make_product_env, regime_size
 from mlp_categorical_helpers import (bounds, categorical_pick, explain_categorical_mismatches, log_softmax_at,
                                      one_hot_torch)
 from mlp_helpers import actor_logits, gumbel_noise, segment_softmax
-from mlp_programs import PROGRAMS, as_sequential, make_policies, make_program_env, mlp_block_cap, state, twins
+from mlp_programs import PROGRAMS, as_sequential, make_policies, mlp_block_cap, state, twins
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -283,7 +283,7 @@ def test_sequential_actors_equal_tuples_and_a_seed_reproduces(tag):
             assert torch.equal(x, y), key
     assert env_a.explore_epoch == 1
     # the same seed and epoch from the same state reproduce every record; the next epoch draws other samples
-    env_c = make_program_env(tag, num_envs=1031, seed=9)
+    env_c = make_product_env(tag, num_envs=1031, seed=9)
     env_c.reset()
     rc = env_c.rollout_policy(pols, 5, explore_seed=2, action_mode="categorical", **RECORDS)
     rd = env_c.rollout_policy(pols, 5, explore_seed=2, action_mode="categorical", **RECORDS)
@@ -301,14 +301,14 @@ def test_sequential_actors_equal_tuples_and_a_seed_reproduces(tag):
 @pytest.mark.parametrize("tag", ["simple_spread_n3", "simple_speaker_listener"])
 def test_sharded_categorical_equals_the_full_batch(tag):
     n, T = 1031, 4
-    full = make_program_env(tag, num_envs=n, seed=9)
+    full = make_product_env(tag, num_envs=n, seed=9)
     full.reset()
     nw = full.world.native
     pols = make_policies(nw.obs_dims, nw.act_dims, 32)
     ex = full.rollout_policy(pols, T, explore_seed=77, action_mode="categorical", **RECORDS)[4]
     lo = 0
     for rank in range(2):
-        sh = make_program_env(tag, num_envs=n, seed=9, rank=rank, world_size=2)
+        sh = make_product_env(tag, num_envs=n, seed=9, rank=rank, world_size=2)
         sh.reset()
         m = sh.world.native.n_env
         ex_s = sh.rollout_policy(pols, T, explore_seed=77, action_mode="categorical", **RECORDS)[4]
@@ -321,7 +321,7 @@ def test_sharded_categorical_equals_the_full_batch(tag):
 
 
 def test_records_are_none_unless_requested():
-    env = make_program_env("simple_speaker_listener", num_envs=100, seed=9)
+    env = make_product_env("simple_speaker_listener", num_envs=100, seed=9)
     env.reset()
     nw = env.world.native
     pols = make_policies(nw.obs_dims, nw.act_dims, 32)
@@ -338,7 +338,7 @@ def test_records_are_none_unless_requested():
 
 def test_refusals_leave_state_and_epochs_unchanged():
     from multiagent_particle_envs_b200._lib import MpeError
-    env = make_program_env("simple_spread_n3", num_envs=64, seed=9)
+    env = make_product_env("simple_spread_n3", num_envs=64, seed=9)
     env.reset()
     nw = env.world.native
     before, epoch = state(env), nw.epoch
@@ -365,7 +365,7 @@ def test_refusals_leave_state_and_epochs_unchanged():
         env.rollout_policy(pols, 7, episode_length=2, action_mode="categorical")
     unchanged(env, before, epoch)
     # (t * 8 + i) * 2 + b must stay below the tag bit 2^30: tag 6+2 at 2^26 + 1 steps, in both forms
-    tag = make_program_env("simple_tag_6v2", num_envs=64, seed=9)
+    tag = make_product_env("simple_tag_6v2", num_envs=64, seed=9)
     tag.reset()
     tnw = tag.world.native
     tbefore, tepoch = state(tag), tnw.epoch

@@ -12,7 +12,7 @@ worlds plus a tail at the block cap; then reseeding, sharding, the device epoch 
 import pytest
 
 from helpers import device_sms, launch_shape, make_product_env, regime_size
-from mlp_programs import PROGRAMS, as_sequential, make_policies, make_program_env, mlp_block_cap, state, twins
+from mlp_programs import PROGRAMS, as_sequential, make_policies, mlp_block_cap, state, twins
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -129,7 +129,7 @@ def test_reseeding_reproduces_the_episodes(tag):
 def test_sharded_episodes_equal_the_full_batch(tag):
     """the global world index keys both the reset draw and the exploration noise"""
     E, L, n = 2, 3, 1031
-    full = make_program_env(tag, num_envs=n, seed=9)
+    full = make_product_env(tag, num_envs=n, seed=9)
     full.reset()
     nw = full.world.native
     pols = make_policies(nw.obs_dims, nw.act_dims, 32)
@@ -137,7 +137,7 @@ def test_sharded_episodes_equal_the_full_batch(tag):
     want = state(full)
     lo = 0
     for rank in range(2):
-        sh = make_program_env(tag, num_envs=n, seed=9, rank=rank, world_size=2)
+        sh = make_product_env(tag, num_envs=n, seed=9, rank=rank, world_size=2)
         sh.reset()
         m = sh.world.native.n_env
         assert sh.world.native.world_offset == lo
@@ -195,7 +195,7 @@ def test_sequential_actors_equal_tuples(tag):
 
 def test_refusals_leave_state_and_epochs_unchanged():
     from multiagent_particle_envs_b200._lib import MpeError
-    env = make_program_env("simple_spread_n3", num_envs=64, seed=9)
+    env = make_product_env("simple_spread_n3", num_envs=64, seed=9)
     env.reset()
     nw = env.world.native
     before, epoch = state(env), nw.epoch
@@ -232,7 +232,7 @@ def test_exploring_episodes_refuse_a_counter_overflow_per_episode():
     """(t * 8 + i) * 2 + b, t < episode_length, must stay below the tag bit 2^30: tag 6+2 with episodes of 2^26 + 1 steps
     is refused before anything runs (no records requested, nothing of that size is allocated)"""
     from multiagent_particle_envs_b200._lib import MpeError
-    env = make_program_env("simple_tag_6v2", num_envs=64, seed=9)
+    env = make_product_env("simple_tag_6v2", num_envs=64, seed=9)
     env.reset()
     nw = env.world.native
     before, epoch = state(env), nw.epoch
@@ -246,7 +246,7 @@ def test_exploring_episodes_refuse_a_counter_overflow_per_episode():
 
 
 def test_records_are_none_unless_requested():
-    env = make_program_env("simple_speaker_listener", num_envs=100, seed=9)
+    env = make_product_env("simple_speaker_listener", num_envs=100, seed=9)
     env.reset()
     nw = env.world.native
     epoch = nw.epoch

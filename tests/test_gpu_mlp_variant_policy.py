@@ -8,9 +8,9 @@ import json
 import numpy as np
 import pytest
 
-from helpers import device_sms, launch_shape, regime_size
+from helpers import device_sms, launch_shape, make_product_env, regime_size
 from mlp_helpers import actor_logits, explain_tf32_mismatches, gumbel_noise, softmax
-from mlp_programs import LOOSE_MAX, TIGHT_ATOL, as_sequential, make_policies, make_variant_env, mlp_block_cap
+from mlp_programs import LOOSE_MAX, TIGHT_ATOL, as_sequential, make_policies, mlp_block_cap
 from mlp_programs import VARIANT_PROGRAMS as PROGRAMS
 
 pytestmark = pytest.mark.gpu
@@ -41,8 +41,8 @@ def mlp_size(tag, shape, H):
 
 
 def twin_envs(tag, n, seed=9, **kw):
-    a = make_variant_env(tag, num_envs=n, seed=seed, **kw)
-    b = make_variant_env(tag, num_envs=n, seed=seed, **kw)
+    a = make_product_env(tag, num_envs=n, seed=seed, **kw)
+    b = make_product_env(tag, num_envs=n, seed=seed, **kw)
     a.reset()
     obs_b = b.reset()
     assert torch.equal(a.world.native.agent_pv, b.world.native.agent_pv)
@@ -99,7 +99,7 @@ def test_launched_block_size_is_the_mirrored_cap(tag, H, tmp_path):
     from torch.profiler import ProfilerActivity, profile
     n = mlp_size(tag, "full", H)
     cap = mlp_block_cap(tag, H)
-    env = make_variant_env(tag, num_envs=n, seed=9)
+    env = make_product_env(tag, num_envs=n, seed=9)
     env.reset()
     nw = env.world.native
     pols = make_policies(nw.obs_dims, nw.act_dims, H)
@@ -146,7 +146,7 @@ def test_variant_exploration_is_reproducible_advances_and_is_independent_of_shar
     # two shards draw the rows of the whole batch, bit for bit
     lo = 0
     for rank in range(2):
-        sh = make_variant_env(tag, num_envs=n, seed=9, rank=rank, world_size=2)
+        sh = make_product_env(tag, num_envs=n, seed=9, rank=rank, world_size=2)
         sh.reset()
         m = sh.world.native.n_env
         assert sh.world.native.world_offset == lo
@@ -162,7 +162,7 @@ def test_tag_6v2_exploring_rollout_refuses_a_counter_overflow():
     2^30, so 2^26 + 1 steps are refused before anything runs (no records requested, nothing of that size is
     allocated)"""
     from multiagent_particle_envs_b200._lib import MpeError
-    env = make_variant_env("simple_tag_6v2", num_envs=64, seed=9)
+    env = make_product_env("simple_tag_6v2", num_envs=64, seed=9)
     env.reset()
     nw = env.world.native
     pv = nw.agent_pv.clone()

@@ -6,8 +6,9 @@ on the kernels' own stored state.  Run on an H100: pytest -m gpu."""
 import numpy as np
 import pytest
 
-from helpers import (CONFIGS, VARIANTS, VELOCITY_TERM_ULPS, explain_flag_mismatches, load_golden, make_product_env,
-                     random_actions, random_goals, random_states, scenario_of, split_cols, velocity_term_scale)
+from helpers import (CONFIGS, PROGRAM_TAGS, STEP_DENSE_TAGS, VARIANTS, VELOCITY_TERM_ULPS, explain_flag_mismatches,
+                     load_golden, make_product_env, random_actions, random_goals, random_states, scenario_of, split_cols,
+                     velocity_term_scale)
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -61,7 +62,9 @@ def gpu_step(env, act, flags_expected=None):
     return obs, rew, done, info
 
 
-GOLDEN_VARIANTS = ["simple_tag_1v1", "simple_tag_4v2", "simple_tag_6v2"]   # reference worlds with other entity counts
+# reference worlds with other entity counts
+GOLDEN_VARIANTS = ["simple_tag_1v1", "simple_tag_4v2", "simple_tag_6v2", "simple_tag_2v1", "simple_spread_n2",
+                   "simple_spread_n4", "simple_spread_n5", "simple_adversary_n4"]
 
 
 @pytest.mark.parametrize("tag", TAGS + ["simple_tag_force_discrete", "simple_tag_discrete_input"] + GOLDEN_VARIANTS)
@@ -127,15 +130,24 @@ def close_per_element(got, want, slack=0.0):
                                    # production sizes (BASELINE.json) and launch shapes of the fused step, see
                                    # helpers.launch_shape "step": (hot kernel, warps per block) -- resolved on the device
                                    ("simple_spread_n3", 65536), ("simple_tag", 262144), ("simple_spread_n6", 131072),
-                                   ("simple_world_comm", 32768), ("simple_tag", "dense_4warp_ragged")])
+                                   ("simple_world_comm", 32768), ("simple_tag", "dense_4warp_ragged")]
+                         # every program: 1-warp blocks of the HOT kernel and the general kernel's ragged tail
+                         + [(tag, "1warp_ragged") for tag in PROGRAM_TAGS]
+                         # the 80-register builds in 2- and 4-warp blocks, partial last block, ragged tail
+                         + [(tag, r) for tag in STEP_DENSE_TAGS for r in ("dense_2warp_ragged", "dense_4warp_ragged")
+                            if (tag, r) != ("simple_tag", "dense_4warp_ragged")])
 def test_seeded_worlds_vs_oracle(tag, n):
     from oracle import Oracle
     from multiagent_particle_envs_b200 import _lib
     from helpers import device_sms, launch_shape, regime_size, step_uses_dense
     sms = device_sms()
-    if n == "dense_4warp_ragged":     # 4-warp blocks of the 80-register kernel + the general kernel's tail at begin > 0
-        n = regime_size("step", sms, 4)
-        assert step_uses_dense(tag, n, sms) and launch_shape("step", n, sms)[:3:2] == (4, True) and n % 32
+    if n == "1warp_ragged":           # 1-warp blocks of the 128-register HOT kernel + the general kernel's 17-world tail
+        n = regime_size("step", sms, 1, base=2048)
+        assert not step_uses_dense(tag, n, sms) and launch_shape("step", n, sms)[0] == 1 and n % 32 == 17
+    elif n in ("dense_2warp_ragged", "dense_4warp_ragged"):   # the 80-register kernel + the general kernel's tail
+        wpb = int(n[6])
+        n = regime_size("step", sms, wpb)
+        assert step_uses_dense(tag, n, sms) and launch_shape("step", n, sms)[:3:2] == (wpb, True) and n % 32
     elif n == 262144:                 # the BASELINE tag size: 80-register kernel, 2-warp blocks on 132 SMs (4 on 114)
         assert step_uses_dense(tag, n, sms) and launch_shape("step", n, sms)[0] == 2
     elif n == 131072:                 # the BASELINE spread N=6 size: 2-warp blocks (on 64 SMs or more)
@@ -190,7 +202,7 @@ def test_seeded_worlds_vs_oracle(tag, n):
         assert (np.abs(rpv[:, :, 2:4] - pv0[:, :, 2:4] * 0.75).max(axis=(1, 2)) > 1.0).mean() > floor
 
 
-@pytest.mark.parametrize("tag", TAGS)
+@pytest.mark.parametrize("tag", PROGRAM_TAGS)
 def test_fused_step_equals_three_kernel_path(tag):
     """mpe_step == mpe_set_action -> mpe_world_step -> mpe_observe, bit for bit"""
     from multiagent_particle_envs_b200 import _lib
@@ -343,7 +355,8 @@ sys.path.insert(0, %(root)r); sys.path.insert(0, %(root)r + "/tests")
 from helpers import make_product_env
 out = {}
 for tag, n in (("simple_spread_n3", 5003), ("simple_spread_n6", 2049), ("simple_tag", 4097), ("simple_world_comm", 3001),
-               ("simple_reference", 1000), ("simple_crypto", 999), ("simple_speaker_listener", 64), ("simple_push", 33)):
+               ("simple_reference", 1000), ("simple_crypto", 999), ("simple_speaker_listener", 64), ("simple_push", 33),
+               ("simple_spread_n4", 2081), ("simple_tag_2v1", 1055), ("simple_tag_4v2", 3093)):
     env = make_product_env(tag, num_envs=n, seed=21)
     env.reset()
     g = torch.Generator(device="cuda").manual_seed(4)
@@ -381,8 +394,8 @@ ALT_KERNELS = {
 @pytest.mark.parametrize("variant", list(ALT_KERNELS))
 def test_alternative_step_kernels_are_bit_identical(tmp_path, variant):
     """The default fused step runs whole tiles on the HOT specialisation and ragged tails on the general kernel.
-    MPE_B200_HOT=0 runs everything on the general kernel.  Three consecutive steps of eight scenarios with ragged batch
-    sizes must agree bit for bit."""
+    MPE_B200_HOT=0 runs everything on the general kernel.  Three consecutive steps of eleven programs (the four with an
+    80-register build among them) with ragged batch sizes must agree bit for bit."""
     import os
     import subprocess
     import sys
@@ -397,6 +410,6 @@ def test_alternative_step_kernels_are_bit_identical(tmp_path, variant):
             env.update(ALT_KERNELS[variant])
         subprocess.run([sys.executable, "-c", _ALT_SCRIPT % {"root": root}, path], check=True, env=env, timeout=900)
         res[mode] = dict(np.load(path))
-    assert set(res["0"]) == set(res["1"]) and len(res["0"]) >= 40
+    assert set(res["0"]) == set(res["1"]) and len(res["0"]) >= 55
     for k in res["0"]:
         assert np.array_equal(res["0"][k], res["1"][k]), k

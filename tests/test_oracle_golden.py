@@ -18,8 +18,9 @@ def goal_of(g):
     return g["goal"] if "goal" in g and g["goal"].shape[1] > 0 else None
 
 
-VARIANT_TAGS = ["simple_tag_1v1", "simple_tag_4v2", "simple_tag_6v2"]   # worlds the reference's callbacks support but its
-#                                                                           make_world hard-codes away (built test-side)
+# worlds the reference's callbacks support but its make_world hard-codes away (built test-side, oracle/refshim.py)
+VARIANT_TAGS = ["simple_tag_1v1", "simple_tag_4v2", "simple_tag_6v2", "simple_tag_2v1", "simple_spread_n2",
+                "simple_spread_n4", "simple_spread_n5", "simple_adversary_n4"]
 
 
 @pytest.mark.parametrize("tag", TAGS + ["simple_tag_force_discrete", "simple_tag_discrete_input"] + VARIANT_TAGS)
