@@ -338,6 +338,38 @@ MPE_API int mpe_rollout_policy_mappo_episodes(
     int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n,
     uint32_t net_flags, float ln_eps, uint8_t *done_dev, uint32_t flags, void *stream);
 
+/* MAPPO's recurrent actor (R_Actor with use_recurrent_policy, recurrent_N = 1), ONE weight set shared by every agent
+ * (share_policy), hidden width 64 only: x = MAPPO's base above without its last Linear, then
+ *     r = sigmoid(W_ir x + b_ir + W_hr h + b_hr),  z = sigmoid(W_iz x + b_iz + W_hz h + b_hz)
+ *     n = tanh(W_in x + b_in + r * (W_hn h + b_hn)),  h' = (1 - z) * n + z * h
+ *     logits = W3 LN(h') + b3
+ * w_ih, w_hh are torch.nn.GRU's weight_ih_l0, weight_hh_l0 ([192][64], rows r, z, n), b_ih, b_hh its biases [192].  The
+ * base folds as MAPPO's; the base's last LayerNorm is folded into w_ih, b_ih and the GRU's LayerNorm into w3, b3.
+ * Built for programs whose agents all have one observation and one action size (simple, simple_spread N = 2..6,
+ * simple_reference); others return MPE_ERR_UNSUPPORTED.  rnn_state_dev ([A][N][64] fp32, required) holds the hidden
+ * state: read at each agent's turn and overwritten with h', so it holds the state after the last step when the call
+ * ends.  The episode form starts every episode from h = 0 and never reads it.  rnn_state_record_dev ([T][A][N][64],
+ * or NULL) receives the h each step's actor consumed.  Everything else is mpe_rollout_policy_mappo[_episodes]'s,
+ * including the return codes and their order; a null weight counts as a null weight array. */
+MPE_API int mpe_rollout_policy_gru(mpe_handle h, void *agent_pv_dev, const void *lm_p_dev, float *comm_dev,
+                                   const int32_t *goal_dev, const float *w1, const float *b1, const float *w2,
+                                   const float *b2, const float *w_ih, const float *b_ih, const float *w_hh,
+                                   const float *b_hh, const float *w3, const float *b3, int32_t hidden, int32_t n_steps,
+                                   int32_t explore, uint64_t explore_seed, uint64_t explore_epoch, uint64_t world_offset,
+                                   float *const *obs_n_dev, float *rew_sum_dev, float *rew_steps_dev,
+                                   float *logp_steps_dev, int32_t *const *act_index_record_n, float *const *obs_record_n,
+                                   float *rnn_state_dev, float *rnn_state_record_dev, uint32_t net_flags, float ln_eps,
+                                   uint8_t *done_dev, uint32_t flags, void *stream);
+MPE_API int mpe_rollout_policy_gru_episodes(
+    mpe_handle h, void *agent_pv_dev, void *lm_p_dev, float *comm_dev, int32_t *goal_dev, const float *w1,
+    const float *b1, const float *w2, const float *b2, const float *w_ih, const float *b_ih, const float *w_hh,
+    const float *b_hh, const float *w3, const float *b3, int32_t hidden, int32_t episode_length, int32_t n_episodes,
+    int32_t explore, uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed, uint64_t reset_epoch,
+    uint64_t world_offset, float *const *obs_n_dev, float *ep_rew_dev, float *rew_steps_dev, float *logp_steps_dev,
+    int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n,
+    float *rnn_state_dev, float *rnn_state_record_dev, uint32_t net_flags, float ln_eps, uint8_t *done_dev,
+    uint32_t flags, void *stream);
+
 /* Same step for a caller that holds HOST buffers (what the reference's callers hold):
  * act_n_host[i] -> (async H2D into act_n_dev[i]) -> mpe_step -> (async D2H) obs_n_host[i],
  * rew_host, done_host, all ordered on `stream`.  Host buffers should be pinned for the copies

@@ -895,6 +895,31 @@ struct MlpMappoEpisodeArgs {
 };
 static_assert(sizeof(MlpMappoEpisodeArgs) <= 4096, "kernel parameter space");
 
+// MAPPO's recurrent actor (rMAPPO's R_Actor: MLPBase -> RNNLayer -> categorical ACTLayer, recurrent_N = 1), one weight
+// set shared by every agent (share_policy), categorical form only, H = 64:
+//     [LN(obs_dim)] -> Linear(obs_dim, 64) -> act -> LN(64) -> Linear(64, 64) -> act -> LN(64) = x
+//     h' = GRU(x, h) (torch's gate order r, z, n) -> LN(64) -> Linear(64, act_dim)
+// The base's LayerNorms fold as MAPPO's do; the base's last LayerNorm folds into W_ih, b_ih and the GRU's LayerNorm into
+// the head.  w1..b3 of MlpPolicyArgs hold the base and the head (every agent's pointer the same); the GRU's weights
+// (torch layout, W [192][64], b [192]) and the hidden state live here.  h is [A][n][64]: read at every agent's turn,
+// written back with h' (the state after the last step when the kernel ends), except that in the episode form every
+// episode starts from h = 0 (MAPPO's mask after done).  h_rec ([T][A][n][64] or null) receives the h each step's
+// actor consumed.
+struct MlpGruState {
+    const float *w_ih, *b_ih, *w_hh, *b_hh;
+    float *h;
+    float *h_rec;
+};
+struct MlpGruArgs {
+    MlpMappoArgs m;
+    MlpGruState g;
+};
+struct MlpGruEpisodeArgs {
+    MlpMappoEpisodeArgs m;
+    MlpGruState g;
+};
+static_assert(sizeof(MlpGruEpisodeArgs) <= 4096, "kernel parameter space");
+
 template <class P, int H>
 struct MlpShape {
     static constexpr int NT = H / 8;                                   // n-tiles of a hidden layer (= its k-tiles)
@@ -980,6 +1005,57 @@ static_assert(MlpShape<Spread<6>, 64>::kWeightFloats * 4 == 175296 && MlpShape<S
 static_assert(MlpShape<Tag<6, 2, 3>, 64>::kWeightFloats * 4 == 217344 && MlpShape<Tag<6, 2, 3>, 64>::kWarpFloats * 4 == 4992 &&
               mlp_smem_warps<Tag<6, 2, 3>, 64>() == 3, "tag 6+2, H = 64: 217 344 + 3 x 4992 = 232 320 B");
 
+// The recurrent actor (MlpGruArgs) is built for the programs whose agents all observe and act alike, which one shared
+// policy needs: simple, simple_spread N = 2..6 and simple_reference.
+template <class P> struct GruBuilt { static constexpr bool value = false; };
+template <> struct GruBuilt<Simple<1, 1>> { static constexpr bool value = true; };
+template <> struct GruBuilt<Spread<2>> { static constexpr bool value = true; };
+template <> struct GruBuilt<Spread<3>> { static constexpr bool value = true; };
+template <> struct GruBuilt<Spread<4>> { static constexpr bool value = true; };
+template <> struct GruBuilt<Spread<5>> { static constexpr bool value = true; };
+template <> struct GruBuilt<Spread<6>> { static constexpr bool value = true; };
+template <> struct GruBuilt<Reference> { static constexpr bool value = true; };
+
+// One weight set in shared memory, in floats: B fragments [k-tile][n-tile][lane][2] of W1, W2, W_ih (24 n-tiles: r, z,
+// n), W_hh, the head W3, then b1 [64], b2 [64], b_ih [192], b_hh [192], b3 [NOUT].  Per warp the MLP actor's
+// observation and logit tiles: h and h' stay in registers (one m-tile at a time, see mlp_agent).
+template <class P>
+struct GruShape {
+    using M = MlpShape<P, 64>;
+    static constexpr bool shared_ok() {
+        for (int i = 1; i < P::A; ++i)
+            if (P::obs_dim(i) != P::obs_dim(0) || P::act_dim(i) != P::act_dim(0)) return false;
+        return true;
+    }
+    static_assert(shared_ok(), "one shared policy: every agent observes and acts alike");
+    static constexpr int NT = 8, NG = 24;
+    static constexpr int w2_off = 64 * M::kt1(0) * NT;
+    static constexpr int wih_off = w2_off + 64 * NT * NT;
+    static constexpr int whh_off = wih_off + 64 * NT * NG;
+    static constexpr int w3_off = whh_off + 64 * NT * NG;
+    static constexpr int b1_off = w3_off + 64 * NT * (M::nout(0) / 8);
+    static constexpr int b2_off = b1_off + 64;
+    static constexpr int bih_off = b2_off + 64;
+    static constexpr int bhh_off = bih_off + 192;
+    static constexpr int b3_off = bhh_off + 192;
+    static constexpr int kWeightFloats = b3_off + M::nout(0);
+    static constexpr int kWarpFloats = M::kWarpFloats;
+};
+static_assert(GruShape<Simple<1, 1>>::kWeightFloats * 4 == 120864, "simple: 120 864 B of weights");
+static_assert(GruShape<Spread<3>>::kWeightFloats * 4 == 124960, "spread N=3: 124 960 B");
+static_assert(GruShape<Reference>::kWeightFloats * 4 == 127040, "simple_reference: 127 040 B");
+static_assert(GruShape<Spread<6>>::kWeightFloats * 4 == 129056, "spread N=6: 129 056 B");
+// Warps per block, both forms and every program: 8, which leaves 255 registers per thread -- x, h (TF32) and h' of one
+// m-tile are 96 of them next to 16 gate accumulators, the world state and the logits (ptxas -v: no stack, 164-252
+// registers).  One block per SM: the weights take more than half of its shared memory.
+constexpr int kGruWarps = 8;
+template <class P>
+__host__ __device__ constexpr int gru_block_warps() {
+    static_assert((GruShape<P>::kWeightFloats + kGruWarps * GruShape<P>::kWarpFloats) * 4 <= kMlpSmemBytes,
+                  "8 warps' tiles fit next to the weights");
+    return kGruWarps;
+}
+
 __device__ __forceinline__ uint32_t to_tf32(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -1020,9 +1096,11 @@ __device__ __forceinline__ void relu_tf32_frag(uint32_t (&a)[4], const float (&c
 // the 4 lanes of a quad (rows g: elements 0, 1; g + 8: 2, 3), so its sums are a local sum and __shfl_xor over 1 and 2.
 // Two-pass fp32 statistics as torch takes them: mu = sum(x) / H, then var = sum((x - mu)^2) / H; the normalised value
 // (x - mu) * rsqrt(var + eps) is rounded to TF32 only then.
+// The LayerNorm alone (norm_tf32_frags) also normalises the recurrent actor's h'.
+template <int NT>
+__device__ __forceinline__ void norm_tf32_frags(uint32_t (&a)[NT][4], const float (&c)[NT][4], float eps);
 template <int NT>
 __device__ __forceinline__ void act_norm_tf32_frags(uint32_t (&a)[NT][4], float (&c)[NT][4], bool tanh_act, float eps) {
-    constexpr float kInvH = 1.0f / (NT * 8);      // H = 8 NT, a power of two: exact
     if (tanh_act) {
 #pragma unroll
         for (int nt = 0; nt < NT; ++nt)
@@ -1034,6 +1112,11 @@ __device__ __forceinline__ void act_norm_tf32_frags(uint32_t (&a)[NT][4], float 
 #pragma unroll
             for (int j = 0; j < 4; ++j) c[nt][j] = fmaxf(c[nt][j], 0.0f);
     }
+    norm_tf32_frags<NT>(a, c, eps);
+}
+template <int NT>
+__device__ __forceinline__ void norm_tf32_frags(uint32_t (&a)[NT][4], const float (&c)[NT][4], float eps) {
+    constexpr float kInvH = 1.0f / (NT * 8);      // H = 8 NT, a power of two: exact
     float s0 = 0.0f, s1 = 0.0f;
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) { s0 += c[nt][0] + c[nt][1]; s1 += c[nt][2] + c[nt][3]; }
@@ -1105,14 +1188,30 @@ __device__ __forceinline__ float categorical_segment(const float (&zs)[N], const
 // kMappoFeatureNorm) normalises each lane's tile row in place; act_norm_tf32_frags replaces relu_tf32_frag; and since
 // the second LayerNorm needs a whole row of h2, layers 2 and 3 run one m-tile at a time (h2 of 16 rows in 32 fp32
 // registers, W2's B fragments read once per m-tile).
-template <class P, int H, int I, bool EPISODES = false, bool CATEGORICAL = false, bool MAPPO = false>
+// GRU adds MAPPO's recurrent actor (MlpGruArgs) to MAPPO's: per m-tile the base's two layers, the GRU step, the
+// LayerNorm of h' and the head, so that x, h and h' fit in registers.  The weights are the one shared set (GruShape).
+//
+// Where the base's second layer, the head and their biases sit in Wsm: the agent's block (MlpShape), or the shared set
+template <class P, int H, int I, bool GRU>
+struct AgentWeights {
+    using S = MlpShape<P, H>;
+    static constexpr int w2 = S::w2_off(I), w3 = S::w3_off(I), b1 = S::b1_off(I), b2 = S::b2_off(I), b3 = S::b3_off(I);
+};
+template <class P, int I>
+struct AgentWeights<P, 64, I, true> {
+    using G = GruShape<P>;
+    static constexpr int w2 = G::w2_off, w3 = G::w3_off, b1 = G::b1_off, b2 = G::b2_off, b3 = G::b3_off;
+};
+template <class P, int H, int I, bool EPISODES = false, bool CATEGORICAL = false, bool MAPPO = false, bool GRU = false>
 __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typename P::W &w, const float *__restrict__ Wsm,
                                             float *s_warp, int lane, int t, int rows, bool active, int64_t w0, int64_t wi,
                                             float *cact, int step = 0, uint64_t epoch = 0,
                                             const MlpCategoricalRecords *cr = nullptr, float ln_eps = 0.0f,
-                                            uint32_t net_flags = 0) {
+                                            uint32_t net_flags = 0, const MlpGruState *gs = nullptr) {
     static_assert(!MAPPO || (CATEGORICAL && H == 64), "the MAPPO actor: categorical form, H = 64");
+    static_assert(!GRU || MAPPO, "the recurrent actor is MAPPO's");
     using S = MlpShape<P, H>;
+    using O = AgentWeights<P, H, I, GRU>;
     constexpr int OD = P::obs_dim(I), KT1 = S::kt1(I), NT = S::NT, PITCH = ObsTile<OD>::kPitch;
     constexpr int AD = P::act_dim(I), NO = S::nout(I) / 8;
     constexpr int MOVE = P::movable(I) ? 5 : 0, COMM = I < P::NS ? P::DIMC : 0;   // sub-spaces, speakers come first
@@ -1148,7 +1247,7 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
     const int gq = lane >> 2, tq = lane & 3;
     // ---- layer 1: [32 x K1] . [K1 x H] + b1 ----
     float h[2][NT][4];
-    const float *B1 = Wsm + S::b1_off(I);
+    const float *B1 = Wsm + O::b1;
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
         const float2 b = *reinterpret_cast<const float2 *>(B1 + nt * 8 + 2 * tq);
@@ -1178,7 +1277,9 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
         }
     }
     uint32_t x1[2][NT][4];
-    if constexpr (MAPPO) {
+    if constexpr (GRU) {
+        // the recurrent actor runs layer 1 again one m-tile at a time (below): h above is dead code for it
+    } else if constexpr (MAPPO) {
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt) act_norm_tf32_frags<NT>(x1[mt], h[mt], net_flags & kMappoTanh, ln_eps);
     } else {
@@ -1188,7 +1289,7 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
             for (int nt = 0; nt < NT; ++nt) relu_tf32_frag(x1[mt][nt], h[mt][nt]);
     }
     // ---- layers 2 and 3, one 8-unit tile of h2 at a time: logits += relu(x1 . W2^T[:, tile] + b2[tile]) . W3^T[tile, :]
-    const float *W2 = Wsm + S::w2_off(I), *W3 = Wsm + S::w3_off(I), *B2 = Wsm + S::b2_off(I), *B3 = Wsm + S::b3_off(I);
+    const float *W2 = Wsm + O::w2, *W3 = Wsm + O::w3, *B2 = Wsm + O::b2, *B3 = Wsm + O::b3;
     float lg[2][NO][4];
 #pragma unroll
     for (int ot = 0; ot < NO; ++ot) {
@@ -1196,7 +1297,118 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt) { lg[mt][ot][0] = b.x; lg[mt][ot][1] = b.y; lg[mt][ot][2] = b.x; lg[mt][ot][3] = b.y; }
     }
-    if constexpr (MAPPO) {   // ---- MAPPO: per m-tile, h2 = x1 . W2^T + b2 whole, act + LayerNorm, then logits += x2 . W3^T
+    if constexpr (GRU) {   // ---- the recurrent actor, one m-tile (16 worlds) at a time: layers 1 and 2 with their
+                           //      LayerNorms -> x, h' = GRU(x, h), logits += LN(h') . W3^T
+        using G = GruShape<P>;
+        const float *Wih = Wsm + G::wih_off, *Whh = Wsm + G::whh_off, *Bih = Wsm + G::bih_off, *Bhh = Wsm + G::bhh_off;
+        const bool h_zero = EPISODES && step == 0;         // every episode starts from h = 0
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+            uint32_t x[NT][4];
+            {
+                float c[NT][4];
+#pragma unroll
+                for (int nt = 0; nt < NT; ++nt) {
+                    const float2 b = *reinterpret_cast<const float2 *>(B1 + nt * 8 + 2 * tq);
+                    c[nt][0] = b.x; c[nt][1] = b.y; c[nt][2] = b.x; c[nt][3] = b.y;
+                }
+#pragma unroll
+                for (int kt = 0; kt < KT1; ++kt) {
+                    uint32_t a[4];
+                    const int c0 = kt * 8 + tq, c1 = c0 + 4;
+                    const float *r0 = tile + (mt * 16 + gq) * PITCH, *r1 = r0 + 8 * PITCH;
+                    a[0] = to_tf32(c0 < OD ? r0[c0] : 0.0f); a[1] = to_tf32(c0 < OD ? r1[c0] : 0.0f);
+                    a[2] = to_tf32(c1 < OD ? r0[c1] : 0.0f); a[3] = to_tf32(c1 < OD ? r1[c1] : 0.0f);
+#pragma unroll
+                    for (int nt = 0; nt < NT; ++nt)
+                        mma_tf32(c[nt], a, *reinterpret_cast<const float2 *>(Wsm + ((kt * NT + nt) * 32 + lane) * 2));
+                }
+                uint32_t xa[NT][4];
+                act_norm_tf32_frags<NT>(xa, c, net_flags & kMappoTanh, ln_eps);
+#pragma unroll
+                for (int nt = 0; nt < NT; ++nt) {
+                    const float2 bb = *reinterpret_cast<const float2 *>(B2 + nt * 8 + 2 * tq);
+                    c[nt][0] = bb.x; c[nt][1] = bb.y; c[nt][2] = bb.x; c[nt][3] = bb.y;
+#pragma unroll
+                    for (int kt = 0; kt < NT; ++kt)
+                        mma_tf32(c[nt], xa[kt], *reinterpret_cast<const float2 *>(W2 + ((kt * NT + nt) * 32 + lane) * 2));
+                }
+                act_norm_tf32_frags<NT>(x, c, net_flags & kMappoTanh, ln_eps);
+            }
+            // this lane's rows g and g + 8 of the m-tile in the accumulator layout (units nt * 8 + 2 tq, + 1): a quad
+            // reads and writes whole 32-byte sectors.  Idle rows replay world w0 and store nothing.
+            const int ra = mt * 16 + gq, rb = ra + 8;
+            const int64_t wa = w0 + (ra < rows ? ra : 0), wb = w0 + (rb < rows ? rb : 0);
+            float *ha = gs->h + (static_cast<int64_t>(I) * n + wa) * 64 + 2 * tq;
+            float *hb = gs->h + (static_cast<int64_t>(I) * n + wb) * 64 + 2 * tq;
+            // h as W_hh's A operand, TF32: the accumulator layout is relu_tf32_frag's permuted A layout
+            uint32_t ht[NT][4];
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+                const float2 va = h_zero ? make_float2(0.0f, 0.0f) : *reinterpret_cast<const float2 *>(ha + nt * 8);
+                const float2 vb = h_zero ? make_float2(0.0f, 0.0f) : *reinterpret_cast<const float2 *>(hb + nt * 8);
+                if (gs->h_rec != nullptr) {                // the h this step's actor consumes
+                    float *qa = gs->h_rec + ((static_cast<int64_t>(t) * P::A + I) * n + wa) * 64 + 2 * tq;
+                    float *qb = gs->h_rec + ((static_cast<int64_t>(t) * P::A + I) * n + wb) * 64 + 2 * tq;
+                    if (ra < rows) *reinterpret_cast<float2 *>(qa + nt * 8) = va;
+                    if (rb < rows) *reinterpret_cast<float2 *>(qb + nt * 8) = vb;
+                }
+                ht[nt][0] = to_tf32(va.x); ht[nt][1] = to_tf32(vb.x); ht[nt][2] = to_tf32(va.y); ht[nt][3] = to_tf32(vb.y);
+            }
+            // h' for units j * 8 .. j * 8 + 7: r and z each accumulate both GEMMs and both biases, n keeps W_in x + b_in
+            // and W_hn h + b_hn apart.  The update reads the unrounded h of those units again (L1) rather than holding
+            // all of it next to its TF32 copy.
+            float hn[NT][4];
+#pragma unroll
+            for (int j = 0; j < NT; ++j) {
+                float r[4], z[4], ni[4], nh[4];
+                {
+                    const float2 bir = *reinterpret_cast<const float2 *>(Bih + j * 8 + 2 * tq);
+                    const float2 bhr = *reinterpret_cast<const float2 *>(Bhh + j * 8 + 2 * tq);
+                    const float2 biz = *reinterpret_cast<const float2 *>(Bih + 64 + j * 8 + 2 * tq);
+                    const float2 bhz = *reinterpret_cast<const float2 *>(Bhh + 64 + j * 8 + 2 * tq);
+                    const float2 bin = *reinterpret_cast<const float2 *>(Bih + 128 + j * 8 + 2 * tq);
+                    const float2 bhn = *reinterpret_cast<const float2 *>(Bhh + 128 + j * 8 + 2 * tq);
+                    r[0] = r[2] = bir.x + bhr.x; r[1] = r[3] = bir.y + bhr.y;
+                    z[0] = z[2] = biz.x + bhz.x; z[1] = z[3] = biz.y + bhz.y;
+                    ni[0] = ni[2] = bin.x; ni[1] = ni[3] = bin.y;
+                    nh[0] = nh[2] = bhn.x; nh[1] = nh[3] = bhn.y;
+                }
+#pragma unroll
+                for (int kt = 0; kt < NT; ++kt) {
+                    const float *bi = Wih + ((kt * G::NG + j) * 32 + lane) * 2, *bh = Whh + ((kt * G::NG + j) * 32 + lane) * 2;
+                    mma_tf32(r, x[kt], *reinterpret_cast<const float2 *>(bi));
+                    mma_tf32(r, ht[kt], *reinterpret_cast<const float2 *>(bh));
+                    mma_tf32(z, x[kt], *reinterpret_cast<const float2 *>(bi + NT * 64));
+                    mma_tf32(z, ht[kt], *reinterpret_cast<const float2 *>(bh + NT * 64));
+                    mma_tf32(ni, x[kt], *reinterpret_cast<const float2 *>(bi + 2 * NT * 64));
+                    mma_tf32(nh, ht[kt], *reinterpret_cast<const float2 *>(bh + 2 * NT * 64));
+                }
+                const float2 va = h_zero ? make_float2(0.0f, 0.0f) : *reinterpret_cast<const float2 *>(ha + j * 8);
+                const float2 vb = h_zero ? make_float2(0.0f, 0.0f) : *reinterpret_cast<const float2 *>(hb + j * 8);
+                const float hf[4] = {va.x, va.y, vb.x, vb.y};
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const float rg = 1.0f / (1.0f + expf(-r[e])), zg = 1.0f / (1.0f + expf(-z[e]));
+                    const float ng = tanhf(ni[e] + rg * nh[e]);
+                    hn[j][e] = (1.0f - zg) * ng + zg * hf[e];
+                }
+            }
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+                if (ra < rows) *reinterpret_cast<float2 *>(ha + nt * 8) = make_float2(hn[nt][0], hn[nt][1]);
+                if (rb < rows) *reinterpret_cast<float2 *>(hb + nt * 8) = make_float2(hn[nt][2], hn[nt][3]);
+            }
+            uint32_t xh[NT][4];
+            norm_tf32_frags<NT>(xh, hn, ln_eps);
+#pragma unroll
+            for (int ot = 0; ot < NO; ++ot)
+#pragma unroll
+                for (int kt = 0; kt < NT; ++kt)
+                    mma_tf32(lg[mt][ot], xh[kt], *reinterpret_cast<const float2 *>(W3 + ((kt * NO + ot) * 32 + lane) * 2));
+            __syncwarp();   // as in MAPPO's branch: the second m-tile reads its B fragments again
+        }
+    } else if constexpr (MAPPO) {   // ---- MAPPO: per m-tile, h2 = x1 . W2^T + b2 whole, act + LayerNorm, then logits += x2 . W3^T
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt) {
             float c[NT][4];
@@ -1321,19 +1533,44 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
 }
 
 // the body of both forms; ea is null in the single-episode form (EPISODES = false), cr unless CATEGORICAL; ln_eps and
-// net_flags are MAPPO's (MlpMappoArgs)
-template <class P, int H, bool EPISODES, bool CATEGORICAL = false, bool MAPPO = false>
+// net_flags are MAPPO's (MlpMappoArgs), gs the recurrent actor's (GRU, MlpGruArgs)
+template <class P, int H, bool EPISODES, bool CATEGORICAL = false, bool MAPPO = false, bool GRU = false>
 __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEpisodeArgs *ea,
                                             const MlpCategoricalRecords *cr = nullptr, float ln_eps = 0.0f,
-                                            uint32_t net_flags = 0) {
+                                            uint32_t net_flags = 0, const MlpGruState *gs = nullptr) {
     static_assert(H == 32 || H == 64, "MLP policy rollout: hidden width 32 or 64");
     constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     using S = MlpShape<P, H>;
-    constexpr int kWarps = mlp_block_warps<P, H, EPISODES | (MAPPO ? 2 : CATEGORICAL) << 1>();
-    static_assert(kWarps >= 1 && (S::kWeightFloats + kWarps * S::kWarpFloats) * 4 <= kMlpSmemBytes, "one block fits an SM");
+    constexpr int kWarps = [] {
+        if constexpr (GRU) return gru_block_warps<P>();
+        else return mlp_block_warps<P, H, EPISODES | (MAPPO ? 2 : CATEGORICAL) << 1>();
+    }();
+    constexpr int kWeightFloats = [] {
+        if constexpr (GRU) return GruShape<P>::kWeightFloats;
+        else return S::kWeightFloats;
+    }();
+    static_assert(kWarps >= 1 && (kWeightFloats + kWarps * S::kWarpFloats) * 4 <= kMlpSmemBytes, "one block fits an SM");
     const StepArgs &a = pa.s;
     extern __shared__ __align__(16) float smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if constexpr (GRU) {   // ---- the one shared weight set -> TF32 B fragments in shared memory, once per block ----
+        using G = GruShape<P>;
+        constexpr int OD = P::obs_dim(0), AD = P::act_dim(0);
+        stage_fragments<S::kt1(0), G::NT, false>(smem, pa.w1[0], 64, OD);
+        stage_fragments<G::NT, G::NT, true>(smem + G::w2_off, pa.w2[0], 64, 64);
+        stage_fragments<G::NT, G::NG, true>(smem + G::wih_off, gs->w_ih, 192, 64);
+        stage_fragments<G::NT, G::NG, true>(smem + G::whh_off, gs->w_hh, 192, 64);
+        stage_fragments<G::NT, S::nout(0) / 8, true>(smem + G::w3_off, pa.w3[0], AD, 64);
+        for (int q = threadIdx.x; q < 64; q += blockDim.x) {
+            smem[G::b1_off + q] = pa.b1[0][q];
+            smem[G::b2_off + q] = pa.b2[0][q];
+        }
+        for (int q = threadIdx.x; q < 192; q += blockDim.x) {
+            smem[G::bih_off + q] = gs->b_ih[q];
+            smem[G::bhh_off + q] = gs->b_hh[q];
+        }
+        for (int q = threadIdx.x; q < S::nout(0); q += blockDim.x) smem[G::b3_off + q] = q < AD ? pa.b3[0][q] : 0.0f;
+    } else {
     // ---- all agents' weights -> TF32 B fragments in shared memory, once per block ----
     static_for<A>([&](auto ic) {
         constexpr int i = decltype(ic)::value;
@@ -1348,6 +1585,7 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
         }
         for (int q = threadIdx.x; q < S::nout(i); q += blockDim.x) base[S::b3_off(i) + q] = q < P::act_dim(i) ? pa.b3[i][q] : 0.0f;
     });
+    }
     __syncthreads();
 
     const int64_t n = a.n;
@@ -1357,7 +1595,7 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
     const int rows = (end - w0) < 32 ? static_cast<int>(end - w0) : 32;
     const bool active = lane < rows;
     const int64_t wi = w0 + (active ? lane : 0);   // idle lanes of a partial tile replay world w0: every tile row is finite
-    float *s_warp = smem + S::kWeightFloats + warp * S::kWarpFloats;
+    float *s_warp = smem + kWeightFloats + warp * S::kWarpFloats;
     const DevDesc &d = a.d;
 
     typename P::W w;
@@ -1393,9 +1631,9 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
             P::prepare(d, w);
             static_for<A>([&](auto ic) {
                 constexpr int i = decltype(ic)::value;
-                const float2 u = mlp_agent<P, H, i, EPISODES, CATEGORICAL, MAPPO>(pa, w, smem + S::agent_off(i), s_warp, lane,
-                                                                                  tg, rows, active, w0, wi, cact, t,
-                                                                                  pa.epoch + e, cr, ln_eps, net_flags);
+                const float2 u = mlp_agent<P, H, i, EPISODES, CATEGORICAL, MAPPO, GRU>(
+                    pa, w, GRU ? smem : smem + S::agent_off(i), s_warp, lane, tg, rows, active, w0, wi, cact, t,
+                    pa.epoch + e, cr, ln_eps, net_flags, gs);
                 ux[i] = u.x;
                 uy[i] = u.y;
             });
@@ -1509,6 +1747,26 @@ __global__ void __launch_bounds__(mlp_block_warps<P, 64, 5>() * 32)
     mlp_rollout<P, 64, true, true, true>(ma.c.e.p, &ma.c.e, &ma.c.c, ma.eps, ma.net_flags);
 }
 
+template <class P>
+__global__ void __launch_bounds__(gru_block_warps<P>() * 32) mpe_policy_gru_kernel(const __grid_constant__ MlpGruArgs ga) {
+    mlp_rollout<P, 64, false, true, true, true>(ga.m.c.p, nullptr, &ga.m.c.c, ga.m.eps, ga.m.net_flags, &ga.g);
+}
+
+template <class P>
+__global__ void __launch_bounds__(gru_block_warps<P>() * 32)
+    mpe_policy_gru_episode_kernel(const __grid_constant__ MlpGruEpisodeArgs ga) {
+    mlp_rollout<P, 64, true, true, true, true>(ga.m.c.e.p, &ga.m.c.e, &ga.m.c.c, ga.m.eps, ga.m.net_flags, &ga.g);
+}
+
+// The recurrent actor's two kernels of program P (episodes = 0, 1).  mpe_gru.cu defines it and so instantiates the 14
+// kernels in a translation unit of their own, which the Makefile compiles alongside this one: in one unit the library
+// took half as long again to build.
+template <class P>
+const void *gru_kernel(int episodes);
+
+#ifdef MPE_KERNEL_TEMPLATES_ONLY   // mpe_gru.cu: the device code above, without the programs and the C ABI below
+}  // namespace mpe
+#else
 // ---- generic program for user scenarios (MPE_SCN_CUSTOM) ------------------------------------------
 // Any entity table, flags read at run time; same arithmetic primitives and the same (a, b) pair order as
 // the compiled programs, so for a table that matches a built-in scenario the state is bit-identical.
@@ -1692,9 +1950,10 @@ struct Program {
     void (*policy_fn[2])(PolicyArgs);  // K-step closed-loop rollout, hidden width 32 / 64 (null: not built for this program)
     int policy_weight_floats[2];
     // the same with the two-hidden-layer actor on the tensor cores, by form (episodes | kind << 1) and H = 32 / 64: the
-    // kernel and its warps per block at most (mlp_block_warps); null for MAPPO's forms at H = 32
-    struct { const void *fn; int warps; } mlp[kMlpForms][2];
-    int mlp_weight_floats[2], mlp_warp_floats[2];
+    // kernel and its warps per block at most (mlp_block_warps); null for MAPPO's forms at H = 32.  Forms 6 and 7 are
+    // the recurrent actor's (gru_block_warps, H = 64 only), whose one shared weight set takes gru_weight_floats.
+    struct { const void *fn; int warps; } mlp[kMlpForms + 2][2];
+    int mlp_weight_floats[2], mlp_warp_floats[2], gru_weight_floats;
     int mlp_explore_stride;           // Philox blocks per (step, agent) of its exploration noise
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
     int rollout_smem;   // dynamic shared memory per WARP of the rollout kernel
@@ -1741,6 +2000,12 @@ static Program make_program() {
         set_mlp<P, 32>(p, 0);
         set_mlp<P, 64>(p, 1);
         p.mlp_explore_stride = mlp_explore_stride<P>();
+    }
+    if constexpr (GruBuilt<P>::value) {
+        static_assert(MlpBuilt<P>::value, "the recurrent actor shares the MLP actor's tiles and exploration stride");
+        p.mlp[kMlpForms][1] = {gru_kernel<P>(0), gru_block_warps<P>()};
+        p.mlp[kMlpForms + 1][1] = {gru_kernel<P>(1), gru_block_warps<P>()};
+        p.gru_weight_floats = GruShape<P>::kWeightFloats;
     }
     p.smem_bytes = Shape<P>::kWarpBytes;  // per warp
     p.A = P::A; p.L = P::L; p.NS = P::NS; p.DIMC = P::DIMC; p.INFO = P::INFO; p.G = P::G;
@@ -1872,11 +2137,12 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
             if (prog->policy_fn[k])
                 CUDA_TRY(cudaFuncSetAttribute(prog->policy_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               prog->policy_weight_floats[k] * 4 + prog->smem_bytes * 4));
-        for (int f = 0; f < kMlpForms; ++f)
+        for (int f = 0; f < kMlpForms + 2; ++f)   // and the recurrent actor's two, whose weights are gru_weight_floats
             for (int k = 0; k < 2; ++k)
                 if (prog->mlp[f][k].fn)
                     CUDA_TRY(cudaFuncSetAttribute(prog->mlp[f][k].fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                  (prog->mlp_weight_floats[k] + prog->mlp_warp_floats[k] * prog->mlp[f][k].warps) * 4));
+                                                  ((f < kMlpForms ? prog->mlp_weight_floats[k] : prog->gru_weight_floats) +
+                                                   prog->mlp_warp_floats[k] * prog->mlp[f][k].warps) * 4));
         if (prog->rollout_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->rollout_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->rollout_smem * max_warps_per_block(prog->rollout_smem)));
@@ -2232,9 +2498,11 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
 
 // The arguments of the six two-hidden-layer rollout entry points, filled by name (several neighbours share a type).
 // form: episodes | kind << 1 (kMlpForms).  T is the episode length (n_steps in the single-episode forms); a record the
-// form does not have is null.  net_flags and ln_eps are MAPPO's (MlpMappoArgs).
+// form does not have is null.  net_flags and ln_eps are MAPPO's (MlpMappoArgs); forms 6 and 7 (kMlpForms + episodes)
+// are the recurrent actor's, whose w[j] hold the shared set's pointer for every agent and gru its MlpGruState.
 struct MlpCall {
     int form;
+    MlpGruState gru;
     uint32_t net_flags;
     float ln_eps;
     void *pv;
@@ -2255,14 +2523,16 @@ struct MlpCall {
 };
 
 static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
-    static const char *const kName[kMlpForms][2] = {   // the NVTX range, the launch's error context
+    static const char *const kName[kMlpForms + 2][2] = {   // the NVTX range, the launch's error context
         {"mpe_rollout_policy_mlp", "cudaLaunchKernelExC(rollout_policy_mlp)"},
         {"mpe_rollout_policy_mlp_episodes", "cudaLaunchKernelExC(rollout_policy_mlp_episodes)"},
         {"mpe_rollout_policy_mlp_categorical", "cudaLaunchKernelExC(rollout_policy_mlp_categorical)"},
         {"mpe_rollout_policy_mlp_categorical_episodes", "cudaLaunchKernelExC(rollout_policy_mlp_categorical_episodes)"},
         {"mpe_rollout_policy_mappo", "cudaLaunchKernelExC(rollout_policy_mappo)"},
-        {"mpe_rollout_policy_mappo_episodes", "cudaLaunchKernelExC(rollout_policy_mappo_episodes)"}};
-    const bool episodes = c.form & 1, categorical = c.form >= 2, mappo = c.form >= 4;
+        {"mpe_rollout_policy_mappo_episodes", "cudaLaunchKernelExC(rollout_policy_mappo_episodes)"},
+        {"mpe_rollout_policy_gru", "cudaLaunchKernelExC(rollout_policy_gru)"},
+        {"mpe_rollout_policy_gru_episodes", "cudaLaunchKernelExC(rollout_policy_gru_episodes)"}};
+    const bool episodes = c.form & 1, categorical = c.form >= 2, mappo = c.form >= 4, gru = c.form >= kMlpForms;
     const bool no_weights = !c.w[0] || !c.w[1] || !c.w[2] || !c.w[3] || !c.w[4] || !c.w[5];
     // the single-episode forms refuse a negative n_steps and null weight arrays before anything else, the episode forms
     // after the device, program and length checks
@@ -2281,6 +2551,9 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     if (c.explore && static_cast<int64_t>(c.T) * h->prog->A * h->prog->mlp_explore_stride > static_cast<int64_t>(kExploreTag))
         return MPE_ERR_BAD_ARG;
     if (no_weights || (c.rew_steps != nullptr && !ok4(c.rew_steps))) return MPE_ERR_BAD_ARG;
+    if (gru && (!ok4(c.gru.w_ih) || !ok4(c.gru.b_ih) || !ok4(c.gru.w_hh) || !ok4(c.gru.b_hh) || !ok8(c.gru.h) ||
+                (c.gru.h_rec != nullptr && !ok8(c.gru.h_rec))))
+        return MPE_ERR_BAD_ARG;
     NvtxRange range(kName[c.form][0]);
     MlpCategoricalRecords cr{};
     if (categorical) {
@@ -2321,7 +2594,9 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     MlpCategoricalEpisodeArgs cea{ea, cr};
     MlpMappoArgs ma{ca, c.ln_eps, c.net_flags};
     MlpMappoEpisodeArgs mea{cea, c.ln_eps, c.net_flags};
-    void *const form_args[kMlpForms] = {&pa, &ea, &ca, &cea, &ma, &mea};
+    MlpGruArgs ga{ma, c.gru};
+    MlpGruEpisodeArgs gea{mea, c.gru};
+    void *const form_args[kMlpForms + 2] = {&pa, &ea, &ca, &cea, &ma, &mea, &ga, &gea};
     const void *const fn = h->prog->mlp[c.form][k].fn;
     const int cap = h->prog->mlp[c.form][k].warps;
     // every block stages all agents' weights once, so blocks are as large as possible while every SM still gets work
@@ -2329,7 +2604,8 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
     if (wpb > cap) wpb = cap;
-    return launch_persistent(h, fn, warps, wpb, static_cast<size_t>(h->prog->mlp_weight_floats[k]) * 4,
+    const int weight_floats = gru ? h->prog->gru_weight_floats : h->prog->mlp_weight_floats[k];
+    return launch_persistent(h, fn, warps, wpb, static_cast<size_t>(weight_floats) * 4,
                              static_cast<size_t>(h->prog->mlp_warp_floats[k]) * 4, form_args[c.form], c.stream,
                              kName[c.form][1]);
 }
@@ -2447,6 +2723,62 @@ extern "C" int mpe_rollout_policy_mappo_episodes(
     c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
     c.net_flags = net_flags; c.ln_eps = ln_eps;
     return rollout_policy_mlp(h, c);
+}
+
+// The recurrent actor's weight set (W1, b1, W2, b2, W_ih, b_ih, W_hh, b_hh, W3, b3) -> every agent's base and head
+// pointers and c.gru; a null weight leaves c.w null, which the launcher refuses as MAPPO's null weight arrays
+static int rollout_policy_gru(mpe_handle h, MlpCall &c, const float *const (&wt)[10], float *rnn_state,
+                              float *rnn_state_record) {
+    const float *per_agent[6][kMaxA];
+    bool all = true;
+    for (int j = 0; j < 10; ++j) all = all && wt[j] != nullptr;
+    static const int kBaseHead[6] = {0, 1, 2, 3, 8, 9};
+    for (int j = 0; j < 6; ++j) {
+        for (int i = 0; i < kMaxA; ++i) per_agent[j][i] = wt[kBaseHead[j]];
+        c.w[j] = all ? per_agent[j] : nullptr;
+    }
+    c.gru = MlpGruState{wt[4], wt[5], wt[6], wt[7], rnn_state, rnn_state_record};
+    return rollout_policy_mlp(h, c);
+}
+
+extern "C" int mpe_rollout_policy_gru(mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal,
+                                      const float *w1, const float *b1, const float *w2, const float *b2,
+                                      const float *w_ih, const float *b_ih, const float *w_hh, const float *b_hh,
+                                      const float *w3, const float *b3, int32_t hidden, int32_t n_steps, int32_t explore,
+                                      uint64_t explore_seed, uint64_t explore_epoch, uint64_t world_offset,
+                                      float *const *obs_n, float *rew_sum, float *rew_steps, float *logp_steps,
+                                      int32_t *const *act_index_record_n, float *const *obs_record_n, float *rnn_state,
+                                      float *rnn_state_record, uint32_t net_flags, float ln_eps, uint8_t *done,
+                                      uint32_t flags, void *stream) {
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = kMlpForms; c.T = n_steps; c.episodes = 1; c.rew = rew_sum;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    c.net_flags = net_flags; c.ln_eps = ln_eps;
+    return rollout_policy_gru(h, c, {w1, b1, w2, b2, w_ih, b_ih, w_hh, b_hh, w3, b3}, rnn_state, rnn_state_record);
+}
+
+extern "C" int mpe_rollout_policy_gru_episodes(
+    mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal, const float *w1, const float *b1, const float *w2,
+    const float *b2, const float *w_ih, const float *b_ih, const float *w_hh, const float *b_hh, const float *w3,
+    const float *b3, int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore, uint64_t explore_seed,
+    uint64_t explore_epoch, uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n,
+    float *ep_rew, float *rew_steps, float *logp_steps, int32_t *const *act_index_record_n, float *const *obs_record_n,
+    float *const *final_obs_record_n, float *rnn_state, float *rnn_state_record, uint32_t net_flags, float ln_eps,
+    uint8_t *done, uint32_t flags, void *stream) {
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = kMlpForms + 1; c.T = episode_length; c.episodes = n_episodes; c.rew = ep_rew;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
+    c.net_flags = net_flags; c.ln_eps = ln_eps;
+    return rollout_policy_gru(h, c, {w1, b1, w2, b2, w_ih, b_ih, w_hh, b_hh, w3, b3}, rnn_state, rnn_state_record);
 }
 
 // adjacent (dst, src, bytes) copies with equal small gaps on both sides are issued as one DMA
@@ -2660,3 +2992,4 @@ extern "C" const char *mpe_strerror(int err) {
 extern "C" const char *mpe_last_cuda_error(void) { return g_cuda_err; }
 extern "C" int mpe_abi_version(void) { return MPE_ABI_VERSION; }
 extern "C" int64_t mpe_kernel_launches(void) { return __atomic_load_n(&g_launches, __ATOMIC_RELAXED); }
+#endif  // MPE_KERNEL_TEMPLATES_ONLY

@@ -244,7 +244,8 @@ class MultiAgentEnv(_Env):
         return obs_n, reward_n, done_n, info_n
 
     def rollout_policy(self, policies, n_steps, record_actions=False, per_step_rewards=False, record_observations=False,
-                       explore_seed=None, episode_length=None, action_mode="softmax", record_log_probs=False):
+                       explore_seed=None, episode_length=None, action_mode="softmax", record_log_probs=False,
+                       rnn_states=None, record_rnn_states=False):
         """T closed-loop steps in ONE kernel launch with the actors inside the kernel.
 
         One hidden layer (mpe_rollout_policy, fp32): agent i acts with softmax(W2_i relu(W1_i obs_i + b1_i) + b2_i).
@@ -305,7 +306,22 @@ class MultiAgentEnv(_Env):
         next Linear (float64, then float32); the kernel normalises with fp32 statistics and TF32 GEMM operands.  Records,
         extras, sampling, log-probabilities and episodes are those of the categorical mode above; observation records and
         final observations hold the raw observations (before the input LayerNorm).  action_mode="softmax" and a hidden
-        width other than 64 raise NotImplementedError.  GRU actors are not supported."""
+        width other than 64 raise NotImplementedError.
+
+        MAPPO's recurrent actor (mpe_rollout_policy_gru, action_mode="categorical" only; rMAPPO with recurrent_N = 1 and
+        share_policy): policies is [actor] * n, ONE tuple (base, gru, norm, head) for every agent -- base the MAPPO
+        actor above without its last Linear, gru an nn.GRU(64, 64), norm a LayerNorm(64), head a Linear(64, act_dim);
+        rmappo_actor_params checks it (ValueError) and folds it.  Any policy tuple holding an nn.GRU takes this path;
+        distinct per-agent tuples raise NotImplementedError.  Built for simple, simple_spread N = 2..6 and
+        simple_reference (every other program raises MpeError before anything runs).  Per step the logits are
+        head(norm(h')), h' = gru(base(obs), h), h carried across steps.  rnn_states: the initial hidden state, a float32
+        CUDA tensor [n, N, 64] on the env's device, read and never written (None: zeros); it cannot be combined with
+        episode_length, whose episodes each start from h = 0 (MAPPO's mask after done).  extras["final_rnn_states"] is a
+        new [n, N, 64] tensor: h after the last step (of the last episode, before its reset), what the next call's
+        rnn_states continues from.  record_rnn_states=True returns extras["rnn_states"], a float32 [T, n, N, 64] tensor
+        of the h each step's actor consumed (MAPPO's buffer rnn_states[t]; zero at every episode's first step), else
+        None -- T * n * N * 256 bytes.  Records, sampling, log-probabilities, episodes and epochs are the categorical
+        mode's.  rnn_states or record_rnn_states with any other actor raise ValueError."""
         import torch
         world = self.world
         if action_mode not in ("softmax", "categorical"):
@@ -322,6 +338,18 @@ class MultiAgentEnv(_Env):
                                            or int(n_steps) % int(episode_length) != 0):
             raise ValueError("rollout_policy: n_steps (%d) must be a positive multiple of episode_length (%d)"
                              % (int(n_steps), int(episode_length)))
+        if any(_is_recurrent(p) for p in policies):
+            if action_mode != "categorical":
+                raise NotImplementedError("rollout_policy: MAPPO's recurrent actor has action_mode='categorical' only")
+            if rnn_states is not None and episode_length is not None:
+                raise ValueError("rollout_policy: rnn_states cannot be combined with episode_length (every episode "
+                                 "starts from h = 0)")
+            return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
+                                            explore_seed, episode_length, True, record_log_probs, mappo=True,
+                                            gru=(rnn_states, record_rnn_states))
+        if rnn_states is not None or record_rnn_states:
+            raise ValueError("rollout_policy: rnn_states and record_rnn_states need MAPPO's recurrent actor "
+                             "(a policy tuple with an nn.GRU)")
         if any(_has_layer_norm(p) for p in policies):
             if action_mode != "categorical":
                 raise NotImplementedError("rollout_policy: MAPPO's actor (LayerNorm layers) has action_mode='categorical' "
@@ -376,13 +404,34 @@ class MultiAgentEnv(_Env):
         return list(out.obs), list(out.rew_list), list(out.done_list), info_n, {"actions": actions, "rewards": rew_steps}
 
     def _rollout_policy_mlp(self, policies, n_steps, record_actions, per_step_rewards, record_observations, explore_seed,
-                            episode_length=None, categorical=False, record_log_probs=False, mappo=False):
+                            episode_length=None, categorical=False, record_log_probs=False, mappo=False, gru=None):
         import torch
         world = self.world
         nw = world.bind()
         N, T = nw.n_env, int(n_steps)
         nw.require_mlp_actor()   # a program without the kernel is refused as such, before its heads are checked
-        if mappo:
+        rnn = None
+        if gru is not None:      # MAPPO's recurrent actor: gru = (rnn_states, record_rnn_states)
+            nw.require_gru_actor()
+            params, tanh, feature_norm, eps = rmappo_actor_params(policies, nw.obs_dims, nw.act_dims)
+            params = [params]    # one shared set
+            hidden = MAPPO_HIDDEN
+            net = ((_lib.MAPPO_FEATURE_NORM if feature_norm else 0) | (_lib.MAPPO_TANH if tanh else 0), eps)
+            h0, record = gru
+            shape = (self.n, N, MAPPO_HIDDEN)
+            if h0 is not None:
+                if not (torch.is_tensor(h0) and tuple(h0.shape) == shape and h0.dtype == torch.float32
+                        and h0.device == torch.device(nw.device)):
+                    raise ValueError("rollout_policy: rnn_states must be a float32 tensor %s on %s; got %s"
+                                     % (list(shape), nw.device, (tuple(h0.shape), h0.dtype, h0.device)
+                                        if torch.is_tensor(h0) else type(h0).__name__))
+                h = h0.clone(memory_format=torch.contiguous_format)   # the kernel overwrites its state buffer
+            elif episode_length is None:
+                h = torch.zeros(shape, dtype=torch.float32, device=nw.device)
+            else:                # every episode starts from h = 0 without reading the buffer
+                h = torch.empty(shape, dtype=torch.float32, device=nw.device)
+            rnn = (h, torch.empty((T,) + shape, dtype=torch.float32, device=nw.device) if record else None)
+        elif mappo:
             params, tanh, feature_norm, eps = mappo_actor_params(policies, nw.obs_dims, nw.act_dims)
             hidden = MAPPO_HIDDEN
             net = ((_lib.MAPPO_FEATURE_NORM if feature_norm else 0) | (_lib.MAPPO_TANH if tanh else 0), eps)
@@ -390,7 +439,10 @@ class MultiAgentEnv(_Env):
             params, hidden = mlp_actor_params(policies, nw.obs_dims, nw.act_dims)
             net = None
         keep = [[t.detach().to(device=nw.device, dtype=torch.float32).contiguous() for t in p] for p in params]
-        w_ptrs = [_lib.ptr_array([keep[i][j].data_ptr() for i in range(self.n)]) for j in range(6)]
+        if rnn is not None:
+            w_ptrs = [t.data_ptr() for t in keep[0]]
+        else:
+            w_ptrs = [_lib.ptr_array([keep[i][j].data_ptr() for i in range(self.n)]) for j in range(6)]
         out = nw.out if self.reuse_buffers else nw.new_outputs()
         dev = dict(dtype=torch.float32, device=nw.device)
         rew_steps = torch.empty((T, self.n, N), **dev) if per_step_rewards else None
@@ -416,7 +468,9 @@ class MultiAgentEnv(_Env):
                               rew_steps=rew_steps, act_rec_ptrs=act_ptrs, obs_rec_ptrs=obs_ptrs,
                               final_obs_ptrs=_lib.ptr_array([o.data_ptr() for o in final]) if final is not None else None,
                               logp_steps=log_probs, ep_rew=ep_rew, explore_seed=seed, explore_epoch=self.explore_epoch,
-                              mappo=net)
+                              mappo=net, gru=rnn)
+        if rnn is not None:
+            extras["final_rnn_states"], extras["rnn_states"] = rnn
         if episode_length is None:
             reward_n = list(out.rew_list)
         else:
@@ -831,3 +885,97 @@ def mappo_actor_params(policies, obs_dims, act_dims=None):
     if len(eps) != 1:
         raise ValueError("every LayerNorm must have the same eps; got %s" % sorted(eps))
     return params, acts.pop() is nn.Tanh, feature_norms.pop(), eps.pop()
+
+
+# ---- MAPPO's recurrent actor (R_Actor with use_recurrent_policy, recurrent_N = 1, share_policy) -----------------------
+_RMAPPO_SHAPE = ("(base, gru, norm, head) with base = nn.Sequential([LayerNorm(obs_dim)], Linear(obs_dim, 64), Act, "
+                 "LayerNorm(64), Linear(64, 64), Act, LayerNorm(64)), Act = ReLU() or Tanh(), gru = nn.GRU(64, 64), "
+                 "norm = LayerNorm(64), head = Linear(64, act_dim)")
+
+
+def _is_recurrent(pol):
+    """does this policy ask for MAPPO's recurrent actor?  (A tuple holding an nn.GRU; rmappo_actor_params checks it.)"""
+    import torch
+    return isinstance(pol, (tuple, list)) and any(isinstance(m, torch.nn.GRU) for m in pol)
+
+
+def _fold_layer_norm(W, b, ln):
+    """W, b of the Linear (or GRU input map) after LayerNorm ln, in float64, with ln's affine folded in:
+    W' = W diag(gamma), b' = b + W beta"""
+    import torch
+    W, b = W.detach().to(torch.float64), b.detach().to(torch.float64)
+    if ln is None:
+        return W, b
+    g = ln.weight.detach().to(torch.float64)
+    beta = ln.bias.detach().to(torch.float64) if ln.bias is not None else torch.zeros_like(g)
+    return W * g, b + W @ beta
+
+
+def rmappo_actor_params(policies, obs_dims, act_dims=None):
+    """MAPPO's recurrent actor -> (params, tanh, feature_norm, eps), or ValueError.  policies must be one 4-tuple
+    (base, gru, norm, head) shared by every agent ([actor] * n, MAPPO's share_policy; distinct tuples raise
+    NotImplementedError even when their values are equal):
+        base = nn.Sequential([LayerNorm(obs_dim)], Linear(obs_dim, 64), Act, LayerNorm(64), Linear(64, 64), Act,
+               LayerNorm(64))   -- MAPPO's MLPBase, Act = ReLU() or Tanh() in both places
+        gru  = nn.GRU(64, 64) with num_layers=1, bias=True, bidirectional=False
+        norm = nn.LayerNorm(64), head = nn.Linear(64, act_dim)
+    Every LayerNorm affine with one eps, every Linear with a bias, and every agent with the same obs_dim and act_dim
+    (act_dims None means 5).  From an on-policy R_Actor `a`: (nn.Sequential(a.base.feature_norm, *a.base.mlp.fc1,
+    *a.base.mlp.fc2[0]), a.rnn.rnn, a.rnn.norm, a.act.action_out.linear).
+
+    params = (W1, b1, W2, b2, W_ih, b_ih, W_hh, b_hh, W3, b3) in float64, torch's layouts, with each LayerNorm's affine
+    folded into what follows it (the base's last one into W_ih, b_ih; norm into the head), so that the kernel needs only
+    the parameter-free (x - mu) * rsqrt(var + eps).  No device is needed."""
+    import torch
+    nn = torch.nn
+    if act_dims is None:
+        act_dims = [5] * len(obs_dims)
+    if len(policies) != len(obs_dims):
+        raise ValueError("expected %d policies, got %d" % (len(obs_dims), len(policies)))
+    pol = policies[0]
+    if any(p is not pol for p in policies):
+        raise NotImplementedError("the recurrent actor must be one policy object shared by every agent ([actor] * n, "
+                                  "MAPPO's share_policy); distinct per-agent recurrent policies are not supported")
+    if len(set(obs_dims)) != 1 or len(set(act_dims)) != 1:
+        raise ValueError("one shared policy needs every agent to have the same observation and action sizes; got %s "
+                         "and %s" % (list(obs_dims), list(act_dims)))
+    if not (isinstance(pol, (tuple, list)) and len(pol) == 4):
+        raise ValueError("the recurrent actor must be %s" % _RMAPPO_SHAPE)
+    base, gru, norm, head = pol
+    H, od, ad = MAPPO_HIDDEN, obs_dims[0], act_dims[0]
+    layers = [m for m in base.modules() if not list(m.children())] if isinstance(base, nn.Module) else []
+    fn = len(layers) == 7 and type(layers[0]) is nn.LayerNorm
+    body = layers[1:] if fn else layers
+    if not (isinstance(base, nn.Sequential) and len(body) == 6 and type(body[0]) is nn.Linear
+            and type(body[3]) is nn.Linear and type(body[2]) is nn.LayerNorm and type(body[5]) is nn.LayerNorm
+            and type(body[1]) in (nn.ReLU, nn.Tanh) and type(body[4]) is type(body[1])):
+        raise ValueError("the recurrent actor's base must be %s; got %s (%s)"
+                         % (_RMAPPO_SHAPE, type(base).__name__, " -> ".join(type(m).__name__ for m in layers)))
+    if type(gru) is not nn.GRU:
+        raise ValueError("the recurrent actor's second part must be an nn.GRU; got %s" % type(gru).__name__)
+    if gru.num_layers != 1 or gru.bidirectional or not gru.bias or gru.input_size != H or gru.hidden_size != H:
+        raise ValueError("the recurrent actor's GRU must be nn.GRU(%d, %d) with num_layers=1, bias=True and "
+                         "bidirectional=False; got %r" % (H, H, gru))
+    if type(norm) is not nn.LayerNorm or tuple(norm.normalized_shape) != (H,):
+        raise ValueError("the recurrent actor's third part must be nn.LayerNorm(%d); got %r" % (H, norm))
+    if type(head) is not nn.Linear or tuple(head.weight.shape) != (ad, H):
+        raise ValueError("the recurrent actor's head must be nn.Linear(%d, %d); got %r" % (H, ad, head))
+    norms = ((layers[0] if fn else None), body[2], body[5], norm)
+    if any(ln is not None and ln.weight is None for ln in norms):
+        raise ValueError("the recurrent actor: every LayerNorm needs elementwise_affine=True")
+    if any(lin.bias is None for lin in (body[0], body[3], head)):
+        raise ValueError("the recurrent actor: every Linear layer needs a bias")
+    got = (tuple(body[0].weight.shape), tuple(body[3].weight.shape))
+    ln_got = tuple(None if ln is None else tuple(ln.normalized_shape) for ln in norms[:3])
+    if got != ((H, od), (H, H)) or any(g is not None and g != w for g, w in zip(ln_got, ((od,), (H,), (H,)))):
+        raise ValueError("the recurrent actor's base: expected Linear weights %s and LayerNorm shapes %s; got %s and %s"
+                         % ([(H, od), (H, H)], [(od,), (H,), (H,)], list(got), list(ln_got)))
+    eps = {float(ln.eps) for ln in norms if ln is not None}
+    if len(eps) != 1:
+        raise ValueError("every LayerNorm must have the same eps; got %s" % sorted(eps))
+    W1, b1 = _fold_layer_norm(body[0].weight, body[0].bias, norms[0])
+    W2, b2 = _fold_layer_norm(body[3].weight, body[3].bias, body[2])
+    W_ih, b_ih = _fold_layer_norm(gru.weight_ih_l0, gru.bias_ih_l0, body[5])
+    W_hh, b_hh = _fold_layer_norm(gru.weight_hh_l0, gru.bias_hh_l0, None)
+    W3, b3 = _fold_layer_norm(head.weight, head.bias, norm)
+    return (W1, b1, W2, b2, W_ih, b_ih, W_hh, b_hh, W3, b3), type(body[1]) is nn.Tanh, fn, eps.pop()

@@ -282,9 +282,18 @@ class NativeWorld(ShapeHandle):
         if rc == _lib.ERR_UNSUPPORTED:
             check(rc, "mpe_rollout_policy_mlp")
 
+    def require_gru_actor(self):
+        """MpeError unless the library has MAPPO's recurrent actor for this program.  As in require_mlp_actor, the probe
+        reaches the program check and stops at the null state: the aligned dummy weight addresses are never read."""
+        rc = self.lib.mpe_rollout_policy_gru(self.handle, None, None, None, None, *([256] * 10), 64, 0, 0, 0, 0, 0,
+                                             None, None, None, None, None, None, None, None, 0, 0.0, None, 0,
+                                             self._stream())
+        if rc == _lib.ERR_UNSUPPORTED:
+            check(rc, "mpe_rollout_policy_gru")
+
     def rollout_policy_mlp(self, w_ptrs, hidden, n_steps, out=None, flags=0, *, episode_length=None, categorical=False,
                            rew_steps=None, act_rec_ptrs=None, obs_rec_ptrs=None, final_obs_ptrs=None, logp_steps=None,
-                           ep_rew=None, explore_seed=None, explore_epoch=0, mappo=None):
+                           ep_rew=None, explore_seed=None, explore_epoch=0, mappo=None, gru=None):
         """n_steps fused steps in ONE launch with every agent's two-hidden-layer actor evaluated on the tensor cores
         (mpe_rollout_policy_mlp); w_ptrs: the six pointer arrays (W1, b1, W2, b2, W3, b3), one device pointer per
         agent each.  explore_seed (not None) switches the Gumbel-softmax sampling on.
@@ -300,9 +309,17 @@ class NativeWorld(ShapeHandle):
         reset; final_obs_ptrs: one [episodes, N, obs_dim_i] record per agent of each episode's last observation.
 
         mappo=(net_flags, eps) (mpe_rollout_policy_mappo[_episodes], categorical only): MAPPO's actor, w_ptrs holding
-        its folded network (environment.mappo_actor_params); net_flags is _lib.MAPPO_FEATURE_NORM | _lib.MAPPO_TANH."""
+        its folded network (environment.mappo_actor_params); net_flags is _lib.MAPPO_FEATURE_NORM | _lib.MAPPO_TANH.
+
+        gru=(rnn_state, rnn_record) with mappo (mpe_rollout_policy_gru[_episodes]): MAPPO's recurrent actor.  w_ptrs is
+        then the ten device pointers of its one shared folded weight set (W1, b1, W2, b2, W_ih, b_ih, W_hh, b_hh, W3,
+        b3; environment.rmappo_actor_params); rnn_state, a float32 [A, N, 64] CUDA tensor, holds the initial hidden
+        state and receives the final one, and rnn_record (float32 [n_steps, A, N, 64], or None) the h each step
+        consumed."""
         out = out or self.out
         episodes = episode_length is not None
+        if gru is not None and mappo is None:
+            raise ValueError("rollout_policy_mlp: the recurrent actor is MAPPO's (pass mappo=(net_flags, eps))")
         if mappo is not None and not categorical:
             raise ValueError("rollout_policy_mlp: the MAPPO actor has the categorical form only")
         if episodes and self.torch.cuda.is_current_stream_capturing():
@@ -313,7 +330,12 @@ class NativeWorld(ShapeHandle):
         explore_args = (int(explore), int(explore_seed) if explore else 0, int(explore_epoch))
         rew_ptr = rew_steps.data_ptr() if rew_steps is not None else None
         logp = (logp_steps.data_ptr() if logp_steps is not None else None,) if categorical else ()
-        if mappo is not None:
+        rnn = ()
+        if gru is not None:
+            name = "mpe_rollout_policy_gru" + ("_episodes" if episodes else "")
+            net = (int(mappo[0]), float(mappo[1]))
+            rnn = (gru[0].data_ptr(), gru[1].data_ptr() if gru[1] is not None else None)
+        elif mappo is not None:
             name = "mpe_rollout_policy_mappo" + ("_episodes" if episodes else "")
             net = (int(mappo[0]), float(mappo[1]))
         else:
@@ -325,11 +347,11 @@ class NativeWorld(ShapeHandle):
             rc = getattr(self.lib, name)(self.handle, pv, lm, comm, goal, *w_ptrs, int(hidden), int(episode_length),
                                          n_episodes, *explore_args, self.seed, epoch, self.world_offset, out.obs_ptrs,
                                          ep_rew.data_ptr(), rew_ptr, *logp, act_rec_ptrs, obs_rec_ptrs, final_obs_ptrs,
-                                         *net, out.done_ptr, flags, self._stream())
+                                         *rnn, *net, out.done_ptr, flags, self._stream())
         else:
             rc = getattr(self.lib, name)(self.handle, pv, lm, comm, goal, *w_ptrs, int(hidden), int(n_steps), *explore_args,
                                          self.world_offset, out.obs_ptrs, out.rew_ptr, rew_ptr, *logp, act_rec_ptrs,
-                                         obs_rec_ptrs, *net, out.done_ptr, flags, self._stream())
+                                         obs_rec_ptrs, *rnn, *net, out.done_ptr, flags, self._stream())
         check(rc, name)
         if episodes:
             self.epoch = epoch + n_episodes

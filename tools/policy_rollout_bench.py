@@ -11,9 +11,14 @@
       mpe_rollout_policy_mappo), --categorical and --layers 3 implied; --tanh for Act = Tanh (else ReLU),
       --feature-norm for the input LayerNorm.  The MADDPG categorical kernel is timed in the same run
       ("maddpg_in_kernel"), so the cost of the LayerNorms and the tanh shows;
+      --actor rmappo: MAPPO's recurrent actor, one (base, gru, norm, head) tuple shared by every agent (base = the MAPPO
+      actor without its last Linear, nn.GRU(64, 64), LayerNorm(64), Linear(64, act_dim); mpe_rollout_policy_gru), with
+      the same implied options and --tanh / --feature-norm;
   (b) the same actors as torch modules + env.step, all captured in one CUDA graph (rollout.GraphedRollout); with
       --categorical the graphed policy takes argmax(logits - log(-log u)) per sub-space, its one_hot and
-      log_softmax(logits).gather(k) for the log-probabilities.
+      log_softmax(logits).gather(k) for the log-probabilities.  With --actor rmappo the graphed policy evaluates the
+      shared tuple once on every agent's observations stacked (base -> one nn.GRU step from the carried h, kept in a
+      graph-resident tensor -> LayerNorm -> head), at float32 matmul precision "highest".
 Device time per step of each.  With --layers 3 the actor of agent i has act_dim_i outputs and its action is one
 (Gumbel-)softmax per action sub-space (5 movement logits if the agent moves, then dim_c utterance logits if it speaks).
 Also the actor's FLOPs per step, computed from the padded shapes the kernel multiplies (2 (K1 H + H H + NOUT H) per
@@ -62,15 +67,16 @@ def main():
     ap.add_argument("--explore", action="store_true", help="Gumbel-softmax exploration (--layers 3)")
     ap.add_argument("--categorical", action="store_true",
                     help="one-hot arg-max actions with index and log-probability records (--layers 3)")
-    ap.add_argument("--actor", choices=("maddpg", "mappo"), default="maddpg",
-                    help="mappo: MAPPO's LayerNorm actor (implies --layers 3 --categorical)")
+    ap.add_argument("--actor", choices=("maddpg", "mappo", "rmappo"), default="maddpg",
+                    help="mappo: MAPPO's LayerNorm actor, rmappo: its recurrent actor (both imply --layers 3 "
+                         "--categorical)")
     ap.add_argument("--tanh", action="store_true", help="MAPPO's actor with Tanh instead of ReLU")
     ap.add_argument("--feature-norm", action="store_true", help="MAPPO's actor with the input LayerNorm")
     args = ap.parse_args()
-    if args.actor == "mappo":
+    if args.actor in ("mappo", "rmappo"):
         args.layers, args.categorical = 3, True
     elif args.tanh or args.feature_norm:
-        ap.error("--tanh and --feature-norm need --actor mappo")
+        ap.error("--tanh and --feature-norm need --actor mappo or rmappo")
     try:
         skw = {k: int(v) for k, v in (kv.split("=", 1) for kv in args.scenario_kwargs)}
     except ValueError:
@@ -104,13 +110,24 @@ def main():
         mods = [nn.Sequential(*(([nn.LayerNorm(od)] if args.feature_norm else []) +
                                 [nn.Linear(od, H), Act(), nn.LayerNorm(H), nn.Linear(H, H), Act(), nn.LayerNorm(H),
                                  nn.Linear(H, ad)])).to(dev) for od, ad in zip(nw.obs_dims, nw.act_dims)]
+    rnn = None
+    if args.actor == "rmappo":
+        nn = torch.nn
+        torch.set_float32_matmul_precision("highest")
+        Act = nn.Tanh if args.tanh else nn.ReLU
+        od, ad = nw.obs_dims[0], nw.act_dims[0]
+        base = nn.Sequential(*(([nn.LayerNorm(od)] if args.feature_norm else []) +
+                               [nn.Linear(od, H), Act(), nn.LayerNorm(H), nn.Linear(H, H), Act(), nn.LayerNorm(H)]))
+        actor = tuple(m.to(dev) for m in (base, nn.GRU(H, H), nn.LayerNorm(H), nn.Linear(H, ad)))
+        mods = [actor] * len(nw.obs_dims)
+        rnn = torch.zeros(len(nw.obs_dims) * n, H, device=dev)    # the graphed loop's carried h, agents stacked
     segs = sub_spaces(env.world) if args.layers == 3 else [[5]] * len(nw.obs_dims)
     res = {"config": {"scenario": args.scenario, "scenario_kwargs": skw, "n_env": n, "T": T, "hidden": H}}
     if args.layers == 3:
         res["config"].update(layers=3, explore=args.explore, categorical=args.categorical,
                              torch_float32_matmul_precision=torch.get_float32_matmul_precision())
-    if args.actor == "mappo":
-        res["config"].update(actor="mappo", tanh=args.tanh, feature_norm=args.feature_norm)
+    if args.actor in ("mappo", "rmappo"):
+        res["config"].update(actor=args.actor, tanh=args.tanh, feature_norm=args.feature_norm)
     kw = {"explore_seed": 1} if args.explore else {}
     if args.categorical:
         kw.update(action_mode="categorical", record_actions=True, record_log_probs=True)
@@ -133,7 +150,7 @@ def main():
     if maddpg_mods is not None:   # the MADDPG categorical kernel on the same env, same sizes
         sec_m = time_in_kernel(maddpg_mods)
         res["maddpg_in_kernel"] = {"us_per_step": 1e6 * sec_m, "env_steps_per_sec": n / sec_m}
-    if args.layers == 3:
+    if args.layers == 3 and rnn is None:
         flops = actor_flops_per_step(nw.obs_dims, nw.act_dims, H, n)
         res["in_kernel"].update(actor_flop_per_step=flops, actor_tflops=flops / sec / 1e12)
     # (b) torch actors + env.step in one CUDA graph
@@ -157,7 +174,20 @@ def main():
 
     logps = []   # the graph's log-probability outputs, kept as a trainer would keep them
 
+    def recurrent_policy(obs_n):
+        # torch's GRU step written out (F.linear GEMMs and pointwise kernels capture in a graph on every backend)
+        F = torch.nn.functional
+        base, gru, norm, head = mods[0]
+        gi = F.linear(base(torch.cat(obs_n, 0)), gru.weight_ih_l0, gru.bias_ih_l0).chunk(3, 1)
+        gh = F.linear(rnn, gru.weight_hh_l0, gru.bias_hh_l0).chunk(3, 1)
+        r, z = torch.sigmoid(gi[0] + gh[0]), torch.sigmoid(gi[1] + gh[1])
+        hn = (1 - z) * torch.tanh(gi[2] + r * gh[2]) + z * rnn
+        rnn.copy_(hn)
+        return [categorical(zz, seg) for zz, seg in zip(head(norm(hn)).split(n), segs)]
+
     def policy(obs_n):
+        if rnn is not None:
+            return recurrent_policy(obs_n)
         if args.categorical:
             return [categorical(m(o), seg) for m, o, seg in zip(mods, obs_n, segs)]
         if args.explore:   # the same Gumbel-softmax sample, noise from torch's generator

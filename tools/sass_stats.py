@@ -128,11 +128,11 @@ def main():
     for r in rows:
         print("| " + " | ".join(str(x) for x in r) + " |")
     forms = {"mlp_rollout": "S", "mlp_episode": "E", "mlp_categorical": "C", "mlp_categorical_episode": "CE",
-             "mappo": "M", "mappo_episode": "ME"}
+             "mappo": "M", "mappo_episode": "ME", "gru": "G", "gru_episode": "GE"}
     mlp = []
     for mangled, (reg, stack) in usage.items():
         m = re.match(r"void mpe::mpe_policy_(mlp_rollout|mlp_episode|mlp_categorical|mlp_categorical_episode|mappo|"
-                     r"mappo_episode)_kernel<mpe::(.+?)(?:, (\d+))?\s*>\(", names[mangled])
+                     r"mappo_episode|gru|gru_episode)_kernel<mpe::(.+?)(?:, (\d+))?\s*>\(", names[mangled])
         if m:
             c = mix.get(mangled, {})
             mlp.append((m.group(2), m.group(3) or "64", forms[m.group(1)], reg, stack, c["total"], c["HMMA"], c["LDS"],
@@ -140,7 +140,8 @@ def main():
     if mlp:
         print("\n## Closed-loop rollout with the two-hidden-layer actor (TF32 mma.sync), by form: S "
               "`mpe_policy_mlp_rollout_kernel`, E its episode form `mpe_policy_mlp_episode_kernel`, C and CE the "
-              "categorical forms of both, M and ME MAPPO's LayerNorm actor `mpe_policy_mappo[_episode]_kernel` (H = 64)\n")
+              "categorical forms of both, M and ME MAPPO's LayerNorm actor `mpe_policy_mappo[_episode]_kernel`, G and GE its "
+              "recurrent actor `mpe_policy_gru[_episode]_kernel` (both H = 64)\n")
         print("| program | H | form | regs | stack | instr | HMMA | LDS | MUFU |")
         print("|---|---|---|---|---|---|---|---|---|")
         for r in sorted(mlp):
