@@ -370,6 +370,40 @@ MPE_API int mpe_rollout_policy_gru_episodes(
     float *rnn_state_dev, float *rnn_state_record_dev, uint32_t net_flags, float ln_eps, uint8_t *done_dev,
     uint32_t flags, void *stream);
 
+/* MAPPO's MLP actor (mpe_rollout_policy_mappo[_episodes]) with MAPPO's centralized critic (R_Critic with
+ * use_centralized_V, non-recurrent, hidden width 64) evaluated in the same launch:
+ *     [LN(D)] -> Linear(D, 64) -> act -> LN(64) -> Linear(64, 64) -> act -> LN(64) -> Linear(64, 1)
+ * on share_obs, every agent's raw observation concatenated in agent order (D = sum of obs_dim_i), with the actor's act,
+ * input LayerNorm (net_flags) and ln_eps; cw1_n .. cb3_n its folded weights (as the actor's: [64][D], [64], [64][64],
+ * [64], [1][64], [1]), critic_count pointers each.  critic_count 1: one shared critic whose value is written for every
+ * agent; critic_count A: agent i's own critic.  values_dev ([T][A][N] fp32, required) receives V of the state each step's
+ * actors act on; final_values_dev ([A][N], in the episode form [n_episodes][A][N], required) V of the state after the
+ * last step (of each episode, before its reset).  The critic changes nothing else: every other output, record and
+ * state is bit-identical to mpe_rollout_policy_mappo[_episodes]'s.  Return codes and their order are MAPPO's, plus:
+ * MPE_ERR_UNSUPPORTED, after the program check, for a program without the critic kernel (simple_spread N = 6,
+ * simple_tag 6+2, simple_world_comm) or when critic_count critics leave no room for a warp in shared memory;
+ * MPE_ERR_BAD_ARG there for a critic_count other than 1 or A, and after the recurrent actor's checks for a null or
+ * misaligned critic weight or value record. */
+MPE_API int mpe_rollout_policy_mappo_critic(
+    mpe_handle h, void *agent_pv_dev, const void *lm_p_dev, float *comm_dev, const int32_t *goal_dev,
+    const float *const *w1_n, const float *const *b1_n, const float *const *w2_n, const float *const *b2_n,
+    const float *const *w3_n, const float *const *b3_n, int32_t hidden, int32_t n_steps, int32_t explore,
+    uint64_t explore_seed, uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n_dev, float *rew_sum_dev,
+    float *rew_steps_dev, float *logp_steps_dev, int32_t *const *act_index_record_n, float *const *obs_record_n,
+    uint32_t net_flags, float ln_eps, int32_t critic_count, const float *const *cw1_n, const float *const *cb1_n,
+    const float *const *cw2_n, const float *const *cb2_n, const float *const *cw3_n, const float *const *cb3_n,
+    float *values_dev, float *final_values_dev, uint8_t *done_dev, uint32_t flags, void *stream);
+MPE_API int mpe_rollout_policy_mappo_critic_episodes(
+    mpe_handle h, void *agent_pv_dev, void *lm_p_dev, float *comm_dev, int32_t *goal_dev, const float *const *w1_n,
+    const float *const *b1_n, const float *const *w2_n, const float *const *b2_n, const float *const *w3_n,
+    const float *const *b3_n, int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
+    uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset,
+    float *const *obs_n_dev, float *ep_rew_dev, float *rew_steps_dev, float *logp_steps_dev,
+    int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n,
+    uint32_t net_flags, float ln_eps, int32_t critic_count, const float *const *cw1_n, const float *const *cb1_n,
+    const float *const *cw2_n, const float *const *cb2_n, const float *const *cw3_n, const float *const *cb3_n,
+    float *values_dev, float *final_values_dev, uint8_t *done_dev, uint32_t flags, void *stream);
+
 /* Same step for a caller that holds HOST buffers (what the reference's callers hold):
  * act_n_host[i] -> (async H2D into act_n_dev[i]) -> mpe_step -> (async D2H) obs_n_host[i],
  * rew_host, done_host, all ordered on `stream`.  Host buffers should be pinned for the copies

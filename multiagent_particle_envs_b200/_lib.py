@@ -124,6 +124,18 @@ _SIGNATURES = {
                                          ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64,
                                          ctypes.c_uint64, _PP, _P, _P, _P, _PP, _PP, _PP, _P, _P, ctypes.c_uint32,
                                          ctypes.c_float, _P, ctypes.c_uint32, _P]),
+    "mpe_rollout_policy_mappo_critic": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _PP, _PP, _PP, ctypes.c_int32,
+                                                       ctypes.c_int32, ctypes.c_int32, ctypes.c_uint64, ctypes.c_uint64,
+                                                       ctypes.c_uint64, _PP, _P, _P, _P, _PP, _PP, ctypes.c_uint32,
+                                                       ctypes.c_float, ctypes.c_int32, _PP, _PP, _PP, _PP, _PP, _PP, _P, _P,
+                                                       _P, ctypes.c_uint32, _P]),
+    "mpe_rollout_policy_mappo_critic_episodes": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _PP, _PP, _PP,
+                                                                ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                                                ctypes.c_int32, ctypes.c_uint64, ctypes.c_uint64,
+                                                                ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, _PP, _P,
+                                                                _P, _P, _PP, _PP, _PP, ctypes.c_uint32, ctypes.c_float,
+                                                                ctypes.c_int32, _PP, _PP, _PP, _PP, _PP, _PP, _P, _P, _P,
+                                                                ctypes.c_uint32, _P]),
     "mpe_step_host": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _P, _P, _P, _PP, _P, _P, _P,
                                      ctypes.c_uint32, _P]),
     "mpe_strerror": (ctypes.c_char_p, [ctypes.c_int]),

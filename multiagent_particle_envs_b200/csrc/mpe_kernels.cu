@@ -920,6 +920,31 @@ struct MlpGruEpisodeArgs {
 };
 static_assert(sizeof(MlpGruEpisodeArgs) <= 4096, "kernel parameter space");
 
+// MAPPO's centralized critic (R_Critic with use_centralized_V, recurrent off: MLPBase with layer_N = 1, then v_out) next
+// to MAPPO's actor:
+//     [LN(D)] -> Linear(D, 64) -> act -> LN(64) -> Linear(64, 64) -> act -> LN(64) -> Linear(64, 1)
+// Its input is share_obs, every agent's raw observation concatenated in agent order (D = sum of obs_dim_i); act, eps
+// and the input LayerNorm are the actor's (MlpMappoArgs), the affines folded as the actor's.  count = 1: one shared
+// critic (w*[0]), its value written for every agent; count = A: agent i's critic (w*[i]) evaluates the same input.
+// values [T][A][n] receives V of the state each step's actors act on (MAPPO's value_preds), final_values [A][n] (in the
+// episode form [episodes][A][n]) V of the state after the last step (of each episode, before its reset).
+struct MlpCriticState {
+    const float *w1[kMaxA], *b1[kMaxA];   // [64][D], [64]
+    const float *w2[kMaxA], *b2[kMaxA];   // [64][64], [64]
+    const float *w3[kMaxA], *b3[kMaxA];   // [1][64], [1]
+    int32_t count;
+    float *values, *final_values;
+};
+struct MlpCriticArgs {
+    MlpMappoArgs m;
+    MlpCriticState v;
+};
+struct MlpCriticEpisodeArgs {
+    MlpMappoEpisodeArgs m;
+    MlpCriticState v;
+};
+static_assert(sizeof(MlpCriticEpisodeArgs) <= 4096, "kernel parameter space");
+
 template <class P, int H>
 struct MlpShape {
     static constexpr int NT = H / 8;                                   // n-tiles of a hidden layer (= its k-tiles)
@@ -1055,6 +1080,68 @@ __host__ __device__ constexpr int gru_block_warps() {
                   "8 warps' tiles fit next to the weights");
     return kGruWarps;
 }
+
+// One critic's weights in shared memory, in floats: B fragments [k-tile][n-tile][lane][2] of W1, agent by agent (agent
+// i's obs_dim_i columns zero-padded to whole k-tiles, so that layer 1 is a sum of k-slices over the agents'
+// observation tiles), then of W2 and W3 (one n-tile, its one real column first), then b1 [64], b2 [64], b3 [8].  They
+// follow the actor's weights (MlpShape), count sets in a row; the warps' tiles are the actor's.
+template <class P>
+struct CriticShape {
+    using M = MlpShape<P, 64>;
+    static constexpr int NT = 8;
+    __host__ __device__ static constexpr int in_dim() { int s = 0; for (int i = 0; i < P::A; ++i) s += P::obs_dim(i); return s; }
+    __host__ __device__ static constexpr int col_off(int i) { int s = 0; for (int j = 0; j < i; ++j) s += P::obs_dim(j); return s; }
+    __host__ __device__ static constexpr int w1_off(int i) { int s = 0; for (int j = 0; j < i; ++j) s += 64 * M::kt1(j) * NT; return s; }
+    static constexpr int w2_off = w1_off(P::A);
+    static constexpr int w3_off = w2_off + 64 * NT * NT;
+    static constexpr int b1_off = w3_off + 64 * NT;
+    static constexpr int b2_off = b1_off + 64;
+    static constexpr int b3_off = b2_off + 64;
+    static constexpr int kFloats = b3_off + 8;
+};
+// Warps per block at most, for the critics' count: the weights of the actor and of `count` critics plus kWarpFloats per
+// warp within the 227 KB
+template <class P>
+__host__ __device__ constexpr int critic_smem_warps(int count) {
+    return (kMlpSmemBytes / 4 - MlpShape<P, 64>::kWeightFloats - count * CriticShape<P>::kFloats) / MlpShape<P, 64>::kWarpFloats;
+}
+// The critic is built where one shared critic leaves room for a warp: every MAPPO program but spread N=6 (175 KB of
+// actor weights and an 80 KB critic) and tag 6+2 (212 KB and 85 KB).
+template <class P>
+__host__ __device__ constexpr bool critic_built() { return MlpBuilt<P>::value && critic_smem_warps<P>(1) >= 1; }
+// The compile-time cap of the two critic kernels, sized for one shared critic: MAPPO's register rule for its form
+// (mlp_register_warps) unless an exception below holds (ptxas -v: no spills and no stack), lowered to what the shared
+// critic's weights leave in shared memory.  The launcher lowers it at run time to critic_smem_warps(count).
+// Forms by MAPPO's bits (kFormM: one episode, kFormME: episodes); the stack ptxas -v showed without the exception.
+template <class P> struct CriticRegisterException : MlpException<0, 0> {};
+template <> struct CriticRegisterException<Simple<1, 1>> : MlpException<kFormM, 12> {};                 // 8 at 128
+template <> struct CriticRegisterException<Push<1, 1, 2>> : MlpException<kFormM | kFormME, 12> {};      // 32, 24 at 128
+template <> struct CriticRegisterException<Crypto> : MlpException<kFormME, 12> {};                      // 24 at 128
+template <> struct CriticRegisterException<Spread<4>> : MlpException<kFormM | kFormME, 8> {};           // 40, 40 at 168
+template <> struct CriticRegisterException<Adversary<1, 3, 3>> : MlpException<kFormM | kFormME, 8> {};  // 8, 32 at 168
+template <class P, bool EPISODES>
+__host__ __device__ constexpr int critic_block_warps() {
+    using X = CriticRegisterException<P>;
+    constexpr int r = (X::forms >> (EPISODES ? 5 : 4) & 1) ? X::warps : mlp_register_warps<P, 64, EPISODES ? 5 : 4>();
+    constexpr int s = critic_smem_warps<P>(1);
+    return r < s ? r : s;
+}
+// one critic takes 21-60 KB where it is built (spread N=3: 37 KB); n per-agent ones fit next to the actor for simple,
+// spread N=2 and 3, tag 1+1 and 2+1, adversary 1+2, push, speaker_listener, reference and crypto
+static_assert(CriticShape<Simple<1, 1>>::kFloats * 4 == 21024 && CriticShape<Spread<5>>::kFloats * 4 == 59936,
+              "simple: a 21 024 B critic; spread N=5: 59 936 B");
+static_assert(CriticShape<Spread<3>>::kFloats * 4 == 37408 && critic_smem_warps<Spread<3>>(1) == 34 &&
+              critic_smem_warps<Spread<3>>(3) == 12, "spread N=3: 75 360 + 37 408 + 34 x 3456 B; 3 critics, 12 warps");
+static_assert(critic_smem_warps<Spread<5>>(1) == 7 && critic_smem_warps<Tag<4, 2, 2>>(1) == 6,
+              "the smallest shared-critic blocks: spread N=5 7 warps, tag 4+2 6");
+static_assert(critic_smem_warps<SpeakerListener>(2) == 53 && critic_smem_warps<Reference>(2) == 23 &&
+              critic_smem_warps<Crypto>(3) == 38 && critic_smem_warps<Adversary<1, 2, 2>>(3) == 31,
+              "per-agent critics that fit");
+static_assert(critic_smem_warps<Adversary<1, 3, 3>>(4) < 1 && critic_smem_warps<Tag<3, 1, 2>>(4) < 1 &&
+              critic_smem_warps<Spread<4>>(4) < 1 && critic_smem_warps<Spread<5>>(5) < 1 &&
+              critic_smem_warps<Tag<4, 2, 2>>(6) < 1, "per-agent critics that do not fit");
+static_assert(!critic_built<Spread<6>>() && !critic_built<Tag<6, 2, 3>>() && critic_built<Tag<4, 2, 2>>(),
+              "no critic kernel for spread N=6 and tag 6+2");
 
 __device__ __forceinline__ uint32_t to_tf32(float x) {
     uint32_t r;
@@ -1532,24 +1619,172 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
     }
 }
 
+// register-only observation writers: the sum of an observation's entries, and the sum of their squared deviations from
+// mu (P::observe is pure in the world registers, so the critic calls it once per pass)
+struct SumWriter {
+    float s = 0.0f;
+    __device__ __forceinline__ void put(float x) { s += x; }
+    __device__ __forceinline__ void put2(float a, float b) { s += a; s += b; }
+    __device__ __forceinline__ void put2(float2 v) { put2(v.x, v.y); }
+};
+struct SqDevWriter {
+    float mu, s = 0.0f;
+    __device__ __forceinline__ void put(float x) { const float dx = x - mu; s += dx * dx; }
+    __device__ __forceinline__ void put2(float a, float b) { put(a); put(b); }
+    __device__ __forceinline__ void put2(float2 v) { put2(v.x, v.y); }
+};
+
+// Critic W1's columns of agent I ([64][D] torch layout, global) -> TF32 B fragments of its kt1(I) k-tiles, as
+// stage_fragments (PERM = false) lays them out; columns beyond obs_dim_I are zero
+template <class P, int I>
+__device__ __forceinline__ void stage_critic_w1(float *dst, const float *__restrict__ W) {
+    using C = CriticShape<P>;
+    constexpr int KT = MlpShape<P, 64>::kt1(I), OD = P::obs_dim(I), D = C::in_dim(), OFF = C::col_off(I);
+    for (int q = threadIdx.x; q < KT * C::NT * 64; q += blockDim.x) {
+        const int j = q & 1, l = (q >> 1) & 31, tile = q >> 6;
+        const int nt = tile % C::NT, kt = tile / C::NT;
+        const int nn = nt * 8 + (l >> 2);
+        const int k = kt * 8 + (l & 3) + 4 * j;
+        dst[q] = __uint_as_float(to_tf32(k < OD ? W[nn * D + OFF + k] : 0.0f));
+    }
+}
+
+// MAPPO's centralized critic for the warp's 32 worlds (MlpCriticState), one weight set Wc (CriticShape): its value of
+// row r goes to dst[s * n + r], s < slots, for r < rows.  The input LayerNorm's statistics over all D entries are two
+// fp32 passes of register-only writers over every agent's observation; layer 1 then sums, agent by agent, that agent's
+// observation in the warp's observation tile, normalised in place, times its k-tiles of W1.  Layers 2 and 3 run as
+// MAPPO's actor runs them, one m-tile at a time, with act_norm_tf32_frags; layer 3 has one real output column.  Called
+// by all 32 lanes; the tile is free on entry and on return.
+template <class P>
+__device__ __forceinline__ void mlp_critic(const float *__restrict__ Wc, const DevDesc &d, const typename P::W &w,
+                                           float *tile, int lane, int rows, float ln_eps, uint32_t net_flags, float *dst,
+                                           int slots, int64_t n) {
+    using C = CriticShape<P>;
+    constexpr int NT = C::NT, D = C::in_dim();
+    const int gq = lane >> 2, tq = lane & 3;
+    const bool feature_norm = net_flags & kMappoFeatureNorm;
+    float mu = 0.0f, rstd = 1.0f;
+    if (feature_norm) {
+        SumWriter sw;
+        static_for<P::A>([&](auto ic) { P::template observe<decltype(ic)::value>(d, w, sw); });
+        mu = sw.s / static_cast<float>(D);
+        SqDevWriter vw{mu};
+        static_for<P::A>([&](auto ic) { P::template observe<decltype(ic)::value>(d, w, vw); });
+        rstd = rsqrtf(vw.s / static_cast<float>(D) + ln_eps);
+    }
+    // ---- layer 1: sum over agents of [32 x K1_i] . W1[:, agent i's columns]^T, + b1 ----
+    float h[2][NT][4];
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+        const float2 b = *reinterpret_cast<const float2 *>(Wc + C::b1_off + nt * 8 + 2 * tq);
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) { h[mt][nt][0] = b.x; h[mt][nt][1] = b.y; h[mt][nt][2] = b.x; h[mt][nt][3] = b.y; }
+    }
+    static_for<P::A>([&](auto ic) {
+        constexpr int I = decltype(ic)::value;
+        constexpr int OD = P::obs_dim(I), KT1 = MlpShape<P, 64>::kt1(I), PITCH = ObsTile<OD>::kPitch;
+        {
+            TileWriter<OD> o(tile, lane);
+            P::template observe<I>(d, w, o);
+        }
+        __syncwarp();
+        if (feature_norm) {
+            float *row = tile + lane * PITCH;
+#pragma unroll
+            for (int c = 0; c < OD; ++c) row[c] = (row[c] - mu) * rstd;
+            __syncwarp();
+        }
+        const float *W1 = Wc + C::w1_off(I);
+#pragma unroll
+        for (int kt = 0; kt < KT1; ++kt) {
+            uint32_t a[2][4];
+            const int c0 = kt * 8 + tq, c1 = c0 + 4;
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt) {
+                const float *r0 = tile + (mt * 16 + gq) * PITCH, *r1 = r0 + 8 * PITCH;
+                a[mt][0] = to_tf32(c0 < OD ? r0[c0] : 0.0f); a[mt][1] = to_tf32(c0 < OD ? r1[c0] : 0.0f);
+                a[mt][2] = to_tf32(c1 < OD ? r0[c1] : 0.0f); a[mt][3] = to_tf32(c1 < OD ? r1[c1] : 0.0f);
+            }
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+                const float2 b = *reinterpret_cast<const float2 *>(W1 + ((kt * NT + nt) * 32 + lane) * 2);
+                mma_tf32(h[0][nt], a[0], b);
+                mma_tf32(h[1][nt], a[1], b);
+            }
+        }
+        __syncwarp();   // every lane has read the tile before the next observation overwrites it
+    });
+    uint32_t x1[2][NT][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt) act_norm_tf32_frags<NT>(x1[mt], h[mt], net_flags & kMappoTanh, ln_eps);
+    // ---- layers 2 and 3 per m-tile: h2 = x1 . W2^T + b2, act + LayerNorm, v = x2 . W3^T + b3 ----
+    const float *W2 = Wc + C::w2_off, *W3 = Wc + C::w3_off;
+    const float2 b3 = *reinterpret_cast<const float2 *>(Wc + C::b3_off + 2 * tq);
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt) {
+        float c[NT][4];
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) {
+            const float2 bb = *reinterpret_cast<const float2 *>(Wc + C::b2_off + nt * 8 + 2 * tq);
+            c[nt][0] = bb.x; c[nt][1] = bb.y; c[nt][2] = bb.x; c[nt][3] = bb.y;
+#pragma unroll
+            for (int kt = 0; kt < NT; ++kt)
+                mma_tf32(c[nt], x1[mt][kt], *reinterpret_cast<const float2 *>(W2 + ((kt * NT + nt) * 32 + lane) * 2));
+        }
+        uint32_t x2[NT][4];
+        act_norm_tf32_frags<NT>(x2, c, net_flags & kMappoTanh, ln_eps);
+        float v[4] = {b3.x, b3.y, b3.x, b3.y};
+#pragma unroll
+        for (int kt = 0; kt < NT; ++kt) mma_tf32(v, x2[kt], *reinterpret_cast<const float2 *>(W3 + (kt * 32 + lane) * 2));
+        // column 0 of rows g and g + 8 sits in element 0 and 2 of the quad's first lane
+        const int ra = mt * 16 + gq, rb = ra + 8;
+        if (tq == 0) {
+            for (int s = 0; s < slots; ++s) {
+                if (ra < rows) dst[s * n + ra] = v[0];
+                if (rb < rows) dst[s * n + rb] = v[2];
+            }
+        }
+        __syncwarp();   // as in MAPPO's actor: the second m-tile reads W2's and W3's fragments again
+    }
+}
+
+// every critic's values of the current state into record row `row` of rec (values [T][A][n] or final_values):
+// a shared critic's (count 1) for every agent, else critic k's for agent k
+template <class P>
+__device__ __forceinline__ void run_critics(const MlpCriticState &cs, const float *Wc, const DevDesc &d,
+                                            const typename P::W &w, float *tile, int lane, int rows, float ln_eps,
+                                            uint32_t net_flags, float *rec, int row, int64_t w0, int64_t n) {
+    const int slots = cs.count == 1 ? P::A : 1;
+#pragma unroll 1
+    for (int k = 0; k < cs.count; ++k)
+        mlp_critic<P>(Wc + k * CriticShape<P>::kFloats, d, w, tile, lane, rows, ln_eps, net_flags,
+                      rec + (static_cast<int64_t>(row) * P::A + k) * n + w0, slots, n);
+}
+
 // the body of both forms; ea is null in the single-episode form (EPISODES = false), cr unless CATEGORICAL; ln_eps and
-// net_flags are MAPPO's (MlpMappoArgs), gs the recurrent actor's (GRU, MlpGruArgs)
-template <class P, int H, bool EPISODES, bool CATEGORICAL = false, bool MAPPO = false, bool GRU = false>
+// net_flags are MAPPO's (MlpMappoArgs), gs the recurrent actor's (GRU, MlpGruArgs), cs the critic's (CRITIC,
+// MlpCriticArgs)
+template <class P, int H, bool EPISODES, bool CATEGORICAL = false, bool MAPPO = false, bool GRU = false,
+          bool CRITIC = false>
 __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEpisodeArgs *ea,
                                             const MlpCategoricalRecords *cr = nullptr, float ln_eps = 0.0f,
-                                            uint32_t net_flags = 0, const MlpGruState *gs = nullptr) {
+                                            uint32_t net_flags = 0, const MlpGruState *gs = nullptr,
+                                            const MlpCriticState *cs = nullptr) {
+    static_assert(!CRITIC || (MAPPO && !GRU), "the critic runs next to MAPPO's MLP actor");
     static_assert(H == 32 || H == 64, "MLP policy rollout: hidden width 32 or 64");
     constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     using S = MlpShape<P, H>;
     constexpr int kWarps = [] {
         if constexpr (GRU) return gru_block_warps<P>();
+        else if constexpr (CRITIC) return critic_block_warps<P, EPISODES>();
         else return mlp_block_warps<P, H, EPISODES | (MAPPO ? 2 : CATEGORICAL) << 1>();
     }();
     constexpr int kWeightFloats = [] {
         if constexpr (GRU) return GruShape<P>::kWeightFloats;
         else return S::kWeightFloats;
     }();
-    static_assert(kWarps >= 1 && (kWeightFloats + kWarps * S::kWarpFloats) * 4 <= kMlpSmemBytes, "one block fits an SM");
+    static_assert(kWarps >= 1 && (kWeightFloats + (CRITIC ? CriticShape<P>::kFloats : 0) + kWarps * S::kWarpFloats) * 4 <=
+                  kMlpSmemBytes, "one block fits an SM");
     const StepArgs &a = pa.s;
     extern __shared__ __align__(16) float smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1586,6 +1821,26 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
         for (int q = threadIdx.x; q < S::nout(i); q += blockDim.x) base[S::b3_off(i) + q] = q < P::act_dim(i) ? pa.b3[i][q] : 0.0f;
     });
     }
+    int crit_floats = 0;   // the critics' weights after the actor's (CriticShape), cs->count sets
+    if constexpr (CRITIC) {
+        using C = CriticShape<P>;
+        crit_floats = cs->count * C::kFloats;
+#pragma unroll 1
+        for (int k = 0; k < cs->count; ++k) {
+            float *base = smem + kWeightFloats + k * C::kFloats;
+            static_for<A>([&](auto ic) {
+                constexpr int i = decltype(ic)::value;
+                stage_critic_w1<P, i>(base + C::w1_off(i), cs->w1[k]);
+            });
+            stage_fragments<C::NT, C::NT, true>(base + C::w2_off, cs->w2[k], 64, 64);
+            stage_fragments<C::NT, 1, true>(base + C::w3_off, cs->w3[k], 1, 64);
+            for (int q = threadIdx.x; q < 64; q += blockDim.x) {
+                base[C::b1_off + q] = cs->b1[k][q];
+                base[C::b2_off + q] = cs->b2[k][q];
+            }
+            for (int q = threadIdx.x; q < 8; q += blockDim.x) base[C::b3_off + q] = q == 0 ? cs->b3[k][0] : 0.0f;
+        }
+    }
     __syncthreads();
 
     const int64_t n = a.n;
@@ -1595,7 +1850,8 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
     const int rows = (end - w0) < 32 ? static_cast<int>(end - w0) : 32;
     const bool active = lane < rows;
     const int64_t wi = w0 + (active ? lane : 0);   // idle lanes of a partial tile replay world w0: every tile row is finite
-    float *s_warp = smem + kWeightFloats + warp * S::kWarpFloats;
+    float *s_warp = smem + kWeightFloats + crit_floats + warp * S::kWarpFloats;
+    const float *Wc = smem + kWeightFloats;   // the critics' weights
     const DevDesc &d = a.d;
 
     typename P::W w;
@@ -1629,6 +1885,7 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
             float ux[A], uy[A];
             float cact[NC > 0 ? NC : 1];
             P::prepare(d, w);
+            if constexpr (CRITIC) run_critics<P>(*cs, Wc, d, w, s_warp, lane, rows, ln_eps, net_flags, cs->values, tg, w0, n);   // V of the state the actors act on
             static_for<A>([&](auto ic) {
                 constexpr int i = decltype(ic)::value;
                 const float2 u = mlp_agent<P, H, i, EPISODES, CATEGORICAL, MAPPO, GRU>(
@@ -1660,6 +1917,11 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
             if (active) {
 #pragma unroll
                 for (int i = 0; i < A; ++i) a.rew[(static_cast<int64_t>(e) * A + i) * n + wi] = rsum[i];
+            }
+            if constexpr (CRITIC) {                            // V of the final state, before the reset
+                P::prepare(d, w);
+                __syncwarp();                                  // every lane has read its logits before the tile is reused
+                run_critics<P>(*cs, Wc, d, w, s_warp, lane, rows, ln_eps, net_flags, cs->final_values, e, w0, n);
             }
             if (ea->final_obs[0] != nullptr) {                 // all agents or none (checked by the launcher)
                 P::prepare(d, w);
@@ -1702,6 +1964,8 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
     }
     P::prepare(d, w);
     __syncwarp();                  // every lane has read its logits before the tile is reused
+    if constexpr (CRITIC && !EPISODES)
+        run_critics<P>(*cs, Wc, d, w, s_warp, lane, rows, ln_eps, net_flags, cs->final_values, 0, w0, n);   // V after the last step
     write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi);   // the slot is this warp's observation tile
     if (active) {
 #pragma unroll
@@ -1747,6 +2011,20 @@ __global__ void __launch_bounds__(mlp_block_warps<P, 64, 5>() * 32)
     mlp_rollout<P, 64, true, true, true>(ma.c.e.p, &ma.c.e, &ma.c.c, ma.eps, ma.net_flags);
 }
 
+// MAPPO's actor with its centralized critic (MlpCriticArgs); mpe_critic.cu instantiates them (critic_kernel)
+template <class P>
+__global__ void __launch_bounds__(critic_block_warps<P, false>() * 32)
+    mpe_policy_mappo_critic_kernel(const __grid_constant__ MlpCriticArgs ca) {
+    mlp_rollout<P, 64, false, true, true, false, true>(ca.m.c.p, nullptr, &ca.m.c.c, ca.m.eps, ca.m.net_flags, nullptr, &ca.v);
+}
+
+template <class P>
+__global__ void __launch_bounds__(critic_block_warps<P, true>() * 32)
+    mpe_policy_mappo_critic_episode_kernel(const __grid_constant__ MlpCriticEpisodeArgs ca) {
+    mlp_rollout<P, 64, true, true, true, false, true>(ca.m.c.e.p, &ca.m.c.e, &ca.m.c.c, ca.m.eps, ca.m.net_flags, nullptr,
+                                                      &ca.v);
+}
+
 template <class P>
 __global__ void __launch_bounds__(gru_block_warps<P>() * 32) mpe_policy_gru_kernel(const __grid_constant__ MlpGruArgs ga) {
     mlp_rollout<P, 64, false, true, true, true>(ga.m.c.p, nullptr, &ga.m.c.c, ga.m.eps, ga.m.net_flags, &ga.g);
@@ -1763,6 +2041,9 @@ __global__ void __launch_bounds__(gru_block_warps<P>() * 32)
 // took half as long again to build.
 template <class P>
 const void *gru_kernel(int episodes);
+// The critic's two kernels of program P (episodes = 0, 1), instantiated by mpe_critic.cu in the same way
+template <class P>
+const void *critic_kernel(int episodes);
 
 #ifdef MPE_KERNEL_TEMPLATES_ONLY   // mpe_gru.cu: the device code above, without the programs and the C ABI below
 }  // namespace mpe
@@ -1951,9 +2232,10 @@ struct Program {
     int policy_weight_floats[2];
     // the same with the two-hidden-layer actor on the tensor cores, by form (episodes | kind << 1) and H = 32 / 64: the
     // kernel and its warps per block at most (mlp_block_warps); null for MAPPO's forms at H = 32.  Forms 6 and 7 are
-    // the recurrent actor's (gru_block_warps, H = 64 only), whose one shared weight set takes gru_weight_floats.
-    struct { const void *fn; int warps; } mlp[kMlpForms + 2][2];
-    int mlp_weight_floats[2], mlp_warp_floats[2], gru_weight_floats;
+    // the recurrent actor's (gru_block_warps, H = 64 only), whose one shared weight set takes gru_weight_floats; forms
+    // 8 and 9 MAPPO's actor with its critic (critic_block_warps, H = 64 only), each critic taking critic_floats more.
+    struct { const void *fn; int warps; } mlp[kMlpForms + 4][2];
+    int mlp_weight_floats[2], mlp_warp_floats[2], gru_weight_floats, critic_floats;
     int mlp_explore_stride;           // Philox blocks per (step, agent) of its exploration noise
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
     int rollout_smem;   // dynamic shared memory per WARP of the rollout kernel
@@ -2006,6 +2288,11 @@ static Program make_program() {
         p.mlp[kMlpForms][1] = {gru_kernel<P>(0), gru_block_warps<P>()};
         p.mlp[kMlpForms + 1][1] = {gru_kernel<P>(1), gru_block_warps<P>()};
         p.gru_weight_floats = GruShape<P>::kWeightFloats;
+    }
+    if constexpr (critic_built<P>()) {
+        p.mlp[kMlpForms + 2][1] = {critic_kernel<P>(0), critic_block_warps<P, false>()};
+        p.mlp[kMlpForms + 3][1] = {critic_kernel<P>(1), critic_block_warps<P, true>()};
+        p.critic_floats = CriticShape<P>::kFloats;
     }
     p.smem_bytes = Shape<P>::kWarpBytes;  // per warp
     p.A = P::A; p.L = P::L; p.NS = P::NS; p.DIMC = P::DIMC; p.INFO = P::INFO; p.G = P::G;
@@ -2143,6 +2430,10 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
                     CUDA_TRY(cudaFuncSetAttribute(prog->mlp[f][k].fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                   ((f < kMlpForms ? prog->mlp_weight_floats[k] : prog->gru_weight_floats) +
                                                    prog->mlp_warp_floats[k] * prog->mlp[f][k].warps) * 4));
+        for (int f = kMlpForms + 2; f < kMlpForms + 4; ++f)   // the critic's two: their size depends on the critics'
+            if (prog->mlp[f][1].fn)                            // count, so they may take the whole opt-in
+                CUDA_TRY(cudaFuncSetAttribute(prog->mlp[f][1].fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              kMlpSmemBytes));
         if (prog->rollout_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->rollout_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->rollout_smem * max_warps_per_block(prog->rollout_smem)));
@@ -2499,10 +2790,12 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
 // The arguments of the six two-hidden-layer rollout entry points, filled by name (several neighbours share a type).
 // form: episodes | kind << 1 (kMlpForms).  T is the episode length (n_steps in the single-episode forms); a record the
 // form does not have is null.  net_flags and ln_eps are MAPPO's (MlpMappoArgs); forms 6 and 7 (kMlpForms + episodes)
-// are the recurrent actor's, whose w[j] hold the shared set's pointer for every agent and gru its MlpGruState.
+// are the recurrent actor's, whose w[j] hold the shared set's pointer for every agent and gru its MlpGruState; forms 8
+// and 9 (kMlpForms + 2 + episodes) MAPPO's actor with critic, the critics' count, weights and value records.
 struct MlpCall {
     int form;
     MlpGruState gru;
+    MlpCriticState critic;
     uint32_t net_flags;
     float ln_eps;
     void *pv;
@@ -2523,7 +2816,7 @@ struct MlpCall {
 };
 
 static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
-    static const char *const kName[kMlpForms + 2][2] = {   // the NVTX range, the launch's error context
+    static const char *const kName[kMlpForms + 4][2] = {   // the NVTX range, the launch's error context
         {"mpe_rollout_policy_mlp", "cudaLaunchKernelExC(rollout_policy_mlp)"},
         {"mpe_rollout_policy_mlp_episodes", "cudaLaunchKernelExC(rollout_policy_mlp_episodes)"},
         {"mpe_rollout_policy_mlp_categorical", "cudaLaunchKernelExC(rollout_policy_mlp_categorical)"},
@@ -2531,8 +2824,11 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
         {"mpe_rollout_policy_mappo", "cudaLaunchKernelExC(rollout_policy_mappo)"},
         {"mpe_rollout_policy_mappo_episodes", "cudaLaunchKernelExC(rollout_policy_mappo_episodes)"},
         {"mpe_rollout_policy_gru", "cudaLaunchKernelExC(rollout_policy_gru)"},
-        {"mpe_rollout_policy_gru_episodes", "cudaLaunchKernelExC(rollout_policy_gru_episodes)"}};
-    const bool episodes = c.form & 1, categorical = c.form >= 2, mappo = c.form >= 4, gru = c.form >= kMlpForms;
+        {"mpe_rollout_policy_gru_episodes", "cudaLaunchKernelExC(rollout_policy_gru_episodes)"},
+        {"mpe_rollout_policy_mappo_critic", "cudaLaunchKernelExC(rollout_policy_mappo_critic)"},
+        {"mpe_rollout_policy_mappo_critic_episodes", "cudaLaunchKernelExC(rollout_policy_mappo_critic_episodes)"}};
+    const bool episodes = c.form & 1, categorical = c.form >= 2, mappo = c.form >= 4;
+    const bool gru = c.form == kMlpForms || c.form == kMlpForms + 1, critic = c.form >= kMlpForms + 2;
     const bool no_weights = !c.w[0] || !c.w[1] || !c.w[2] || !c.w[3] || !c.w[4] || !c.w[5];
     // the single-episode forms refuse a negative n_steps and null weight arrays before anything else, the episode forms
     // after the device, program and length checks
@@ -2540,6 +2836,14 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     if (h->device < 0) return MPE_ERR_NO_DEVICE;
     const int k = c.hidden == 32 ? 0 : (c.hidden == 64 ? 1 : -1);
     if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || h->prog->mlp[c.form][k].fn == nullptr) return MPE_ERR_UNSUPPORTED;
+    // 1 (shared) or A critics, whose weights must leave room for a warp's tiles next to the actor's
+    int critic_cap = 0;
+    if (critic) {
+        if (c.critic.count != 1 && c.critic.count != h->prog->A) return MPE_ERR_BAD_ARG;
+        critic_cap = (kMlpSmemBytes / 4 - h->prog->mlp_weight_floats[k] - c.critic.count * h->prog->critic_floats) /
+                     h->prog->mlp_warp_floats[k];
+        if (critic_cap < 1) return MPE_ERR_UNSUPPORTED;
+    }
     if (c.flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
     // unknown network flags, or an eps that is negative, NaN or infinite
     if (mappo && ((c.net_flags & ~(kMappoFeatureNorm | kMappoTanh)) || !(c.ln_eps >= 0.0f && c.ln_eps <= 3.4e38f)))
@@ -2554,6 +2858,13 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     if (gru && (!ok4(c.gru.w_ih) || !ok4(c.gru.b_ih) || !ok4(c.gru.w_hh) || !ok4(c.gru.b_hh) || !ok8(c.gru.h) ||
                 (c.gru.h_rec != nullptr && !ok8(c.gru.h_rec))))
         return MPE_ERR_BAD_ARG;
+    if (critic) {
+        if (!ok4(c.critic.values) || !ok4(c.critic.final_values)) return MPE_ERR_BAD_ARG;
+        for (int q = 0; q < c.critic.count; ++q)
+            if (!ok4(c.critic.w1[q]) || !ok4(c.critic.b1[q]) || !ok4(c.critic.w2[q]) || !ok4(c.critic.b2[q]) ||
+                !ok4(c.critic.w3[q]) || !ok4(c.critic.b3[q]))
+                return MPE_ERR_BAD_ARG;
+    }
     NvtxRange range(kName[c.form][0]);
     MlpCategoricalRecords cr{};
     if (categorical) {
@@ -2596,15 +2907,19 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     MlpMappoEpisodeArgs mea{cea, c.ln_eps, c.net_flags};
     MlpGruArgs ga{ma, c.gru};
     MlpGruEpisodeArgs gea{mea, c.gru};
-    void *const form_args[kMlpForms + 2] = {&pa, &ea, &ca, &cea, &ma, &mea, &ga, &gea};
+    MlpCriticArgs va{ma, c.critic};
+    MlpCriticEpisodeArgs vea{mea, c.critic};
+    void *const form_args[kMlpForms + 4] = {&pa, &ea, &ca, &cea, &ma, &mea, &ga, &gea, &va, &vea};
     const void *const fn = h->prog->mlp[c.form][k].fn;
-    const int cap = h->prog->mlp[c.form][k].warps;
+    int cap = h->prog->mlp[c.form][k].warps;
+    if (critic && critic_cap < cap) cap = critic_cap;   // per-agent critics leave fewer warps than the shared one
     // every block stages all agents' weights once, so blocks are as large as possible while every SM still gets work
     const int64_t warps = (h->n + 31) / 32;
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
     if (wpb > cap) wpb = cap;
-    const int weight_floats = gru ? h->prog->gru_weight_floats : h->prog->mlp_weight_floats[k];
+    const int weight_floats = gru ? h->prog->gru_weight_floats
+                                  : h->prog->mlp_weight_floats[k] + (critic ? c.critic.count * h->prog->critic_floats : 0);
     return launch_persistent(h, fn, warps, wpb, static_cast<size_t>(weight_floats) * 4,
                              static_cast<size_t>(h->prog->mlp_warp_floats[k]) * 4, form_args[c.form], c.stream,
                              kName[c.form][1]);
@@ -2779,6 +3094,61 @@ extern "C" int mpe_rollout_policy_gru_episodes(
     c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
     c.net_flags = net_flags; c.ln_eps = ln_eps;
     return rollout_policy_gru(h, c, {w1, b1, w2, b2, w_ih, b_ih, w_hh, b_hh, w3, b3}, rnn_state, rnn_state_record);
+}
+
+// The critics' six weight arrays (W1, b1, W2, b2, W3, b3: critic_count pointers each) and value records -> c.critic
+static int rollout_policy_critic(mpe_handle h, MlpCall &c, int32_t critic_count, const float *const *const (&cw)[6],
+                                 float *values, float *final_values) {
+    c.critic.count = critic_count;
+    c.critic.values = values;
+    c.critic.final_values = final_values;
+    const float **dst[6] = {c.critic.w1, c.critic.b1, c.critic.w2, c.critic.b2, c.critic.w3, c.critic.b3};
+    for (int j = 0; j < 6; ++j)
+        for (int q = 0; q < critic_count && q < kMaxA; ++q) dst[j][q] = cw[j] ? cw[j][q] : nullptr;
+    return rollout_policy_mlp(h, c);
+}
+
+extern "C" int mpe_rollout_policy_mappo_critic(
+    mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal, const float *const *w1_n,
+    const float *const *b1_n, const float *const *w2_n, const float *const *b2_n, const float *const *w3_n,
+    const float *const *b3_n, int32_t hidden, int32_t n_steps, int32_t explore, uint64_t explore_seed,
+    uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n, float *rew_sum, float *rew_steps, float *logp_steps,
+    int32_t *const *act_index_record_n, float *const *obs_record_n, uint32_t net_flags, float ln_eps, int32_t critic_count,
+    const float *const *cw1, const float *const *cb1, const float *const *cw2, const float *const *cb2,
+    const float *const *cw3, const float *const *cb3, float *values, float *final_values, uint8_t *done, uint32_t flags,
+    void *stream) {
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.w[0] = w1_n; c.w[1] = b1_n; c.w[2] = w2_n; c.w[3] = b2_n; c.w[4] = w3_n; c.w[5] = b3_n;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = kMlpForms + 2; c.T = n_steps; c.episodes = 1; c.rew = rew_sum;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    c.net_flags = net_flags; c.ln_eps = ln_eps;
+    return rollout_policy_critic(h, c, critic_count, {cw1, cb1, cw2, cb2, cw3, cb3}, values, final_values);
+}
+
+extern "C" int mpe_rollout_policy_mappo_critic_episodes(
+    mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal, const float *const *w1_n, const float *const *b1_n,
+    const float *const *w2_n, const float *const *b2_n, const float *const *w3_n, const float *const *b3_n, int32_t hidden,
+    int32_t episode_length, int32_t n_episodes, int32_t explore, uint64_t explore_seed, uint64_t explore_epoch,
+    uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew, float *rew_steps,
+    float *logp_steps, int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n,
+    uint32_t net_flags, float ln_eps, int32_t critic_count, const float *const *cw1, const float *const *cb1,
+    const float *const *cw2, const float *const *cb2, const float *const *cw3, const float *const *cb3, float *values,
+    float *final_values, uint8_t *done, uint32_t flags, void *stream) {
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.w[0] = w1_n; c.w[1] = b1_n; c.w[2] = w2_n; c.w[3] = b2_n; c.w[4] = w3_n; c.w[5] = b3_n;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = kMlpForms + 3; c.T = episode_length; c.episodes = n_episodes; c.rew = ep_rew;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
+    c.net_flags = net_flags; c.ln_eps = ln_eps;
+    return rollout_policy_critic(h, c, critic_count, {cw1, cb1, cw2, cb2, cw3, cb3}, values, final_values);
 }
 
 // adjacent (dst, src, bytes) copies with equal small gaps on both sides are issued as one DMA

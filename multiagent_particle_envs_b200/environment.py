@@ -245,7 +245,7 @@ class MultiAgentEnv(_Env):
 
     def rollout_policy(self, policies, n_steps, record_actions=False, per_step_rewards=False, record_observations=False,
                        explore_seed=None, episode_length=None, action_mode="softmax", record_log_probs=False,
-                       rnn_states=None, record_rnn_states=False):
+                       rnn_states=None, record_rnn_states=False, critic=None):
         """T closed-loop steps in ONE kernel launch with the actors inside the kernel.
 
         One hidden layer (mpe_rollout_policy, fp32): agent i acts with softmax(W2_i relu(W1_i obs_i + b1_i) + b2_i).
@@ -321,7 +321,23 @@ class MultiAgentEnv(_Env):
         rnn_states continues from.  record_rnn_states=True returns extras["rnn_states"], a float32 [T, n, N, 64] tensor
         of the h each step's actor consumed (MAPPO's buffer rnn_states[t]; zero at every episode's first step), else
         None -- T * n * N * 256 bytes.  Records, sampling, log-probabilities, episodes and epochs are the categorical
-        mode's.  rnn_states or record_rnn_states with any other actor raise ValueError."""
+        mode's.  rnn_states or record_rnn_states with any other actor raise ValueError.
+
+        critic (MAPPO's MLP actor only, mpe_rollout_policy_mappo_critic[_episodes]) evaluates MAPPO's centralized critic
+        in the same launch: R_Critic with use_centralized_V and no recurrence, `nn.Sequential([LayerNorm(D)], Linear(D,
+        64), Act, LayerNorm(64), Linear(64, 64), Act, LayerNorm(64), Linear(64, 1))`, whose input is share_obs -- every
+        agent's raw observation concatenated in agent order, D = sum of obs_dim_i.  Its Act, input LayerNorm and eps
+        must be the actors' (ValueError); mappo_critic_params checks and folds it as the actor is folded.  Pass one
+        module (or [critic] * n, the same object: share_policy), whose value is computed once per world and step and
+        written for every agent, or a list of n distinct modules (per-agent critics, each evaluating the same input).
+        extras["values"] is then a float32 [T, n, N] tensor, V of the observations step t's actors acted on (MAPPO's
+        value_preds[t]), and extras["final_values"] a float32 [n, N] tensor, V after the last step (MAPPO's next_value);
+        with episode_length it is [E, n, N], V of each episode's final observation, before its reset.  Everything else
+        is bit-identical to the same call without a critic.  A critic with any other actor or with action_mode="softmax"
+        raises NotImplementedError, a malformed one or a list of length other than 1 or n ValueError.  simple_spread N=6
+        and simple_tag 6+2 have no critic kernel, and per-agent critics do not fit in shared memory next to the actors
+        for simple_spread N=4 and 5, simple_tag 3+1 and 4+2 and simple_adversary with 4 agents: those raise MpeError
+        before anything runs."""
         import torch
         world = self.world
         if action_mode not in ("softmax", "categorical"):
@@ -338,6 +354,13 @@ class MultiAgentEnv(_Env):
                                            or int(n_steps) % int(episode_length) != 0):
             raise ValueError("rollout_policy: n_steps (%d) must be a positive multiple of episode_length (%d)"
                              % (int(n_steps), int(episode_length)))
+        if critic is not None:
+            if any(_is_recurrent(p) for p in policies) or not any(_has_layer_norm(p) for p in policies):
+                raise NotImplementedError("rollout_policy: critic needs MAPPO's MLP actor (LayerNorm layers); the "
+                                          "two-hidden-layer and one-hidden-layer actors have no critic, and rMAPPO's "
+                                          "critic is recurrent")
+            if action_mode != "categorical":
+                raise NotImplementedError("rollout_policy: critic needs action_mode='categorical'")
         if any(_is_recurrent(p) for p in policies):
             if action_mode != "categorical":
                 raise NotImplementedError("rollout_policy: MAPPO's recurrent actor has action_mode='categorical' only")
@@ -358,7 +381,8 @@ class MultiAgentEnv(_Env):
                 raise NotImplementedError("rollout_policy: MAPPO's actor is built for hidden width %d only; got %s"
                                           % (MAPPO_HIDDEN, sorted(_mappo_hidden_widths(policies))))
             return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
-                                            explore_seed, episode_length, True, record_log_probs, mappo=True)
+                                            explore_seed, episode_length, True, record_log_probs, mappo=True,
+                                            critic=critic)
         if any(_has_two_hidden_layers(p) for p in policies):
             return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
                                             explore_seed, episode_length, action_mode == "categorical", record_log_probs)
@@ -404,7 +428,8 @@ class MultiAgentEnv(_Env):
         return list(out.obs), list(out.rew_list), list(out.done_list), info_n, {"actions": actions, "rewards": rew_steps}
 
     def _rollout_policy_mlp(self, policies, n_steps, record_actions, per_step_rewards, record_observations, explore_seed,
-                            episode_length=None, categorical=False, record_log_probs=False, mappo=False, gru=None):
+                            episode_length=None, categorical=False, record_log_probs=False, mappo=False, gru=None,
+                            critic=None):
         import torch
         world = self.world
         nw = world.bind()
@@ -435,6 +460,14 @@ class MultiAgentEnv(_Env):
             params, tanh, feature_norm, eps = mappo_actor_params(policies, nw.obs_dims, nw.act_dims)
             hidden = MAPPO_HIDDEN
             net = ((_lib.MAPPO_FEATURE_NORM if feature_norm else 0) | (_lib.MAPPO_TANH if tanh else 0), eps)
+            if critic is not None:
+                cparams, ctanh, cfn, ceps = mappo_critic_params(critic, nw.obs_dims)
+                if (ctanh, cfn, ceps) != (tanh, feature_norm, eps):
+                    raise ValueError("rollout_policy: the critic must use the actors' activation, input LayerNorm and "
+                                     "eps (%s, %s, %g); got (%s, %s, %g)"
+                                     % ("Tanh" if tanh else "ReLU", feature_norm, eps, "Tanh" if ctanh else "ReLU", cfn,
+                                        ceps))
+                nw.require_critic(len(cparams))   # a program without the kernel, or critics that do not fit
         else:
             params, hidden = mlp_actor_params(policies, nw.obs_dims, nw.act_dims)
             net = None
@@ -445,6 +478,13 @@ class MultiAgentEnv(_Env):
             w_ptrs = [_lib.ptr_array([keep[i][j].data_ptr() for i in range(self.n)]) for j in range(6)]
         out = nw.out if self.reuse_buffers else nw.new_outputs()
         dev = dict(dtype=torch.float32, device=nw.device)
+        crit = None
+        if critic is not None:
+            ckeep = [[t.to(device=nw.device, dtype=torch.float32).contiguous() for t in p] for p in cparams]
+            cw_ptrs = [_lib.ptr_array([ckeep[k][j].data_ptr() for k in range(len(ckeep))]) for j in range(6)]
+            E = 1 if episode_length is None else T // int(episode_length)
+            final_shape = (self.n, N) if episode_length is None else (E, self.n, N)
+            crit = (len(ckeep), cw_ptrs, torch.empty((T, self.n, N), **dev), torch.empty(final_shape, **dev))
         rew_steps = torch.empty((T, self.n, N), **dev) if per_step_rewards else None
         if categorical:   # int32 [T, N, n_sub_i]: movement if movable, then utterance if it speaks
             n_sub = [int(bool(nw.desc.agent_movable[i])) + int(not nw.desc.agent_silent[i]) for i in range(self.n)]
@@ -468,9 +508,11 @@ class MultiAgentEnv(_Env):
                               rew_steps=rew_steps, act_rec_ptrs=act_ptrs, obs_rec_ptrs=obs_ptrs,
                               final_obs_ptrs=_lib.ptr_array([o.data_ptr() for o in final]) if final is not None else None,
                               logp_steps=log_probs, ep_rew=ep_rew, explore_seed=seed, explore_epoch=self.explore_epoch,
-                              mappo=net, gru=rnn)
+                              mappo=net, gru=rnn, critic=crit)
         if rnn is not None:
             extras["final_rnn_states"], extras["rnn_states"] = rnn
+        if crit is not None:
+            extras["values"], extras["final_values"] = crit[2], crit[3]
         if episode_length is None:
             reward_n = list(out.rew_list)
         else:
@@ -885,6 +927,35 @@ def mappo_actor_params(policies, obs_dims, act_dims=None):
     if len(eps) != 1:
         raise ValueError("every LayerNorm must have the same eps; got %s" % sorted(eps))
     return params, acts.pop() is nn.Tanh, feature_norms.pop(), eps.pop()
+
+
+# ---- MAPPO's centralized critic (R_Critic with use_centralized_V, non-recurrent) -------------------------------------
+_CRITIC_SHAPE = ("nn.Sequential([LayerNorm(D)], Linear(D, 64), Act, LayerNorm(64), Linear(64, 64), Act, LayerNorm(64), "
+                 "Linear(64, 1)) with Act = ReLU() or Tanh() and D the sum of the agents' observation sizes")
+
+
+def mappo_critic_params(critic, obs_dims):
+    """MAPPO's centralized critic -> (params, tanh, feature_norm, eps), or ValueError.  critic is one module (a shared
+    critic), a list of one, or a list of len(obs_dims) modules; a list whose entries are all the same object is one
+    shared critic ([critic] * n, MAPPO's share_policy), any other list of len(obs_dims) per-agent critics.  Each must be
+        [LayerNorm(D)], Linear(D, 64), Act, LayerNorm(64), Linear(64, 64), Act, LayerNorm(64), Linear(64, 1)
+    (D = sum(obs_dims), the width of share_obs) under the rules of mappo_actor_params, with one activation, input
+    LayerNorm and eps for all.  params: one (W1', b1', W2', b2', W3', b3') per critic in float64, each LayerNorm's
+    affine folded into the Linear after it as mappo_actor_params folds the actor's.  No device is needed."""
+    import torch
+    n, D = len(obs_dims), int(sum(obs_dims))
+    if isinstance(critic, torch.nn.Module):
+        critics = [critic]
+    elif isinstance(critic, (list, tuple)) and len(critic) in (1, n):
+        critics = [critic[0]] if all(c is critic[0] for c in critic) else list(critic)
+    else:
+        raise ValueError("critic must be one module, or a list of 1 or %d modules; got %s"
+                         % (n, "a list of %d" % len(critic) if isinstance(critic, (list, tuple))
+                            else type(critic).__name__))
+    try:
+        return mappo_actor_params(critics, [D] * len(critics), [1] * len(critics))
+    except ValueError as e:
+        raise ValueError("critic must be %s: %s" % (_CRITIC_SHAPE, e)) from None
 
 
 # ---- MAPPO's recurrent actor (R_Actor with use_recurrent_policy, recurrent_N = 1, share_policy) -----------------------

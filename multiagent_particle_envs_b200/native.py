@@ -291,9 +291,19 @@ class NativeWorld(ShapeHandle):
         if rc == _lib.ERR_UNSUPPORTED:
             check(rc, "mpe_rollout_policy_gru")
 
+    def require_critic(self, count):
+        """MpeError unless the library has MAPPO's critic kernel for this program and `count` critics (1 or A) fit in
+        shared memory next to the actor.  As in require_gru_actor, the probe stops at the null state."""
+        none = _lib.ptr_array([256] * self.n_agents)
+        rc = self.lib.mpe_rollout_policy_mappo_critic(self.handle, None, None, None, None, *([none] * 6), 64, 0, 0, 0, 0,
+                                                      0, None, None, None, None, None, None, 0, 0.0, int(count),
+                                                      *([none] * 6), None, None, None, 0, self._stream())
+        if rc == _lib.ERR_UNSUPPORTED:
+            check(rc, "mpe_rollout_policy_mappo_critic")
+
     def rollout_policy_mlp(self, w_ptrs, hidden, n_steps, out=None, flags=0, *, episode_length=None, categorical=False,
                            rew_steps=None, act_rec_ptrs=None, obs_rec_ptrs=None, final_obs_ptrs=None, logp_steps=None,
-                           ep_rew=None, explore_seed=None, explore_epoch=0, mappo=None, gru=None):
+                           ep_rew=None, explore_seed=None, explore_epoch=0, mappo=None, gru=None, critic=None):
         """n_steps fused steps in ONE launch with every agent's two-hidden-layer actor evaluated on the tensor cores
         (mpe_rollout_policy_mlp); w_ptrs: the six pointer arrays (W1, b1, W2, b2, W3, b3), one device pointer per
         agent each.  explore_seed (not None) switches the Gumbel-softmax sampling on.
@@ -315,11 +325,18 @@ class NativeWorld(ShapeHandle):
         then the ten device pointers of its one shared folded weight set (W1, b1, W2, b2, W_ih, b_ih, W_hh, b_hh, W3,
         b3; environment.rmappo_actor_params); rnn_state, a float32 [A, N, 64] CUDA tensor, holds the initial hidden
         state and receives the final one, and rnn_record (float32 [n_steps, A, N, 64], or None) the h each step
-        consumed."""
+        consumed.
+
+        critic=(count, cw_ptrs, values, final_values) with mappo (mpe_rollout_policy_mappo_critic[_episodes]): MAPPO's
+        centralized critic next to the actor.  count is 1 (one shared critic) or A; cw_ptrs the six pointer arrays of
+        the folded critics (environment.mappo_critic_params), count device pointers each; values a float32 [n_steps, A,
+        N] and final_values a float32 [A, N] ([episodes, A, N]) CUDA tensor."""
         out = out or self.out
         episodes = episode_length is not None
         if gru is not None and mappo is None:
             raise ValueError("rollout_policy_mlp: the recurrent actor is MAPPO's (pass mappo=(net_flags, eps))")
+        if critic is not None and (mappo is None or gru is not None):
+            raise ValueError("rollout_policy_mlp: the critic runs next to MAPPO's MLP actor (pass mappo, not gru)")
         if mappo is not None and not categorical:
             raise ValueError("rollout_policy_mlp: the MAPPO actor has the categorical form only")
         if episodes and self.torch.cuda.is_current_stream_capturing():
@@ -331,7 +348,11 @@ class NativeWorld(ShapeHandle):
         rew_ptr = rew_steps.data_ptr() if rew_steps is not None else None
         logp = (logp_steps.data_ptr() if logp_steps is not None else None,) if categorical else ()
         rnn = ()
-        if gru is not None:
+        if critic is not None:
+            name = "mpe_rollout_policy_mappo_critic" + ("_episodes" if episodes else "")
+            net = (int(mappo[0]), float(mappo[1]), int(critic[0]), *critic[1], critic[2].data_ptr(),
+                   critic[3].data_ptr())
+        elif gru is not None:
             name = "mpe_rollout_policy_gru" + ("_episodes" if episodes else "")
             net = (int(mappo[0]), float(mappo[1]))
             rnn = (gru[0].data_ptr(), gru[1].data_ptr() if gru[1] is not None else None)

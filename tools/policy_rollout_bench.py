@@ -14,6 +14,12 @@
       --actor rmappo: MAPPO's recurrent actor, one (base, gru, norm, head) tuple shared by every agent (base = the MAPPO
       actor without its last Linear, nn.GRU(64, 64), LayerNorm(64), Linear(64, act_dim); mpe_rollout_policy_gru), with
       the same implied options and --tanh / --feature-norm;
+      --critic shared|separated (with --actor mappo): MAPPO's centralized critic ([LayerNorm(D)] - Linear(D, 64) - Act -
+      LayerNorm - Linear - Act - LayerNorm - Linear(64, 1) on every agent's observation concatenated, one shared
+      module or one per agent) evaluated in the same launch (critic=..., mpe_rollout_policy_mappo_critic), against
+      what a trainer does without it: the same call with record_observations=True, then the torch critic over the
+      concatenated records ([T N, D]) and the final observations ([N, D]), at torch's default float32 matmul
+      precision.  Only these two arms are timed ("in_kernel_critic", "kernel_then_torch_critic");
   (b) the same actors as torch modules + env.step, all captured in one CUDA graph (rollout.GraphedRollout); with
       --categorical the graphed policy takes argmax(logits - log(-log u)) per sub-space, its one_hot and
       log_softmax(logits).gather(k) for the log-probabilities.  With --actor rmappo the graphed policy evaluates the
@@ -54,6 +60,52 @@ def card_info():
         return {"error": "nvidia-smi: %s" % e}
 
 
+def time_critic(args, env, mods, kw, res, e0, e1):
+    """(a) the rollout with MAPPO's critic in the kernel, (b) the rollout recording observations, then the torch critic
+    over the concatenated records and the final observations; device time per step of each"""
+    import torch
+    nn = torch.nn
+    nw = env.world.native
+    n, T, H, D = args.num_envs, args.steps, args.hidden, sum(nw.obs_dims)
+    Act = nn.Tanh if args.tanh else nn.ReLU
+    count = 1 if args.critic == "shared" else len(nw.obs_dims)
+    crits = [nn.Sequential(*(([nn.LayerNorm(D)] if args.feature_norm else []) +
+                             [nn.Linear(D, H), Act(), nn.LayerNorm(H), nn.Linear(H, H), Act(), nn.LayerNorm(H),
+                              nn.Linear(H, 1)])).to(mods[0][0].weight.device) for _ in range(count)]
+    critic = crits[0] if count == 1 else crits
+
+    def in_kernel():
+        env.rollout_policy(mods, T, critic=critic, **kw)
+
+    def kernel_then_torch():
+        obs_n, _, _, _, ex = env.rollout_policy(mods, T, record_observations=True, **kw)
+        x = torch.cat(ex["observations"], -1).reshape(T * n, D)
+        final = torch.cat(list(obs_n), -1)
+        with torch.no_grad():
+            for c in crits:
+                c(x)
+                c(final)
+
+    def timed(fn):
+        for _ in range(2):
+            fn()
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(args.reps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / 1e3 / (args.reps * T)
+
+    res["config"].update(torch_float32_matmul_precision=torch.get_float32_matmul_precision())
+    sa, sb = timed(in_kernel), timed(kernel_then_torch)
+    res["in_kernel_critic"] = {"us_per_step": 1e6 * sa, "env_steps_per_sec": n / sa}
+    res["kernel_then_torch_critic"] = {"us_per_step": 1e6 * sb, "env_steps_per_sec": n / sb}
+    res["speedup"] = sb / sa
+    res["card"] = card_info()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scenario", default="simple_spread")
@@ -72,7 +124,12 @@ def main():
                          "--categorical)")
     ap.add_argument("--tanh", action="store_true", help="MAPPO's actor with Tanh instead of ReLU")
     ap.add_argument("--feature-norm", action="store_true", help="MAPPO's actor with the input LayerNorm")
+    ap.add_argument("--critic", choices=("shared", "separated"),
+                    help="time MAPPO's centralized critic in-kernel against the torch critic after the rollout "
+                         "(--actor mappo)")
     args = ap.parse_args()
+    if args.critic and args.actor != "mappo":
+        ap.error("--critic needs --actor mappo")
     if args.actor in ("mappo", "rmappo"):
         args.layers, args.categorical = 3, True
     elif args.tanh or args.feature_norm:
@@ -145,6 +202,10 @@ def main():
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / 1e3 / (args.reps * T)
 
+    if args.critic:
+        res["config"].update(critic=args.critic)
+        print(json.dumps(time_critic(args, env, mods, kw, res, e0, e1)))
+        return
     sec = time_in_kernel(mods)
     res["in_kernel"] = {"us_per_step": 1e6 * sec, "env_steps_per_sec": n / sec}
     if maddpg_mods is not None:   # the MADDPG categorical kernel on the same env, same sizes
