@@ -404,6 +404,32 @@ MPE_API int mpe_rollout_policy_mappo_critic_episodes(
     const float *const *cw2_n, const float *const *cb2_n, const float *const *cw3_n, const float *const *cb3_n,
     float *values_dev, float *final_values_dev, uint8_t *done_dev, uint32_t flags, void *stream);
 
+/* rMAPPO's recurrent centralized critic (R_Critic with use_recurrent_policy, recurrent_N = 1, use_centralized_V,
+ * hidden width 64), ONE weight set shared by every agent, run as a kernel of its own after
+ * mpe_rollout_policy_gru[_episodes] on the same stream, over that rollout's observation records:
+ *     x = [LN(D)] -> Linear(D, 64) -> act -> LN(64) -> Linear(64, 64) -> act -> LN(64),  h' = GRU(x, h)
+ *     V = w3 LN(h') + b3
+ * on share_obs, every agent's raw observation concatenated in agent order (D = sum of obs_dim_i), folded as
+ * mpe_rollout_policy_gru's actor (w1 [64][D], w3 [1][64], b3 [1]; the others as the actor's).  obs_record_n[i]
+ * ([T][N][obs_dim_i]) is the rollout's observation record, final_obs_n[i] ([E][N][obs_dim_i]) its final observations:
+ * the returned observations for one episode (E = 1), the final-observation record in the episode form.  Per step t:
+ * values_dev[t][a][w] = V (the same for every agent a, [T][A][N]) and h = h'.  episode_length L = 0: one episode of
+ * n_steps, h starting from rnn_state_dev ([N][64], read) and final_values_dev[0] ([1][A][N]) = V(final_obs_n, h') after
+ * the last step.  L > 0: n_steps / L = E episodes, each starting from h = 0 (rnn_state_dev is not read), and
+ * final_values_dev[e] ([E][A][N]) is V of episode e's final observation, taken from the h after its last step.
+ * rnn_state_dev receives the h after the last step in both forms; rnn_state_record_dev ([T][N][64], or NULL) the h
+ * each step consumed.  Checked in this order: MPE_ERR_BAD_ARG for a null handle or n_steps < 0; MPE_ERR_NO_DEVICE;
+ * MPE_ERR_UNSUPPORTED for a program without the kernel (built for simple, simple_spread N = 2..6 and
+ * simple_reference); MPE_ERR_BAD_ARG for episode_length < 0, or > 0 without dividing n_steps >= 1; for unknown
+ * net_flags or an eps that is negative, NaN or infinite; for a null or misaligned weight, state, record, value array,
+ * observation array or agent observation pointer (values_dev and obs_record_n may be null when n_steps is 0). */
+MPE_API int mpe_critic_gru(mpe_handle h, const float *const *obs_record_n, const float *const *final_obs_n,
+                           int32_t n_steps, int32_t episode_length, const float *w1, const float *b1, const float *w2,
+                           const float *b2, const float *w_ih, const float *b_ih, const float *w_hh,
+                           const float *b_hh, const float *w3, const float *b3, float *rnn_state_dev,
+                           float *rnn_state_record_dev, float *values_dev, float *final_values_dev,
+                           uint32_t net_flags, float ln_eps, void *stream);
+
 /* Same step for a caller that holds HOST buffers (what the reference's callers hold):
  * act_n_host[i] -> (async H2D into act_n_dev[i]) -> mpe_step -> (async D2H) obs_n_host[i],
  * rew_host, done_host, all ordered on `stream`.  Host buffers should be pinned for the copies

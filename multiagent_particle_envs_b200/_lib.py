@@ -136,6 +136,8 @@ _SIGNATURES = {
                                                                 _P, _P, _PP, _PP, _PP, ctypes.c_uint32, ctypes.c_float,
                                                                 ctypes.c_int32, _PP, _PP, _PP, _PP, _PP, _PP, _P, _P, _P,
                                                                 ctypes.c_uint32, _P]),
+    "mpe_critic_gru": (ctypes.c_int, [_P, _PP, _PP, ctypes.c_int32, ctypes.c_int32] + [_P] * 10 +
+                       [_P, _P, _P, _P, ctypes.c_uint32, ctypes.c_float, _P]),
     "mpe_step_host": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _P, _P, _P, _PP, _P, _P, _P,
                                      ctypes.c_uint32, _P]),
     "mpe_strerror": (ctypes.c_char_p, [ctypes.c_int]),

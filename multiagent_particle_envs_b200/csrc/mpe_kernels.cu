@@ -1143,6 +1143,55 @@ static_assert(critic_smem_warps<Adversary<1, 3, 3>>(4) < 1 && critic_smem_warps<
 static_assert(!critic_built<Spread<6>>() && !critic_built<Tag<6, 2, 3>>() && critic_built<Tag<4, 2, 2>>(),
               "no critic kernel for spread N=6 and tag 6+2");
 
+// rMAPPO's recurrent centralized critic (R_Critic with use_recurrent_policy, recurrent_N = 1, use_centralized_V), one
+// weight set shared by every agent, in a kernel of its own that runs after the recurrent actor's rollout and reads its
+// observation records:
+//     x = MLPBase(share_obs) = [LN(D)] -> Linear(D, 64) -> act -> LN(64) -> Linear(64, 64) -> act -> LN(64)
+//     h' = GRU(x, h),  V = Linear(64, 1)(LN(h'))
+// folded as the recurrent actor is (the base's last LayerNorm into w_ih, b_ih; the GRU's LayerNorm into w3, b3).
+// share_obs is every agent's raw observation in agent order (D = sum of obs_dim_i), read from obs[i] ([T][n][obs_dim_i])
+// at step t and from final_obs[i] ([E][n][obs_dim_i]) for the bootstrap value.  Every L steps (L = 0: one episode of T)
+// the episode ends: its bootstrap value V(final_obs[e], h') goes to final_values[e] and h restarts from 0.  With L = 0,
+// h starts from h [n][64] (read); h receives the h after the last step in both forms, h_rec ([T][n][64] or null) the h
+// each step's critic consumed.  values [T][A][n] and final_values [E][A][n] hold the shared value for every agent.
+struct RCriticArgs {
+    const float *obs[kMaxA], *final_obs[kMaxA];
+    const float *w1, *b1, *w2, *b2, *w_ih, *b_ih, *w_hh, *b_hh, *w3, *b3;
+    float *h, *h_rec, *values, *final_values;
+    int64_t n;
+    int32_t T, L;
+    uint32_t net_flags;
+    float ln_eps;
+};
+static_assert(sizeof(RCriticArgs) <= 4096, "kernel parameter space");
+
+// Its weights in shared memory, in floats: W1's B fragments agent by agent as the MLP critic's (CriticShape::w1_off,
+// stage_critic_w1), then W2, W_ih and W_hh (GruShape's layout), W3 (one n-tile, its one real column first), b1 [64],
+// b2 [64], b_ih [192], b_hh [192], b3 [8]: 512 sum(kt1_i) + 29 704 floats.  The records stream through registers (no
+// per-warp tile), so the rest of shared memory is the L1 cache that serves their second and third reads.
+template <class P>
+struct RCriticShape {
+    using C = CriticShape<P>;
+    static constexpr int NT = 8, NG = 24;
+    static constexpr int w2_off = C::w2_off;
+    static constexpr int wih_off = w2_off + 64 * NT * NT;
+    static constexpr int whh_off = wih_off + 64 * NT * NG;
+    static constexpr int w3_off = whh_off + 64 * NT * NG;
+    static constexpr int b1_off = w3_off + 64 * NT;
+    static constexpr int b2_off = b1_off + 64;
+    static constexpr int bih_off = b2_off + 64;
+    static constexpr int bhh_off = bih_off + 192;
+    static constexpr int b3_off = bhh_off + 192;
+    static constexpr int kFloats = b3_off + 8;
+};
+static_assert(RCriticShape<Simple<1, 1>>::kFloats * 4 == 120864 && RCriticShape<Spread<3>>::kFloats * 4 == 137248 &&
+              RCriticShape<Reference>::kFloats * 4 == 131104 && RCriticShape<Spread<6>>::kFloats * 4 == 180256,
+              "simple 120 864 B, spread N=3 137 248 B, simple_reference 131 104 B, spread N=6 180 256 B");
+static_assert(RCriticShape<Spread<6>>::kFloats * 4 <= kMlpSmemBytes, "the largest weight set fits an SM");
+// Warps per block, every program: 8 (255 registers per thread for h, its TF32 copy, x and the gate accumulators of
+// one m-tile; ptxas -v: no spills, no stack).  Each warp owns 16 worlds; one block per SM.
+constexpr int kRCriticWarps = 8;
+
 __device__ __forceinline__ uint32_t to_tf32(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -1226,6 +1275,57 @@ __device__ __forceinline__ void norm_tf32_frags(uint32_t (&a)[NT][4], const floa
         a[nt][1] = to_tf32((c[nt][2] - m1) * r1);   // row g+8, k = 2q
         a[nt][2] = to_tf32((c[nt][1] - m0) * r0);   // row g,   k = 2q+1
         a[nt][3] = to_tf32((c[nt][3] - m1) * r1);   // row g+8, k = 2q+1
+    }
+}
+
+// One GRU step of one m-tile, hidden width 64, torch's gate order r, z, n (GruShape's layout: W_ih's and W_hh's B
+// fragments [k-tile][24 n-tiles][lane][2], b_ih and b_hh [192]):
+//     r = sigmoid(W_ir x + b_ir + W_hr h + b_hr),  z = sigmoid(W_iz x + b_iz + W_hz h + b_hz)
+//     n = tanh(W_in x + b_in + r * (W_hn h + b_hn)),  h' = (1 - z) * n + z * h
+// x and ht are the TF32 A fragments of x and h, hn receives h' in the accumulator layout.  For units j * 8 .. j * 8 + 7
+// r and z each accumulate both GEMMs and both biases, n keeps W_in x + b_in and W_hn h + b_hn apart; h_of(j, hf) then
+// supplies the unrounded h of those units (elements as the accumulators').  expf and tanhf are full precision.  The
+// recurrent critic's cell; mlp_agent's GRU branch computes the same operations in the same order inline (calling this
+// from there changed the recurrent actor's SASS).
+template <class HOf>
+__device__ __forceinline__ void gru_cell(const float *Wih, const float *Whh, const float *Bih, const float *Bhh,
+                                         const uint32_t (&x)[8][4], const uint32_t (&ht)[8][4], int lane, float (&hn)[8][4],
+                                         HOf &&h_of) {
+    constexpr int NT = 8, NG = 24;
+    const int tq = lane & 3;
+#pragma unroll
+    for (int j = 0; j < NT; ++j) {
+        float r[4], z[4], ni[4], nh[4];
+        {
+            const float2 bir = *reinterpret_cast<const float2 *>(Bih + j * 8 + 2 * tq);
+            const float2 bhr = *reinterpret_cast<const float2 *>(Bhh + j * 8 + 2 * tq);
+            const float2 biz = *reinterpret_cast<const float2 *>(Bih + 64 + j * 8 + 2 * tq);
+            const float2 bhz = *reinterpret_cast<const float2 *>(Bhh + 64 + j * 8 + 2 * tq);
+            const float2 bin = *reinterpret_cast<const float2 *>(Bih + 128 + j * 8 + 2 * tq);
+            const float2 bhn = *reinterpret_cast<const float2 *>(Bhh + 128 + j * 8 + 2 * tq);
+            r[0] = r[2] = bir.x + bhr.x; r[1] = r[3] = bir.y + bhr.y;
+            z[0] = z[2] = biz.x + bhz.x; z[1] = z[3] = biz.y + bhz.y;
+            ni[0] = ni[2] = bin.x; ni[1] = ni[3] = bin.y;
+            nh[0] = nh[2] = bhn.x; nh[1] = nh[3] = bhn.y;
+        }
+#pragma unroll
+        for (int kt = 0; kt < NT; ++kt) {
+            const float *bi = Wih + ((kt * NG + j) * 32 + lane) * 2, *bh = Whh + ((kt * NG + j) * 32 + lane) * 2;
+            mma_tf32(r, x[kt], *reinterpret_cast<const float2 *>(bi));
+            mma_tf32(r, ht[kt], *reinterpret_cast<const float2 *>(bh));
+            mma_tf32(z, x[kt], *reinterpret_cast<const float2 *>(bi + NT * 64));
+            mma_tf32(z, ht[kt], *reinterpret_cast<const float2 *>(bh + NT * 64));
+            mma_tf32(ni, x[kt], *reinterpret_cast<const float2 *>(bi + 2 * NT * 64));
+            mma_tf32(nh, ht[kt], *reinterpret_cast<const float2 *>(bh + 2 * NT * 64));
+        }
+        float hf[4];
+        h_of(j, hf);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float rg = 1.0f / (1.0f + expf(-r[e])), zg = 1.0f / (1.0f + expf(-z[e]));
+            const float ng = tanhf(ni[e] + rg * nh[e]);
+            hn[j][e] = (1.0f - zg) * ng + zg * hf[e];
+        }
     }
 }
 
@@ -2044,6 +2144,10 @@ const void *gru_kernel(int episodes);
 // The critic's two kernels of program P (episodes = 0, 1), instantiated by mpe_critic.cu in the same way
 template <class P>
 const void *critic_kernel(int episodes);
+// rMAPPO's recurrent critic of program P (RCriticArgs), one kernel for both forms; mpe_critic_gru.cu defines and
+// instantiates it for the programs of GruBuilt
+template <class P>
+const void *critic_gru_kernel();
 
 #ifdef MPE_KERNEL_TEMPLATES_ONLY   // mpe_gru.cu: the device code above, without the programs and the C ABI below
 }  // namespace mpe
@@ -2236,6 +2340,8 @@ struct Program {
     // 8 and 9 MAPPO's actor with its critic (critic_block_warps, H = 64 only), each critic taking critic_floats more.
     struct { const void *fn; int warps; } mlp[kMlpForms + 4][2];
     int mlp_weight_floats[2], mlp_warp_floats[2], gru_weight_floats, critic_floats;
+    const void *critic_gru_fn;   // rMAPPO's recurrent critic (kRCriticWarps per block), its weights critic_gru_floats
+    int critic_gru_floats;
     int mlp_explore_stride;           // Philox blocks per (step, agent) of its exploration noise
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
     int rollout_smem;   // dynamic shared memory per WARP of the rollout kernel
@@ -2293,6 +2399,10 @@ static Program make_program() {
         p.mlp[kMlpForms + 2][1] = {critic_kernel<P>(0), critic_block_warps<P, false>()};
         p.mlp[kMlpForms + 3][1] = {critic_kernel<P>(1), critic_block_warps<P, true>()};
         p.critic_floats = CriticShape<P>::kFloats;
+    }
+    if constexpr (GruBuilt<P>::value) {
+        p.critic_gru_fn = critic_gru_kernel<P>();
+        p.critic_gru_floats = RCriticShape<P>::kFloats;
     }
     p.smem_bytes = Shape<P>::kWarpBytes;  // per warp
     p.A = P::A; p.L = P::L; p.NS = P::NS; p.DIMC = P::DIMC; p.INFO = P::INFO; p.G = P::G;
@@ -2434,6 +2544,9 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
             if (prog->mlp[f][1].fn)                            // count, so they may take the whole opt-in
                 CUDA_TRY(cudaFuncSetAttribute(prog->mlp[f][1].fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               kMlpSmemBytes));
+        if (prog->critic_gru_fn)
+            CUDA_TRY(cudaFuncSetAttribute(prog->critic_gru_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          prog->critic_gru_floats * 4));
         if (prog->rollout_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->rollout_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->rollout_smem * max_warps_per_block(prog->rollout_smem)));
@@ -3149,6 +3262,47 @@ extern "C" int mpe_rollout_policy_mappo_critic_episodes(
     c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
     c.net_flags = net_flags; c.ln_eps = ln_eps;
     return rollout_policy_critic(h, c, critic_count, {cw1, cb1, cw2, cb2, cw3, cb3}, values, final_values);
+}
+
+extern "C" int mpe_critic_gru(mpe_handle h, const float *const *obs_record_n, const float *const *final_obs_n,
+                              int32_t n_steps, int32_t episode_length, const float *w1, const float *b1, const float *w2,
+                              const float *b2, const float *w_ih, const float *b_ih, const float *w_hh, const float *b_hh,
+                              const float *w3, const float *b3, float *rnn_state, float *rnn_state_record, float *values,
+                              float *final_values, uint32_t net_flags, float ln_eps, void *stream) {
+    if (!h || n_steps < 0) return MPE_ERR_BAD_ARG;
+    if (h->device < 0) return MPE_ERR_NO_DEVICE;
+    const Program *p = h->prog;
+    if (p->scenario == MPE_SCN_CUSTOM || p->critic_gru_fn == nullptr) return MPE_ERR_UNSUPPORTED;
+    if (episode_length < 0 || (episode_length > 0 && (n_steps < 1 || n_steps % episode_length != 0)))
+        return MPE_ERR_BAD_ARG;
+    // unknown network flags, or an eps that is negative, NaN or infinite
+    if ((net_flags & ~(kMappoFeatureNorm | kMappoTanh)) || !(ln_eps >= 0.0f && ln_eps <= 3.4e38f)) return MPE_ERR_BAD_ARG;
+    const float *const wt[10] = {w1, b1, w2, b2, w_ih, b_ih, w_hh, b_hh, w3, b3};
+    for (int j = 0; j < 10; ++j)
+        if (!ok4(wt[j])) return MPE_ERR_BAD_ARG;
+    if (!ok8(rnn_state) || (rnn_state_record != nullptr && !ok8(rnn_state_record)) || !ok4(final_values) || !final_obs_n)
+        return MPE_ERR_BAD_ARG;
+    if (n_steps > 0 && (!ok4(values) || !obs_record_n)) return MPE_ERR_BAD_ARG;
+    RCriticArgs a{};
+    for (int i = 0; i < p->A; ++i) {
+        if (!ok4(final_obs_n[i]) || (n_steps > 0 && !ok4(obs_record_n[i]))) return MPE_ERR_BAD_ARG;
+        a.obs[i] = n_steps > 0 ? obs_record_n[i] : nullptr;
+        a.final_obs[i] = final_obs_n[i];
+    }
+    a.w1 = w1; a.b1 = b1; a.w2 = w2; a.b2 = b2; a.w_ih = w_ih; a.b_ih = b_ih; a.w_hh = w_hh; a.b_hh = b_hh;
+    a.w3 = w3; a.b3 = b3;
+    a.h = rnn_state; a.h_rec = rnn_state_record; a.values = values; a.final_values = final_values;
+    a.n = h->n; a.T = n_steps; a.L = episode_length;
+    a.net_flags = net_flags; a.ln_eps = ln_eps;
+    NvtxRange range("mpe_critic_gru");
+    const int64_t warps = (h->n + 15) / 16;   // one warp per 16 worlds
+    int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
+    if (wpb < 1) wpb = 1;
+    if (wpb > kRCriticWarps) wpb = kRCriticWarps;
+    void *params[] = {&a};
+    return launch_kernel(h, p->critic_gru_fn, (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb),
+                         static_cast<size_t>(p->critic_gru_floats) * 4, stream, params, false,
+                         "cudaLaunchKernelExC(critic_gru)");
 }
 
 // adjacent (dst, src, bytes) copies with equal small gaps on both sides are issued as one DMA

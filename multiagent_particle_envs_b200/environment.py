@@ -245,7 +245,8 @@ class MultiAgentEnv(_Env):
 
     def rollout_policy(self, policies, n_steps, record_actions=False, per_step_rewards=False, record_observations=False,
                        explore_seed=None, episode_length=None, action_mode="softmax", record_log_probs=False,
-                       rnn_states=None, record_rnn_states=False, critic=None):
+                       rnn_states=None, record_rnn_states=False, critic=None, critic_rnn_states=None,
+                       record_critic_rnn_states=False):
         """T closed-loop steps in ONE kernel launch with the actors inside the kernel.
 
         One hidden layer (mpe_rollout_policy, fp32): agent i acts with softmax(W2_i relu(W1_i obs_i + b1_i) + b2_i).
@@ -337,7 +338,29 @@ class MultiAgentEnv(_Env):
         raises NotImplementedError, a malformed one or a list of length other than 1 or n ValueError.  simple_spread N=6
         and simple_tag 6+2 have no critic kernel, and per-agent critics do not fit in shared memory next to the actors
         for simple_spread N=4 and 5, simple_tag 3+1 and 4+2 and simple_adversary with 4 agents: those raise MpeError
-        before anything runs."""
+        before anything runs.
+
+        critic with MAPPO's recurrent actor (mpe_critic_gru, rMAPPO) evaluates rMAPPO's recurrent centralized critic,
+        R_Critic with recurrent_N = 1: ONE tuple (base, gru, norm, v_out), or [critic] * n (the same object) -- base
+        MAPPO's MLPBase on share_obs (nn.Sequential([LayerNorm(D)], Linear(D, 64), Act, LayerNorm(64), Linear(64, 64),
+        Act, LayerNorm(64))), gru an nn.GRU(64, 64), norm a LayerNorm(64), v_out a Linear(64, 1).  rmappo_critic_params
+        checks and folds it as the recurrent actor is folded; its Act, input LayerNorm and eps must be the actor's
+        (ValueError).  Per step t, h' = gru(base(share_obs_t), h), extras["values"][t] = v_out(norm(h')) (float32 [T, n,
+        N], the same value for every agent) and h = h'; extras["final_values"] ([n, N], with episode_length [E, n, N])
+        is the same formula once more on the observation after the last step (of each episode, before its reset) with
+        the carried h.  critic_rnn_states: the critic's initial h, a float32 CUDA tensor [N, 64] on the env's device,
+        read and never written (None: zeros; not with episode_length, whose episodes each start from h = 0).  A shared
+        critic's MAPPO buffer rnn_states_critic[:, a] is the same for every agent a: pass its slice [:, 0].
+        extras["final_critic_rnn_states"] is a new [N, 64] tensor, h after the last step (of the last episode), what
+        the next call's critic_rnn_states continues from; record_critic_rnn_states=True returns
+        extras["critic_rnn_states"], a float32 [T, N, 64] tensor of the h each step's critic consumed (zero at every
+        episode's first step), else None.  The critic runs as a second kernel on the same stream, after the rollout,
+        over the rollout's observation records: without record_observations they are scratch, T * N * D * 4 bytes
+        (1.4 GB for simple_spread N=6 at 65 536 worlds and T = 25), and extras["observations"] stays None.  Everything
+        else is bit-identical to the same call without a critic.  A recurrent critic with any other actor, an
+        nn.Sequential critic with the recurrent actor (rMAPPO pairs the actor's and the critic's recurrence) and
+        distinct per-agent recurrent critics raise NotImplementedError; critic_rnn_states or record_critic_rnn_states
+        without a recurrent critic raise ValueError."""
         import torch
         world = self.world
         if action_mode not in ("softmax", "categorical"):
@@ -354,22 +377,39 @@ class MultiAgentEnv(_Env):
                                            or int(n_steps) % int(episode_length) != 0):
             raise ValueError("rollout_policy: n_steps (%d) must be a positive multiple of episode_length (%d)"
                              % (int(n_steps), int(episode_length)))
+        recurrent = any(_is_recurrent(p) for p in policies)
+        recurrent_critic = critic is not None and _is_recurrent_critic(critic)
         if critic is not None:
-            if any(_is_recurrent(p) for p in policies) or not any(_has_layer_norm(p) for p in policies):
+            if recurrent_critic and not recurrent:
+                raise NotImplementedError("rollout_policy: a recurrent critic (a tuple holding an nn.GRU) needs MAPPO's "
+                                          "recurrent actor: rMAPPO pairs the actor's and the critic's recurrence")
+            if recurrent and not recurrent_critic:
+                raise NotImplementedError("rollout_policy: MAPPO's recurrent actor takes rMAPPO's recurrent critic "
+                                          "(base, gru, norm, v_out): rMAPPO pairs the actor's and the critic's "
+                                          "recurrence")
+            if not recurrent and not any(_has_layer_norm(p) for p in policies):
                 raise NotImplementedError("rollout_policy: critic needs MAPPO's MLP actor (LayerNorm layers); the "
                                           "two-hidden-layer and one-hidden-layer actors have no critic, and rMAPPO's "
                                           "critic is recurrent")
             if action_mode != "categorical":
                 raise NotImplementedError("rollout_policy: critic needs action_mode='categorical'")
-        if any(_is_recurrent(p) for p in policies):
+        if (critic_rnn_states is not None or record_critic_rnn_states) and not recurrent_critic:
+            raise ValueError("rollout_policy: critic_rnn_states and record_critic_rnn_states need rMAPPO's recurrent "
+                             "critic (a critic tuple holding an nn.GRU)")
+        if recurrent:
             if action_mode != "categorical":
                 raise NotImplementedError("rollout_policy: MAPPO's recurrent actor has action_mode='categorical' only")
             if rnn_states is not None and episode_length is not None:
                 raise ValueError("rollout_policy: rnn_states cannot be combined with episode_length (every episode "
                                  "starts from h = 0)")
+            if critic_rnn_states is not None and episode_length is not None:
+                raise ValueError("rollout_policy: critic_rnn_states cannot be combined with episode_length (every "
+                                 "episode starts from h = 0)")
             return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
                                             explore_seed, episode_length, True, record_log_probs, mappo=True,
-                                            gru=(rnn_states, record_rnn_states))
+                                            gru=(rnn_states, record_rnn_states),
+                                            rcritic=(critic, critic_rnn_states, record_critic_rnn_states)
+                                            if critic is not None else None)
         if rnn_states is not None or record_rnn_states:
             raise ValueError("rollout_policy: rnn_states and record_rnn_states need MAPPO's recurrent actor "
                              "(a policy tuple with an nn.GRU)")
@@ -429,7 +469,7 @@ class MultiAgentEnv(_Env):
 
     def _rollout_policy_mlp(self, policies, n_steps, record_actions, per_step_rewards, record_observations, explore_seed,
                             episode_length=None, categorical=False, record_log_probs=False, mappo=False, gru=None,
-                            critic=None):
+                            critic=None, rcritic=None):
         import torch
         world = self.world
         nw = world.bind()
@@ -456,6 +496,29 @@ class MultiAgentEnv(_Env):
             else:                # every episode starts from h = 0 without reading the buffer
                 h = torch.empty(shape, dtype=torch.float32, device=nw.device)
             rnn = (h, torch.empty((T,) + shape, dtype=torch.float32, device=nw.device) if record else None)
+            if rcritic is not None:   # rMAPPO's recurrent critic: rcritic = (critic, critic_rnn_states, record)
+                rmodule, ch0, crecord = rcritic
+                rparams, ctanh, cfn, ceps = rmappo_critic_params(rmodule, nw.obs_dims)
+                if (ctanh, cfn, ceps) != (tanh, feature_norm, eps):
+                    raise ValueError("rollout_policy: the critic must use the actor's activation, input LayerNorm and "
+                                     "eps (%s, %s, %g); got (%s, %s, %g)"
+                                     % ("Tanh" if tanh else "ReLU", feature_norm, eps, "Tanh" if ctanh else "ReLU", cfn,
+                                        ceps))
+                nw.require_critic_gru()
+                cshape = (N, MAPPO_HIDDEN)
+                if ch0 is not None:
+                    if not (torch.is_tensor(ch0) and tuple(ch0.shape) == cshape and ch0.dtype == torch.float32
+                            and ch0.device == torch.device(nw.device)):
+                        raise ValueError("rollout_policy: critic_rnn_states must be a float32 tensor %s on %s; got %s"
+                                         % (list(cshape), nw.device, (tuple(ch0.shape), ch0.dtype, ch0.device)
+                                            if torch.is_tensor(ch0) else type(ch0).__name__))
+                    ch = ch0.clone(memory_format=torch.contiguous_format)   # the kernel overwrites its state buffer
+                elif episode_length is None:
+                    ch = torch.zeros(cshape, dtype=torch.float32, device=nw.device)
+                else:            # every episode starts from h = 0 without reading the buffer
+                    ch = torch.empty(cshape, dtype=torch.float32, device=nw.device)
+                rkeep = [t.to(device=nw.device, dtype=torch.float32).contiguous() for t in rparams]
+                rcrit = (ch, torch.empty((T,) + cshape, dtype=torch.float32, device=nw.device) if crecord else None)
         elif mappo:
             params, tanh, feature_norm, eps = mappo_actor_params(policies, nw.obs_dims, nw.act_dims)
             hidden = MAPPO_HIDDEN
@@ -492,18 +555,20 @@ class MultiAgentEnv(_Env):
         else:
             actions = [torch.empty((T, N, ad), **dev) for ad in nw.act_dims] if record_actions else None
         log_probs = torch.empty((T, self.n, N), **dev) if record_log_probs else None
-        observations = [torch.empty((T, N, od), **dev) for od in nw.obs_dims] if record_observations else None
+        # the recurrent critic reads the rollout's observation records: scratch unless the caller asked for them
+        need_obs = record_observations or rcritic is not None
+        observations = [torch.empty((T, N, od), **dev) for od in nw.obs_dims] if need_obs else None
         seed = None if explore_seed is None else int(explore_seed) & 0xFFFFFFFFFFFFFFFF
         act_ptrs = _lib.ptr_array([a.data_ptr() for a in actions]) if actions is not None else None
         obs_ptrs = _lib.ptr_array([o.data_ptr() for o in observations]) if observations is not None else None
-        extras = {"actions": actions, "rewards": rew_steps, "observations": observations}
+        extras = {"actions": actions, "rewards": rew_steps, "observations": observations if record_observations else None}
         if categorical:
             extras["log_probs"] = log_probs
         E, ep_rew, final = 1, None, None
         if episode_length is not None:
             E = T // int(episode_length)
             ep_rew = torch.empty((E, self.n, N), **dev)
-            final = [torch.empty((E, N, od), **dev) for od in nw.obs_dims] if record_observations else None
+            final = [torch.empty((E, N, od), **dev) for od in nw.obs_dims] if need_obs else None
         nw.rollout_policy_mlp(w_ptrs, hidden, T, out, self._flags(), episode_length=episode_length, categorical=categorical,
                               rew_steps=rew_steps, act_rec_ptrs=act_ptrs, obs_rec_ptrs=obs_ptrs,
                               final_obs_ptrs=_lib.ptr_array([o.data_ptr() for o in final]) if final is not None else None,
@@ -511,13 +576,21 @@ class MultiAgentEnv(_Env):
                               mappo=net, gru=rnn, critic=crit)
         if rnn is not None:
             extras["final_rnn_states"], extras["rnn_states"] = rnn
+        if rcritic is not None:   # on the same stream, after the rollout that wrote its input records
+            values = torch.empty((T, self.n, N), **dev)
+            final_values = torch.empty((self.n, N) if episode_length is None else (E, self.n, N), **dev)
+            nw.critic_gru([t.data_ptr() for t in rkeep], obs_ptrs,
+                          out.obs_ptrs if final is None else _lib.ptr_array([o.data_ptr() for o in final]), T,
+                          episode_length, rcrit[0], rcrit[1], values, final_values, net)
+            extras["values"], extras["final_values"] = values, final_values
+            extras["final_critic_rnn_states"], extras["critic_rnn_states"] = rcrit
         if crit is not None:
             extras["values"], extras["final_values"] = crit[2], crit[3]
         if episode_length is None:
             reward_n = list(out.rew_list)
         else:
             reward_n = list(ep_rew.unbind(1))
-            extras["final_observations"] = final
+            extras["final_observations"] = final if record_observations else None
         if seed is not None:
             self.explore_epoch += E
         self._last_out = out
@@ -970,6 +1043,13 @@ def _is_recurrent(pol):
     return isinstance(pol, (tuple, list)) and any(isinstance(m, torch.nn.GRU) for m in pol)
 
 
+def _is_recurrent_critic(critic):
+    """does this critic ask for rMAPPO's recurrent critic?  (A tuple holding an nn.GRU, or a list of such tuples;
+    rmappo_critic_params checks the rest.)"""
+    return _is_recurrent(critic) or (isinstance(critic, (tuple, list)) and len(critic) > 0
+                                     and all(_is_recurrent(c) for c in critic))
+
+
 def _fold_layer_norm(W, b, ln):
     """W, b of the Linear (or GRU input map) after LayerNorm ln, in float64, with ln's affine folded in:
     W' = W diag(gamma), b' = b + W beta"""
@@ -1050,3 +1130,34 @@ def rmappo_actor_params(policies, obs_dims, act_dims=None):
     W_hh, b_hh = _fold_layer_norm(gru.weight_hh_l0, gru.bias_hh_l0, None)
     W3, b3 = _fold_layer_norm(head.weight, head.bias, norm)
     return (W1, b1, W2, b2, W_ih, b_ih, W_hh, b_hh, W3, b3), type(body[1]) is nn.Tanh, fn, eps.pop()
+
+
+# ---- rMAPPO's recurrent centralized critic (R_Critic with use_recurrent_policy, recurrent_N = 1, use_centralized_V) ----
+_RCRITIC_SHAPE = ("(base, gru, norm, v_out) with base = nn.Sequential([LayerNorm(D)], Linear(D, 64), Act, LayerNorm(64), "
+                  "Linear(64, 64), Act, LayerNorm(64)), Act = ReLU() or Tanh(), gru = nn.GRU(64, 64), norm = "
+                  "LayerNorm(64), v_out = Linear(64, 1) and D the sum of the agents' observation sizes")
+
+
+def rmappo_critic_params(critic, obs_dims):
+    """rMAPPO's recurrent centralized critic -> (params, tanh, feature_norm, eps), or ValueError.  critic is one tuple
+    (base, gru, norm, v_out), or a list of 1 or len(obs_dims) entries that are all that same tuple object ([critic] * n,
+    a shared critic); distinct tuples raise NotImplementedError.  The tuple is checked under the rules of
+    rmappo_actor_params with input width D = sum(obs_dims) (share_obs) and head Linear(64, 1).  From an on-policy
+    R_Critic `c`: (nn.Sequential(c.base.feature_norm, *c.base.mlp.fc1, *c.base.mlp.fc2[0]), c.rnn.rnn, c.rnn.norm,
+    c.v_out).  params = (W1, b1, W2, b2, W_ih, b_ih, W_hh, b_hh, W3, b3) in float64, folded as rmappo_actor_params
+    folds the actor (W1 [64, D], W3 [1, 64], b3 [1]).  No device is needed."""
+    n, D = len(obs_dims), int(sum(obs_dims))
+    if _is_recurrent(critic):
+        one = critic
+    elif isinstance(critic, (tuple, list)) and len(critic) in (1, n) and all(_is_recurrent(c) for c in critic):
+        if any(c is not critic[0] for c in critic):
+            raise NotImplementedError("the recurrent critic must be one tuple shared by every agent ([critic] * n); "
+                                      "distinct per-agent recurrent critics are not supported")
+        one = critic[0]
+    else:
+        raise ValueError("the recurrent critic must be one tuple %s, or a list of 1 or %d of that same tuple"
+                         % (_RCRITIC_SHAPE, n))
+    try:
+        return rmappo_actor_params([one], [D], [1])
+    except ValueError as e:
+        raise ValueError("the recurrent critic must be %s: %s" % (_RCRITIC_SHAPE, e)) from None

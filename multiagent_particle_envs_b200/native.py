@@ -301,6 +301,28 @@ class NativeWorld(ShapeHandle):
         if rc == _lib.ERR_UNSUPPORTED:
             check(rc, "mpe_rollout_policy_mappo_critic")
 
+    def require_critic_gru(self):
+        """MpeError unless the library has rMAPPO's recurrent critic for this program.  mpe_critic_gru checks the program
+        before any pointer, so the probe stops at the null state and runs nothing."""
+        rc = self.lib.mpe_critic_gru(self.handle, None, None, 0, 0, *([256] * 10), None, None, None, None, 0, 0.0,
+                                     self._stream())
+        if rc == _lib.ERR_UNSUPPORTED:
+            check(rc, "mpe_critic_gru")
+
+    def critic_gru(self, w_ptrs, obs_rec_ptrs, final_obs_ptrs, n_steps, episode_length, rnn_state, rnn_record, values,
+                   final_values, net):
+        """rMAPPO's recurrent critic over a finished rollout's records (mpe_critic_gru), on the current stream: w_ptrs
+        the ten device pointers of its folded weight set (environment.rmappo_critic_params), obs_rec_ptrs and
+        final_obs_ptrs one [n_steps, N, obs_dim_i] and one [E, N, obs_dim_i] record per agent, episode_length None
+        (one episode) or L.  rnn_state (float32 [N, 64]) holds the initial h (unless episode_length) and receives the
+        final one, rnn_record (float32 [n_steps, N, 64] or None) the h each step consumed; values [n_steps, A, N] and
+        final_values [E, A, N] receive the values.  net = (net_flags, eps) as in rollout_policy_mlp."""
+        rc = self.lib.mpe_critic_gru(self.handle, obs_rec_ptrs, final_obs_ptrs, int(n_steps), int(episode_length or 0),
+                                     *w_ptrs, rnn_state.data_ptr(), rnn_record.data_ptr() if rnn_record is not None
+                                     else None, values.data_ptr(), final_values.data_ptr(), int(net[0]), float(net[1]),
+                                     self._stream())
+        check(rc, "mpe_critic_gru")
+
     def rollout_policy_mlp(self, w_ptrs, hidden, n_steps, out=None, flags=0, *, episode_length=None, categorical=False,
                            rew_steps=None, act_rec_ptrs=None, obs_rec_ptrs=None, final_obs_ptrs=None, logp_steps=None,
                            ep_rew=None, explore_seed=None, explore_epoch=0, mappo=None, gru=None, critic=None):

@@ -20,6 +20,13 @@
       what a trainer does without it: the same call with record_observations=True, then the torch critic over the
       concatenated records ([T N, D]) and the final observations ([N, D]), at torch's default float32 matmul
       precision.  Only these two arms are timed ("in_kernel_critic", "kernel_then_torch_critic");
+      --critic recurrent (with --actor rmappo): rMAPPO's recurrent critic, one (base, gru, norm, v_out) tuple on the
+      concatenated observations (critic=..., mpe_critic_gru after the rollout).  Three arms are timed in the same run:
+      "in_kernel_critic" (the rollout with the critic), "rollout_recording_observations" (the same rollout with
+      record_observations=True and no critic: the difference is the critic kernel's own cost) and
+      "kernel_then_torch_critic" (that rollout, then the torch critic under no_grad in its fastest form: base over
+      [T N, D] in one call, one cuDNN nn.GRU call over the [T, N, 64] sequence, norm and v_out, plus the bootstrap step
+      on the returned observations);
   (b) the same actors as torch modules + env.step, all captured in one CUDA graph (rollout.GraphedRollout); with
       --categorical the graphed policy takes argmax(logits - log(-log u)) per sub-space, its one_hot and
       log_softmax(logits).gather(k) for the log-probabilities.  With --actor rmappo the graphed policy evaluates the
@@ -106,6 +113,59 @@ def time_critic(args, env, mods, kw, res, e0, e1):
     return res
 
 
+def time_rcritic(args, env, mods, kw, res, e0, e1):
+    """rMAPPO's recurrent critic: (a) the rollout with the critic kernel after it, (b) the rollout recording
+    observations without a critic, (c) (b), then the torch critic; device time per step of each"""
+    import torch
+    nn = torch.nn
+    nw = env.world.native
+    n, T, H, D = args.num_envs, args.steps, args.hidden, sum(nw.obs_dims)
+    dev = mods[0][0][-1].weight.device
+    Act = nn.Tanh if args.tanh else nn.ReLU
+    base = nn.Sequential(*(([nn.LayerNorm(D)] if args.feature_norm else []) +
+                           [nn.Linear(D, H), Act(), nn.LayerNorm(H), nn.Linear(H, H), Act(), nn.LayerNorm(H)]))
+    critic = tuple(m.to(dev) for m in (base, nn.GRU(H, H), nn.LayerNorm(H), nn.Linear(H, 1)))
+    b, gru, norm, v_out = critic
+    h0 = torch.zeros(1, n, H, device=dev)
+
+    def in_kernel():
+        env.rollout_policy(mods, T, critic=critic, **kw)
+
+    def recording():
+        return env.rollout_policy(mods, T, record_observations=True, **kw)
+
+    def kernel_then_torch():
+        obs_n, _, _, _, ex = recording()
+        x = torch.cat(ex["observations"], -1).reshape(T * n, D)
+        with torch.no_grad():
+            out, hT = gru(b(x).reshape(T, n, H), h0)
+            v_out(norm(out))
+            _, hb = gru(b(torch.cat(list(obs_n), -1))[None], hT)
+            v_out(norm(hb[0]))
+
+    def timed(fn):
+        for _ in range(2):
+            fn()
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(args.reps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / 1e3 / (args.reps * T)
+
+    res["config"].update(torch_float32_matmul_precision=torch.get_float32_matmul_precision(),
+                         cudnn_allow_tf32=torch.backends.cudnn.allow_tf32)
+    sa, sr, sb = timed(in_kernel), timed(recording), timed(kernel_then_torch)
+    res["in_kernel_critic"] = {"us_per_step": 1e6 * sa, "env_steps_per_sec": n / sa}
+    res["rollout_recording_observations"] = {"us_per_step": 1e6 * sr, "env_steps_per_sec": n / sr}
+    res["kernel_then_torch_critic"] = {"us_per_step": 1e6 * sb, "env_steps_per_sec": n / sb}
+    res["critic_kernel_us_per_step"] = 1e6 * (sa - sr)
+    res["speedup"] = sb / sa
+    res["card"] = card_info()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scenario", default="simple_spread")
@@ -124,12 +184,14 @@ def main():
                          "--categorical)")
     ap.add_argument("--tanh", action="store_true", help="MAPPO's actor with Tanh instead of ReLU")
     ap.add_argument("--feature-norm", action="store_true", help="MAPPO's actor with the input LayerNorm")
-    ap.add_argument("--critic", choices=("shared", "separated"),
+    ap.add_argument("--critic", choices=("shared", "separated", "recurrent"),
                     help="time MAPPO's centralized critic in-kernel against the torch critic after the rollout "
-                         "(--actor mappo)")
+                         "(shared, separated: --actor mappo; recurrent: --actor rmappo)")
     args = ap.parse_args()
-    if args.critic and args.actor != "mappo":
-        ap.error("--critic needs --actor mappo")
+    if args.critic in ("shared", "separated") and args.actor != "mappo":
+        ap.error("--critic shared|separated needs --actor mappo")
+    if args.critic == "recurrent" and args.actor != "rmappo":
+        ap.error("--critic recurrent needs --actor rmappo")
     if args.actor in ("mappo", "rmappo"):
         args.layers, args.categorical = 3, True
     elif args.tanh or args.feature_norm:
@@ -204,7 +266,8 @@ def main():
 
     if args.critic:
         res["config"].update(critic=args.critic)
-        print(json.dumps(time_critic(args, env, mods, kw, res, e0, e1)))
+        timer = time_rcritic if args.critic == "recurrent" else time_critic
+        print(json.dumps(timer(args, env, mods, kw, res, e0, e1)))
         return
     sec = time_in_kernel(mods)
     res["in_kernel"] = {"us_per_step": 1e6 * sec, "env_steps_per_sec": n / sec}

@@ -129,11 +129,12 @@ def main():
         print("| " + " | ".join(str(x) for x in r) + " |")
     forms = {"mlp_rollout": "S", "mlp_episode": "E", "mlp_categorical": "C", "mlp_categorical_episode": "CE",
              "mappo": "M", "mappo_episode": "ME", "gru": "G", "gru_episode": "GE", "mappo_critic": "V",
-             "mappo_critic_episode": "VE"}
+             "mappo_critic_episode": "VE", "critic_gru": "R"}
     mlp = []
     for mangled, (reg, stack) in usage.items():
-        m = re.match(r"void mpe::mpe_policy_(mlp_rollout|mlp_episode|mlp_categorical|mlp_categorical_episode|mappo|"
-                     r"mappo_episode|gru|gru_episode|mappo_critic|mappo_critic_episode)_kernel<mpe::(.+?)(?:, (\d+))?\s*>\(", names[mangled])
+        m = re.match(r"void mpe::mpe_(?:policy_)?(mlp_rollout|mlp_episode|mlp_categorical|mlp_categorical_episode|mappo|"
+                     r"mappo_episode|gru|gru_episode|mappo_critic|mappo_critic_episode|critic_gru)_kernel<mpe::(.+?)"
+                     r"(?:, (\d+))?\s*>\(", names[mangled])
         if m:
             c = mix.get(mangled, {})
             mlp.append((m.group(2), m.group(3) or "64", forms[m.group(1)], reg, stack, c["total"], c["HMMA"], c["LDS"],
@@ -143,7 +144,8 @@ def main():
               "`mpe_policy_mlp_rollout_kernel`, E its episode form `mpe_policy_mlp_episode_kernel`, C and CE the "
               "categorical forms of both, M and ME MAPPO's LayerNorm actor `mpe_policy_mappo[_episode]_kernel`, G and GE its "
               "recurrent actor `mpe_policy_gru[_episode]_kernel`, V and VE its LayerNorm actor with the centralized critic "
-              "`mpe_policy_mappo_critic[_episode]_kernel` (all H = 64)\n")
+              "`mpe_policy_mappo_critic[_episode]_kernel`, R rMAPPO's recurrent critic `mpe_critic_gru_kernel` (all H = "
+              "64)\n")
         print("| program | H | form | regs | stack | instr | HMMA | LDS | MUFU |")
         print("|---|---|---|---|---|---|---|---|---|")
         for r in sorted(mlp):
