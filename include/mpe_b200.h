@@ -430,6 +430,47 @@ MPE_API int mpe_critic_gru(mpe_handle h, const float *const *obs_record_n, const
                            float *rnn_state_record_dev, float *values_dev, float *final_values_dev,
                            uint32_t net_flags, float ln_eps, void *stream);
 
+/* flags of mpe_gae */
+enum mpe_gae_flags {
+    MPE_GAE_BOOTSTRAP = 1,              /* an episode end is a time-limit truncation: continue with gamma * V(final) */
+    MPE_GAE_NORMALIZE = 2,              /* normalise the advantages over all T * A * N entries (PPO's update step) */
+    MPE_GAE_PER_AGENT_VALUE_NORM = 4    /* value_norm_dev holds one (mean, std) row per agent, [A][2] */
+};
+
+/* MAPPO's GAE advantages and returns (SharedReplayBuffer.compute_returns with use_gae) over a finished buffer, on the
+ * device, for any handle: only its A and N are used.  rewards_dev, values_dev, returns_dev and advantages_dev are
+ * float32 [T][A][N] (T = n_steps); final_values_dev [E][A][N], E = n_steps / L.  episode_length L = 0 is one episode
+ * of n_steps; L > 0 makes episode e steps e*L .. e*L + L - 1.  value_norm_dev (NULL: no ValueNorm) holds float32
+ * (mean, std), [2] for every agent or [A][2] with MPE_GAE_PER_AGENT_VALUE_NORM; every value v is denormalised as
+ * dv = v * std + mean (else dv = v).  It is read on the device: the call never synchronises with the host and can be
+ * captured in a CUDA graph.  Per column (agent, world), t running backwards inside each episode:
+ *     last   = t is the last step of its episode
+ *     next   = last ? (MPE_GAE_BOOTSTRAP ? dv(final_values[e]) : 0) : dv[t + 1]
+ *     carry  = last ? 0 : gae[t + 1]
+ *     delta  = (r[t] + gamma * next) - dv[t]
+ *     gae[t] = delta + (gamma * gae_lambda) * carry      gamma * gae_lambda: one fp32 product
+ *     ret[t] = gae[t] + dv[t]
+ * in fp32, every operation rounded to nearest in exactly this order, with no fused multiply-add.  returns_dev
+ * receives ret, advantages_dev gae.  MPE_GAE_NORMALIZE replaces every advantage a by
+ * float((double(a) - mean) / (std + 1e-5)), mean and std (population) over all T * A * N advantages, summed in fp64
+ * per scan block and combined in a fixed order: two calls give the same bits.  (mean, std) is then left as two
+ * doubles at the start of the workspace.  workspace_dev (8-byte aligned, at least mpe_gae_workspace_bytes(h) bytes,
+ * contents on entry irrelevant) is needed only with MPE_GAE_NORMALIZE and may be NULL without it; calls that share a
+ * workspace must be ordered on one stream.  Outputs must not overlap the inputs, each other or the workspace.
+ * Checked in this order: MPE_ERR_BAD_ARG for a null handle or n_steps < 1; MPE_ERR_NO_DEVICE; MPE_ERR_BAD_ARG for
+ * episode_length < 0 or not dividing n_steps; for gamma or gae_lambda outside [0, 1] or not finite; for unknown flag
+ * bits; for a null or misaligned (not 4-byte aligned) rewards, values, returns or advantages array, a null or
+ * misaligned final_values_dev with MPE_GAE_BOOTSTRAP (without it, it is not read and may be NULL), a misaligned
+ * value_norm_dev or a null one with MPE_GAE_PER_AGENT_VALUE_NORM, and, with MPE_GAE_NORMALIZE, a null, not 8-byte
+ * aligned or too small workspace. */
+MPE_API int mpe_gae(mpe_handle h, const float *rewards_dev, const float *values_dev, const float *final_values_dev,
+                    int32_t n_steps, int32_t episode_length, float gamma, float gae_lambda, uint32_t flags,
+                    const float *value_norm_dev, float *returns_dev, float *advantages_dev, void *workspace_dev,
+                    int64_t workspace_bytes, void *stream);
+/* bytes of mpe_gae's workspace for this handle (32 + 16 per 128 columns of A * N), or MPE_ERR_BAD_ARG for a null
+ * handle */
+MPE_API int64_t mpe_gae_workspace_bytes(mpe_handle h);
+
 /* Same step for a caller that holds HOST buffers (what the reference's callers hold):
  * act_n_host[i] -> (async H2D into act_n_dev[i]) -> mpe_step -> (async D2H) obs_n_host[i],
  * rew_host, done_host, all ordered on `stream`.  Host buffers should be pinned for the copies

@@ -30,6 +30,11 @@ ERR_UNSUPPORTED = -3
 MAPPO_FEATURE_NORM = 1
 MAPPO_TANH = 2
 
+# enum mpe_gae_flags
+GAE_BOOTSTRAP = 1
+GAE_NORMALIZE = 2
+GAE_PER_AGENT_VALUE_NORM = 4
+
 
 class MpeDesc(ctypes.Structure):
     """mirror of `struct mpe_desc` (include/mpe_b200.h)"""
@@ -138,6 +143,9 @@ _SIGNATURES = {
                                                                 ctypes.c_uint32, _P]),
     "mpe_critic_gru": (ctypes.c_int, [_P, _PP, _PP, ctypes.c_int32, ctypes.c_int32] + [_P] * 10 +
                        [_P, _P, _P, _P, ctypes.c_uint32, ctypes.c_float, _P]),
+    "mpe_gae": (ctypes.c_int, [_P, _P, _P, _P, ctypes.c_int32, ctypes.c_int32, ctypes.c_float, ctypes.c_float,
+                               ctypes.c_uint32, _P, _P, _P, _P, ctypes.c_int64, _P]),
+    "mpe_gae_workspace_bytes": (ctypes.c_int64, [_P]),
     "mpe_step_host": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _P, _P, _P, _PP, _P, _P, _P,
                                      ctypes.c_uint32, _P]),
     "mpe_strerror": (ctypes.c_char_p, [ctypes.c_int]),

@@ -2149,6 +2149,31 @@ const void *critic_kernel(int episodes);
 template <class P>
 const void *critic_gru_kernel();
 
+// MAPPO's GAE over a finished buffer (mpe_gae): one thread per (agent, world) column of [T][A][N], walking t backwards.
+// mpe_gae.cu defines the kernels; gae_kernel(0) is the scan, gae_kernel(1) the scan that also sums the advantages and
+// their squares (fp64) into the workspace and, in its last block, writes (mean, std), gae_kernel(2) the in-place
+// normalisation of the advantages.
+constexpr uint32_t kGaeBootstrap = MPE_GAE_BOOTSTRAP, kGaeNormalize = MPE_GAE_NORMALIZE,
+                   kGaePerAgentNorm = MPE_GAE_PER_AGENT_VALUE_NORM;
+constexpr int kGaeThreads = 128;       // scan block: one fp64 partial (two doubles of workspace) per block
+constexpr int kGaeNormThreads = 256;   // normalisation block
+constexpr int64_t kGaeWsHeader = 32;   // workspace: double (mean, std) at 0, the uint32 ticket at 16, partials at 32
+struct GaeArgs {
+    const float *rew, *val;      // [T][A][N]
+    const float *final_val;      // [E][A][N], null without kGaeBootstrap
+    const float *value_norm;     // (mean, std): [2], [A][2] with kGaePerAgentNorm, or null
+    float *ret, *adv;            // [T][A][N]
+    double *stats;               // workspace: (mean, std) of the raw advantages
+    unsigned *ticket;            // workspace: blocks done with their partial (zeroed before the scan)
+    double *partial;             // workspace: [gridDim.x][2] (sum a, sum a^2) per scan block, as two doubles: the
+                                 // workspace need only be 8-byte aligned
+    int64_t cols, n;             // A * N, N
+    int32_t T, L;                // steps, episode length (T for one episode)
+    float gamma, lambda;
+    uint32_t flags;
+};
+const void *gae_kernel(int which);
+
 #ifdef MPE_KERNEL_TEMPLATES_ONLY   // mpe_gru.cu: the device code above, without the programs and the C ABI below
 }  // namespace mpe
 #else
@@ -3303,6 +3328,58 @@ extern "C" int mpe_critic_gru(mpe_handle h, const float *const *obs_record_n, co
     return launch_kernel(h, p->critic_gru_fn, (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb),
                          static_cast<size_t>(p->critic_gru_floats) * 4, stream, params, false,
                          "cudaLaunchKernelExC(critic_gru)");
+}
+
+static int64_t gae_scan_blocks(const mpe_env *h) { return (h->prog->A * h->n + kGaeThreads - 1) / kGaeThreads; }
+
+extern "C" int64_t mpe_gae_workspace_bytes(mpe_handle h) {
+    return h ? kGaeWsHeader + 16 * gae_scan_blocks(h) : static_cast<int64_t>(MPE_ERR_BAD_ARG);
+}
+
+extern "C" int mpe_gae(mpe_handle h, const float *rewards, const float *values, const float *final_values,
+                       int32_t n_steps, int32_t episode_length, float gamma, float gae_lambda, uint32_t flags,
+                       const float *value_norm, float *returns, float *advantages, void *workspace,
+                       int64_t workspace_bytes, void *stream) {
+    if (!h || n_steps < 1) return MPE_ERR_BAD_ARG;
+    if (h->device < 0) return MPE_ERR_NO_DEVICE;
+    if (episode_length < 0 || (episode_length > 0 && n_steps % episode_length != 0)) return MPE_ERR_BAD_ARG;
+    if (!(gamma >= 0.0f && gamma <= 1.0f) || !(gae_lambda >= 0.0f && gae_lambda <= 1.0f)) return MPE_ERR_BAD_ARG;
+    if (flags & ~(kGaeBootstrap | kGaeNormalize | kGaePerAgentNorm)) return MPE_ERR_BAD_ARG;
+    const bool norm = flags & kGaeNormalize;
+    if (!ok4(rewards) || !ok4(values) || !ok4(returns) || !ok4(advantages) ||
+        ((flags & kGaeBootstrap) && !ok4(final_values)) || (value_norm != nullptr && !ok4(value_norm)) ||
+        ((flags & kGaePerAgentNorm) && value_norm == nullptr) ||
+        (norm && (!ok8(workspace) || workspace_bytes < mpe_gae_workspace_bytes(h))))
+        return MPE_ERR_BAD_ARG;
+    GaeArgs a{};
+    a.rew = rewards; a.val = values; a.final_val = (flags & kGaeBootstrap) ? final_values : nullptr;
+    a.value_norm = value_norm; a.ret = returns; a.adv = advantages;
+    char *ws = static_cast<char *>(workspace);
+    if (norm) {
+        a.stats = reinterpret_cast<double *>(ws);
+        a.ticket = reinterpret_cast<unsigned *>(ws + 16);
+        a.partial = reinterpret_cast<double *>(ws + kGaeWsHeader);
+    }
+    a.cols = h->prog->A * h->n; a.n = h->n;
+    a.T = n_steps; a.L = episode_length > 0 ? episode_length : n_steps;
+    a.gamma = gamma; a.lambda = gae_lambda; a.flags = flags;
+    NvtxRange range("mpe_gae");
+    void *params[] = {&a};
+    if (norm) {   // the scan's last block is the one that takes ticket blocks - 1
+        int prev = 0;
+        CUDA_TRY(cudaGetDevice(&prev));
+        if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
+        const cudaError_t e = cudaMemsetAsync(a.ticket, 0, sizeof(unsigned), static_cast<cudaStream_t>(stream));
+        if (prev != h->device) cudaSetDevice(prev);
+        if (e != cudaSuccess) return cuda_fail(e, "cudaMemsetAsync(gae ticket)");
+    }
+    int r = launch_kernel(h, gae_kernel(norm ? 1 : 0), gae_scan_blocks(h), kGaeThreads, 0, stream, params, false,
+                          "cudaLaunchKernelExC(gae)");
+    if (r || !norm) return r;
+    const int64_t total = a.cols * n_steps, want = (total + kGaeNormThreads * 4 - 1) / (kGaeNormThreads * 4);
+    const int64_t cap = 8 * static_cast<int64_t>(h->sms > 0 ? h->sms : 1);   // 2048 threads per SM, grid-stride
+    return launch_kernel(h, gae_kernel(2), want < cap ? want : cap, kGaeNormThreads, 0, stream, params, false,
+                         "cudaLaunchKernelExC(gae_normalize)");
 }
 
 // adjacent (dst, src, bytes) copies with equal small gaps on both sides are issued as one DMA

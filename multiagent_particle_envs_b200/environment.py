@@ -467,6 +467,98 @@ class MultiAgentEnv(_Env):
         info_n = {'n': [{} for _ in range(self.n)]}
         return list(out.obs), list(out.rew_list), list(out.done_list), info_n, {"actions": actions, "rewards": rew_steps}
 
+    def compute_gae(self, rewards, values, final_values=None, gamma=0.99, gae_lambda=0.95, episode_length=None,
+                    bootstrap=True, value_norm=None, normalize_advantages=False):
+        """MAPPO's GAE advantages and returns (SharedReplayBuffer.compute_returns with use_gae) in one kernel launch
+        (mpe_gae), plus PPO's advantage normalisation in a second one.  Any batched env, any source of values: the
+        rollout_policy critics' extras or a trainer's own critic.
+
+        rewards and values are float32 CUDA tensors [T, n, N] on the env's device (extras["rewards"] of
+        per_step_rewards=True, extras["values"]); final_values is [n, N] (extras["final_values"]), or [E, n, N] with
+        episode_length=L, E = T / L: episode e covers steps e*L .. e*L + L - 1 (rollout_policy's episode form); without
+        episode_length the whole buffer is one episode.  value_norm (MAPPO's ValueNorm): None, or a float32 CUDA tensor
+        (mean, std), [2] shared or [n, 2] one row per agent -- mean, var = value_normalizer.running_mean_var(); std =
+        var.sqrt() -- and every value v is then denormalised as v * std + mean; it is read on the device, so the call
+        never waits for the host and can be captured in a CUDA graph.  Per agent and world, t running backwards inside
+        each episode:
+
+            last   = t is the last step of its episode
+            next   = last ? (bootstrap ? dv(final_values[e]) : 0) : dv[t + 1]
+            carry  = last ? 0 : gae[t + 1]
+            delta  = (r[t] + gamma * next) - dv[t]
+            gae[t] = delta + (gamma * gae_lambda) * carry
+            ret[t] = gae[t] + dv[t]
+
+        in float32, every operation rounded in this order without fused multiply-adds (gamma and gae_lambda are rounded
+        to float32 first, gamma * gae_lambda is one float32 product).  bootstrap=True treats an episode end as a
+        time-limit truncation (continue with gamma * V of the final observation); bootstrap=False as terminal, MAPPO on
+        MPE's behaviour, where final_values may be None.
+
+        Returns (returns, advantages, stats): new float32 [T, n, N] tensors ret and gae.  The advantages are gae itself,
+        not MAPPO's recomputed returns - dv; the two are equal in exact arithmetic and differ by at most the one float32
+        rounding of ret.  normalize_advantages=True replaces them by (a - mean) / (std + 1e-5), mean and population std
+        over all T * n * N entries, computed in float64 from per-block partial sums combined in a fixed order (two calls
+        give the same bits), each entry float32((float64(a) - mean) / (std + 1e-5)); stats is then a float64 [2] tensor
+        (mean, std), else None.  ValueError, before anything runs, for a non-batched env, tensors of the wrong shape,
+        dtype, device or layout, a final_values that does not match episode_length, a value_norm that is not [2] or
+        [n, 2], gamma or gae_lambda outside [0, 1], an episode_length that does not divide T, or bootstrap without
+        final_values."""
+        import torch
+        world = self.world
+        if not world.batched:
+            raise ValueError("compute_gae needs a batched env (make_env(..., num_envs=N))")
+        shapes = world.native_shapes()   # shapes first, the device (bind) once everything else is known to be valid
+        n, N = shapes.n_agents, shapes.n_env
+
+        def check_tensor(name, t, shape):
+            if not torch.is_tensor(t) or t.dtype != torch.float32 or not t.is_contiguous():
+                raise ValueError("compute_gae: %s must be a contiguous float32 tensor" % name)
+            if tuple(t.shape) != tuple(shape):
+                raise ValueError("compute_gae: %s must have shape %s, got %s" % (name, tuple(shape), tuple(t.shape)))
+
+        if not torch.is_tensor(rewards) or rewards.dim() != 3 or rewards.shape[0] < 1:
+            raise ValueError("compute_gae: rewards must be a [T, %d, %d] tensor with T >= 1" % (n, N))
+        T = int(rewards.shape[0])
+        check_tensor("rewards", rewards, (T, n, N))
+        check_tensor("values", values, (T, n, N))
+        if episode_length is not None and (int(episode_length) < 1 or T % int(episode_length) != 0):
+            raise ValueError("compute_gae: episode_length (%s) must divide T (%d)" % (episode_length, T))
+        for name, x in (("gamma", gamma), ("gae_lambda", gae_lambda)):
+            if not 0.0 <= float(x) <= 1.0:   # also refuses NaN
+                raise ValueError("compute_gae: %s must be a finite number in [0, 1], got %r" % (name, x))
+        if bootstrap and final_values is None:
+            raise ValueError("compute_gae: bootstrap=True needs final_values (bootstrap=False treats every episode "
+                             "end as terminal)")
+        if final_values is not None:
+            check_tensor("final_values", final_values, (n, N) if episode_length is None
+                         else (T // int(episode_length), n, N))
+        per_agent = False
+        if value_norm is not None:
+            per_agent = torch.is_tensor(value_norm) and value_norm.dim() == 2
+            check_tensor("value_norm", value_norm, (n, 2) if per_agent else (2,))
+        # the env's device as bind() resolves it, so that wrong-device tensors are refused before the world is allocated
+        if world._native is not None:
+            device = world._native.device
+        else:
+            device = torch.device(world.device if world.device is not None else "cuda")
+            if device.type == "cuda" and device.index is None and torch.cuda.is_available():
+                device = torch.device("cuda", torch.cuda.current_device())
+        for name, t in (("rewards", rewards), ("values", values), ("final_values", final_values),
+                        ("value_norm", value_norm)):
+            if t is not None and not (t.is_cuda and t.device == device):
+                raise ValueError("compute_gae: %s must be a CUDA tensor on %s" % (name, device))
+        nw = world.bind()
+        flags = ((_lib.GAE_BOOTSTRAP if bootstrap else 0) | (_lib.GAE_NORMALIZE if normalize_advantages else 0) |
+                 (_lib.GAE_PER_AGENT_VALUE_NORM if per_agent else 0))
+        returns = torch.empty_like(rewards)
+        advantages = torch.empty_like(rewards)
+        ws = None
+        if normalize_advantages:
+            ws = torch.empty((nw.gae_workspace_bytes() + 7) // 8, dtype=torch.float64, device=nw.device)
+        nw.gae(rewards, values, final_values if bootstrap else None, T, episode_length, gamma, gae_lambda, flags,
+               value_norm, returns, advantages, ws)
+        return returns, advantages, (ws[:2] if ws is not None else None)
+
     def _rollout_policy_mlp(self, policies, n_steps, record_actions, per_step_rewards, record_observations, explore_seed,
                             episode_length=None, categorical=False, record_log_probs=False, mappo=False, gru=None,
                             critic=None, rcritic=None):

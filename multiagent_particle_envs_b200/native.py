@@ -323,6 +323,24 @@ class NativeWorld(ShapeHandle):
                                      self._stream())
         check(rc, "mpe_critic_gru")
 
+    def gae_workspace_bytes(self):
+        """bytes of the workspace gae needs to normalise the advantages (mpe_gae_workspace_bytes)"""
+        return check(self.lib.mpe_gae_workspace_bytes(self.handle), "mpe_gae_workspace_bytes")
+
+    def gae(self, rewards, values, final_values, n_steps, episode_length, gamma, gae_lambda, flags, value_norm, returns,
+            advantages, workspace):
+        """MAPPO's GAE and returns (mpe_gae) on the current stream: rewards, values, returns, advantages float32
+        [n_steps, A, N], final_values [E, A, N] (or None without _lib.GAE_BOOTSTRAP), episode_length None (one
+        episode) or L, value_norm None or float32 (mean, std) [2] / [A, 2], workspace None or a tensor of at least
+        gae_workspace_bytes() bytes (with _lib.GAE_NORMALIZE; it then starts with the float64 (mean, std))."""
+        ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
+        rc = self.lib.mpe_gae(self.handle, rewards.data_ptr(), values.data_ptr(), ptr(final_values), int(n_steps),
+                              int(episode_length or 0), float(gamma), float(gae_lambda), int(flags), ptr(value_norm),
+                              returns.data_ptr(), advantages.data_ptr(), ptr(workspace),
+                              workspace.numel() * workspace.element_size() if workspace is not None else 0,
+                              self._stream())
+        check(rc, "mpe_gae")
+
     def rollout_policy_mlp(self, w_ptrs, hidden, n_steps, out=None, flags=0, *, episode_length=None, categorical=False,
                            rew_steps=None, act_rec_ptrs=None, obs_rec_ptrs=None, final_obs_ptrs=None, logp_steps=None,
                            ep_rew=None, explore_seed=None, explore_epoch=0, mappo=None, gru=None, critic=None):

@@ -150,6 +150,14 @@ def main():
         print("|---|---|---|---|---|---|---|---|---|")
         for r in sorted(mlp):
             print("| " + " | ".join(str(x) for x in r) + " |")
+    gae = sorted((names[k].split("(")[0], reg, stack, mix.get(k, {}).get("total", 0)) for k, (reg, stack) in usage.items()
+                 if re.match(r"(void )?mpe::mpe_gae_", names[k]))
+    if gae:
+        print("\n## GAE and returns (`mpe_gae`): the scan without and with the fp64 sums, and the normalisation\n")
+        print("| kernel | regs | stack | instr |")
+        print("|---|---|---|---|")
+        for r in gae:
+            print("| `%s` | %d | %d | %d |" % r)
     other = [(names[k], v) for k, v in usage.items() if "mpe_kernel" not in names[k] or ", 0, " not in names[k]]
     spills = [n for n, (r, s) in other if s]
     print("\nOther kernels with a non-zero stack frame: %s" % (", ".join("`%s`" % s for s in spills) or "none"))
