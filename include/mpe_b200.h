@@ -370,6 +370,43 @@ MPE_API int mpe_rollout_policy_gru_episodes(
     float *rnn_state_dev, float *rnn_state_record_dev, uint32_t net_flags, float ln_eps, uint8_t *done_dev,
     uint32_t flags, void *stream);
 
+/* rMAPPO's separated runner: MAPPO's recurrent actor with agent i's OWN weight set (its own R_Actor), for the programs
+ * whose agents observe or act differently (built for simple_speaker_listener).  The arguments are
+ * mpe_rollout_policy_gru[_episodes]'s with one device pointer per agent for each of the ten folded weights (agent i's
+ * W1 [64][obs_dim_i] ... W3 [act_dim_i][64], b3 [act_dim_i]), plus workspace_dev: at least
+ * mpe_rollout_policy_gru_separated_workspace_bytes(h) bytes, 16-byte aligned, contents on entry irrelevant.  Every
+ * call first writes each agent's TF32 fragment image into the workspace, then runs the rollout, which copies agent i's
+ * image into shared memory (one TMA bulk copy) at agent i's turn of every step: every agent's weights do not fit at
+ * once.  Calls that share a workspace must be ordered on one stream.  rnn_state_dev [A][N][64] and
+ * rnn_state_record_dev [T][A][N][64] are agent i's h at row i, as in the shared form.  Return codes and their order are
+ * mpe_rollout_policy_gru[_episodes]'s: MPE_ERR_UNSUPPORTED at the program check for a program without per-agent
+ * recurrent actors or a hidden width other than 64; MPE_ERR_BAD_ARG with the null weight arrays for a null one of the
+ * ten arrays, with the per-agent weight checks for a null or misaligned agent pointer, and, after the observation
+ * records, for a null, not 16-byte aligned or too small workspace. */
+MPE_API int mpe_rollout_policy_gru_separated(
+    mpe_handle h, void *agent_pv_dev, const void *lm_p_dev, float *comm_dev, const int32_t *goal_dev,
+    const float *const *w1_n, const float *const *b1_n, const float *const *w2_n, const float *const *b2_n,
+    const float *const *w_ih_n, const float *const *b_ih_n, const float *const *w_hh_n, const float *const *b_hh_n,
+    const float *const *w3_n, const float *const *b3_n, int32_t hidden, int32_t n_steps, int32_t explore,
+    uint64_t explore_seed, uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n_dev, float *rew_sum_dev,
+    float *rew_steps_dev, float *logp_steps_dev, int32_t *const *act_index_record_n, float *const *obs_record_n,
+    float *rnn_state_dev, float *rnn_state_record_dev, void *workspace_dev, int64_t workspace_bytes, uint32_t net_flags,
+    float ln_eps, uint8_t *done_dev, uint32_t flags, void *stream);
+MPE_API int mpe_rollout_policy_gru_separated_episodes(
+    mpe_handle h, void *agent_pv_dev, void *lm_p_dev, float *comm_dev, int32_t *goal_dev, const float *const *w1_n,
+    const float *const *b1_n, const float *const *w2_n, const float *const *b2_n, const float *const *w_ih_n,
+    const float *const *b_ih_n, const float *const *w_hh_n, const float *const *b_hh_n, const float *const *w3_n,
+    const float *const *b3_n, int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
+    uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset,
+    float *const *obs_n_dev, float *ep_rew_dev, float *rew_steps_dev, float *logp_steps_dev,
+    int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n,
+    float *rnn_state_dev, float *rnn_state_record_dev, void *workspace_dev, int64_t workspace_bytes, uint32_t net_flags,
+    float ln_eps, uint8_t *done_dev, uint32_t flags, void *stream);
+/* bytes of the separated rollout's workspace: every agent's fragment image, each padded to 16 bytes (speaker_listener:
+ * 120 864 + 122 912 = 243 776).  Needs no device.  MPE_ERR_BAD_ARG for a null handle, MPE_ERR_UNSUPPORTED for a
+ * program without per-agent recurrent actors. */
+MPE_API int64_t mpe_rollout_policy_gru_separated_workspace_bytes(mpe_handle h);
+
 /* MAPPO's MLP actor (mpe_rollout_policy_mappo[_episodes]) with MAPPO's centralized critic (R_Critic with
  * use_centralized_V, non-recurrent, hidden width 64) evaluated in the same launch:
  *     [LN(D)] -> Linear(D, 64) -> act -> LN(64) -> Linear(64, 64) -> act -> LN(64) -> Linear(64, 1)
@@ -429,6 +466,19 @@ MPE_API int mpe_critic_gru(mpe_handle h, const float *const *obs_record_n, const
                            const float *b_hh, const float *w3, const float *b3, float *rnn_state_dev,
                            float *rnn_state_record_dev, float *values_dev, float *final_values_dev,
                            uint32_t net_flags, float ln_eps, void *stream);
+/* rMAPPO's separated runner's critics: agent k's own recurrent critic (R_Critic on share_obs, k = 0 .. A-1), its ten
+ * folded weights at w*_n[k], all A in one launch.  As mpe_critic_gru but: rnn_state_dev is [A][N][64] (critic k's h at
+ * row k), rnn_state_record_dev [n_steps][A][N][64], and values_dev / final_values_dev receive critic k's value in agent
+ * k's row only.  Return codes and their order are mpe_critic_gru's; MPE_ERR_UNSUPPORTED for a program without
+ * per-agent recurrent actors, MPE_ERR_BAD_ARG at the weight check for a null array or a null or misaligned agent
+ * pointer. */
+MPE_API int mpe_critic_gru_separated(mpe_handle h, const float *const *obs_record_n, const float *const *final_obs_n,
+                                     int32_t n_steps, int32_t episode_length, const float *const *w1_n,
+                                     const float *const *b1_n, const float *const *w2_n, const float *const *b2_n,
+                                     const float *const *w_ih_n, const float *const *b_ih_n, const float *const *w_hh_n,
+                                     const float *const *b_hh_n, const float *const *w3_n, const float *const *b3_n,
+                                     float *rnn_state_dev, float *rnn_state_record_dev, float *values_dev,
+                                     float *final_values_dev, uint32_t net_flags, float ln_eps, void *stream);
 
 /* flags of mpe_gae */
 enum mpe_gae_flags {

@@ -129,6 +129,17 @@ _SIGNATURES = {
                                          ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64,
                                          ctypes.c_uint64, _PP, _P, _P, _P, _PP, _PP, _PP, _P, _P, ctypes.c_uint32,
                                          ctypes.c_float, _P, ctypes.c_uint32, _P]),
+    "mpe_rollout_policy_gru_separated": (ctypes.c_int, [_P, _P, _P, _P, _P] + [_PP] * 10 +
+                                         [ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_uint64,
+                                          ctypes.c_uint64, ctypes.c_uint64, _PP, _P, _P, _P, _PP, _PP, _P, _P, _P,
+                                          ctypes.c_int64, ctypes.c_uint32, ctypes.c_float, _P, ctypes.c_uint32, _P]),
+    "mpe_rollout_policy_gru_separated_episodes": (ctypes.c_int, [_P, _P, _P, _P, _P] + [_PP] * 10 +
+                                                  [ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                                   ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64,
+                                                   ctypes.c_uint64, _PP, _P, _P, _P, _PP, _PP, _PP, _P, _P, _P,
+                                                   ctypes.c_int64, ctypes.c_uint32, ctypes.c_float, _P, ctypes.c_uint32,
+                                                   _P]),
+    "mpe_rollout_policy_gru_separated_workspace_bytes": (ctypes.c_int64, [_P]),
     "mpe_rollout_policy_mappo_critic": (ctypes.c_int, [_P, _P, _P, _P, _P, _PP, _PP, _PP, _PP, _PP, _PP, ctypes.c_int32,
                                                        ctypes.c_int32, ctypes.c_int32, ctypes.c_uint64, ctypes.c_uint64,
                                                        ctypes.c_uint64, _PP, _P, _P, _P, _PP, _PP, ctypes.c_uint32,
@@ -143,6 +154,8 @@ _SIGNATURES = {
                                                                 ctypes.c_uint32, _P]),
     "mpe_critic_gru": (ctypes.c_int, [_P, _PP, _PP, ctypes.c_int32, ctypes.c_int32] + [_P] * 10 +
                        [_P, _P, _P, _P, ctypes.c_uint32, ctypes.c_float, _P]),
+    "mpe_critic_gru_separated": (ctypes.c_int, [_P, _PP, _PP, ctypes.c_int32, ctypes.c_int32] + [_PP] * 10 +
+                                 [_P, _P, _P, _P, ctypes.c_uint32, ctypes.c_float, _P]),
     "mpe_gae": (ctypes.c_int, [_P, _P, _P, _P, ctypes.c_int32, ctypes.c_int32, ctypes.c_float, ctypes.c_float,
                                ctypes.c_uint32, _P, _P, _P, _P, ctypes.c_int64, _P]),
     "mpe_gae_workspace_bytes": (ctypes.c_int64, [_P]),

@@ -919,6 +919,24 @@ struct MlpGruEpisodeArgs {
     MlpGruState g;
 };
 static_assert(sizeof(MlpGruEpisodeArgs) <= 4096, "kernel parameter space");
+// Per-agent recurrent actors (mpe_policy_gru_separated[_episode]_kernel): g's state as the shared actor's, agent i's
+// weights in its fragment image at images + GruSeparatedShape::image_off(i) (written by mpe_gru_image_kernel); the
+// weight pointers of g are not read.
+struct MlpGruSeparatedArgs {
+    MlpGruArgs g;
+    const float *images;
+};
+struct MlpGruSeparatedEpisodeArgs {
+    MlpGruEpisodeArgs g;
+    const float *images;
+};
+static_assert(sizeof(MlpGruSeparatedEpisodeArgs) <= 4096, "kernel parameter space");
+// The fragment images' sources: w[j][i] is agent i's W1, b1, W2, b2, W_ih, b_ih, W_hh, b_hh, W3, b3 (j = 0 .. 9,
+// folded as the shared actor's, torch layouts)
+struct GruImageArgs {
+    const float *w[10][kMaxA];
+    float *images;
+};
 
 // MAPPO's centralized critic (R_Critic with use_centralized_V, recurrent off: MLPBase with layer_N = 1, then v_out) next
 // to MAPPO's actor:
@@ -1043,28 +1061,33 @@ template <> struct GruBuilt<Reference> { static constexpr bool value = true; };
 
 // One weight set in shared memory, in floats: B fragments [k-tile][n-tile][lane][2] of W1, W2, W_ih (24 n-tiles: r, z,
 // n), W_hh, the head W3, then b1 [64], b2 [64], b_ih [192], b_hh [192], b3 [NOUT].  Per warp the MLP actor's
-// observation and logit tiles: h and h' stay in registers (one m-tile at a time, see mlp_agent).
-template <class P>
-struct GruShape {
+// observation and logit tiles: h and h' stay in registers (one m-tile at a time, see mlp_agent).  GruAgentShape is the
+// layout for agent I's obs_dim and act_dim; GruShape, the one shared set, is agent 0's.
+template <class P, int I>
+struct GruAgentShape {
     using M = MlpShape<P, 64>;
+    static constexpr int NT = 8, NG = 24;
+    static constexpr int w2_off = 64 * M::kt1(I) * NT;
+    static constexpr int wih_off = w2_off + 64 * NT * NT;
+    static constexpr int whh_off = wih_off + 64 * NT * NG;
+    static constexpr int w3_off = whh_off + 64 * NT * NG;
+    static constexpr int b1_off = w3_off + 64 * NT * (M::nout(I) / 8);
+    static constexpr int b2_off = b1_off + 64;
+    static constexpr int bih_off = b2_off + 64;
+    static constexpr int bhh_off = bih_off + 192;
+    static constexpr int b3_off = bhh_off + 192;
+    static constexpr int kWeightFloats = b3_off + M::nout(I);
+    static constexpr int kImageFloats = (kWeightFloats + 3) & ~3;   // a fragment image: padded to 16 bytes
+};
+template <class P>
+struct GruShape : GruAgentShape<P, 0> {
     static constexpr bool shared_ok() {
         for (int i = 1; i < P::A; ++i)
             if (P::obs_dim(i) != P::obs_dim(0) || P::act_dim(i) != P::act_dim(0)) return false;
         return true;
     }
     static_assert(shared_ok(), "one shared policy: every agent observes and acts alike");
-    static constexpr int NT = 8, NG = 24;
-    static constexpr int w2_off = 64 * M::kt1(0) * NT;
-    static constexpr int wih_off = w2_off + 64 * NT * NT;
-    static constexpr int whh_off = wih_off + 64 * NT * NG;
-    static constexpr int w3_off = whh_off + 64 * NT * NG;
-    static constexpr int b1_off = w3_off + 64 * NT * (M::nout(0) / 8);
-    static constexpr int b2_off = b1_off + 64;
-    static constexpr int bih_off = b2_off + 64;
-    static constexpr int bhh_off = bih_off + 192;
-    static constexpr int b3_off = bhh_off + 192;
-    static constexpr int kWeightFloats = b3_off + M::nout(0);
-    static constexpr int kWarpFloats = M::kWarpFloats;
+    static constexpr int kWarpFloats = MlpShape<P, 64>::kWarpFloats;
 };
 static_assert(GruShape<Simple<1, 1>>::kWeightFloats * 4 == 120864, "simple: 120 864 B of weights");
 static_assert(GruShape<Spread<3>>::kWeightFloats * 4 == 124960, "spread N=3: 124 960 B");
@@ -1080,6 +1103,38 @@ __host__ __device__ constexpr int gru_block_warps() {
                   "8 warps' tiles fit next to the weights");
     return kGruWarps;
 }
+
+// Per-agent recurrent actors (rMAPPO's separated runner: agent i's own R_Actor, MlpGruSeparatedArgs) are built for the
+// programs whose agents observe or act differently, where one shared policy cannot serve: simple_speaker_listener.
+template <class P> struct GruSeparatedBuilt { static constexpr bool value = false; };
+template <> struct GruSeparatedBuilt<SpeakerListener> { static constexpr bool value = true; };
+// Every agent's weight set does not fit in shared memory at once (speaker_listener: 120 864 + 122 912 B against 232 448
+// B), so the block keeps one slot, sized for the largest agent, and restages it at every agent's turn from agent i's
+// fragment image: GruAgentShape<P, i>'s layout, prepared once per call in a global workspace, images back to back.
+template <class P>
+struct GruSeparatedShape {
+    using M = MlpShape<P, 64>;
+    // GruAgentShape<P, i>::kImageFloats for a run-time i (gru_image checks the two agree)
+    __host__ __device__ static constexpr int image_floats(int i) {
+        return (64 * 8 * (M::kt1(i) + 8 + 2 * 24 + M::nout(i) / 8) + 64 + 64 + 192 + 192 + M::nout(i) + 3) & ~3;
+    }
+    __host__ __device__ static constexpr int image_off(int i) { int s = 0; for (int j = 0; j < i; ++j) s += image_floats(j); return s; }
+    static constexpr int kImagesFloats = image_off(P::A);
+    __host__ __device__ static constexpr int slot_floats() { int m = 0; for (int i = 0; i < P::A; ++i) m = image_floats(i) > m ? image_floats(i) : m; return m; }
+    static constexpr int kSlotFloats = slot_floats();
+};
+template <class P>
+__host__ __device__ constexpr int gru_separated_block_warps() {
+    static_assert((GruSeparatedShape<P>::kSlotFloats + kGruWarps * MlpShape<P, 64>::kWarpFloats) * 4 <= kMlpSmemBytes,
+                  "8 warps' tiles fit next to the slot");
+    return kGruWarps;
+}
+static_assert(GruSeparatedShape<SpeakerListener>::image_floats(0) * 4 == 120864 &&
+              GruSeparatedShape<SpeakerListener>::image_floats(1) * 4 == 122912 &&
+              GruSeparatedShape<SpeakerListener>::kImagesFloats * 4 == 243776,
+              "speaker_listener: a 120 864 B speaker and a 122 912 B listener, 243 776 B together");
+static_assert((GruSeparatedShape<SpeakerListener>::kSlotFloats + kGruWarps * MlpShape<SpeakerListener, 64>::kWarpFloats) * 4 ==
+              143392, "speaker_listener: a 122 912 B slot and 8 warps' 2 560 B tiles");
 
 // One critic's weights in shared memory, in floats: B fragments [k-tile][n-tile][lane][2] of W1, agent by agent (agent
 // i's obs_dim_i columns zero-padded to whole k-tiles, so that layer 1 is a sum of k-slices over the agents'
@@ -1164,6 +1219,15 @@ struct RCriticArgs {
     float ln_eps;
 };
 static_assert(sizeof(RCriticArgs) <= 4096, "kernel parameter space");
+// rMAPPO's per-agent recurrent critics (the separated runner: agent k's own R_Critic on share_obs), one launch with
+// blockIdx.y = k: c as above but for the weights, which are w[j][k] (W1, b1, W2, b2, W_ih, b_ih, W_hh, b_hh, W3, b3),
+// and critic k's state, h [A][n][64] and h_rec [T][A][n][64] (or null), its slice k; critic k writes only agent k's row
+// of values and final_values.
+struct RCriticSeparatedArgs {
+    RCriticArgs c;
+    const float *w[10][kMaxA];
+};
+static_assert(sizeof(RCriticSeparatedArgs) <= 4096, "kernel parameter space");
 
 // Its weights in shared memory, in floats: W1's B fragments agent by agent as the MLP critic's (CriticShape::w1_off,
 // stage_critic_w1), then W2, W_ih and W_hh (GruShape's layout), W3 (one n-tile, its one real column first), b1 [64],
@@ -1376,9 +1440,10 @@ __device__ __forceinline__ float categorical_segment(const float (&zs)[N], const
 // the second LayerNorm needs a whole row of h2, layers 2 and 3 run one m-tile at a time (h2 of 16 rows in 32 fp32
 // registers, W2's B fragments read once per m-tile).
 // GRU adds MAPPO's recurrent actor (MlpGruArgs) to MAPPO's: per m-tile the base's two layers, the GRU step, the
-// LayerNorm of h' and the head, so that x, h and h' fit in registers.  The weights are the one shared set (GruShape).
+// LayerNorm of h' and the head, so that x, h and h' fit in registers.  The weights are agent I's set in
+// GruAgentShape<P, I>'s layout: the one shared set (GruShape), or the slot the separated actor restages for agent I.
 //
-// Where the base's second layer, the head and their biases sit in Wsm: the agent's block (MlpShape), or the shared set
+// Where the base's second layer, the head and their biases sit in Wsm: the agent's block (MlpShape), or the GRU set
 template <class P, int H, int I, bool GRU>
 struct AgentWeights {
     using S = MlpShape<P, H>;
@@ -1386,7 +1451,7 @@ struct AgentWeights {
 };
 template <class P, int I>
 struct AgentWeights<P, 64, I, true> {
-    using G = GruShape<P>;
+    using G = GruAgentShape<P, I>;
     static constexpr int w2 = G::w2_off, w3 = G::w3_off, b1 = G::b1_off, b2 = G::b2_off, b3 = G::b3_off;
 };
 template <class P, int H, int I, bool EPISODES = false, bool CATEGORICAL = false, bool MAPPO = false, bool GRU = false>
@@ -1486,7 +1551,7 @@ __device__ __forceinline__ float2 mlp_agent(const MlpPolicyArgs &pa, const typen
     }
     if constexpr (GRU) {   // ---- the recurrent actor, one m-tile (16 worlds) at a time: layers 1 and 2 with their
                            //      LayerNorms -> x, h' = GRU(x, h), logits += LN(h') . W3^T
-        using G = GruShape<P>;
+        using G = GruAgentShape<P, I>;
         const float *Wih = Wsm + G::wih_off, *Whh = Wsm + G::whh_off, *Bih = Wsm + G::bih_off, *Bhh = Wsm + G::bhh_off;
         const bool h_zero = EPISODES && step == 0;         // every episode starts from h = 0
 #pragma unroll
@@ -1861,26 +1926,53 @@ __device__ __forceinline__ void run_critics(const MlpCriticState &cs, const floa
                       rec + (static_cast<int64_t>(row) * P::A + k) * n + w0, slots, n);
 }
 
+// Agent I's turn in the separated recurrent actor (SEPARATED): the whole block waits until every warp is done with the
+// previous agent's weights, then one thread copies agent I's fragment image into the slot with one TMA bulk copy that
+// completes on the mbarrier, and every thread waits for that phase.  phase counts the block's turns mod 2.
+template <class P, int I>
+__device__ __forceinline__ void gru_restage(float *slot, const float *images, uint64_t *bar, uint32_t &phase) {
+    constexpr uint32_t kBytes = GruSeparatedShape<P>::image_floats(I) * 4;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the slot's generic reads before the async write
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(kBytes) : "memory");
+        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                     ::"r"(smem_u32(slot)), "l"(images + GruSeparatedShape<P>::image_off(I)), "r"(kBytes),
+                     "r"(smem_u32(bar)) : "memory");
+    }
+    uint32_t done;
+    do {
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                     : "=r"(done) : "r"(smem_u32(bar)), "r"(phase) : "memory");
+    } while (!done);
+    phase ^= 1u;
+}
+
 // the body of both forms; ea is null in the single-episode form (EPISODES = false), cr unless CATEGORICAL; ln_eps and
 // net_flags are MAPPO's (MlpMappoArgs), gs the recurrent actor's (GRU, MlpGruArgs), cs the critic's (CRITIC,
-// MlpCriticArgs)
+// MlpCriticArgs).  SEPARATED (with GRU) gives every agent its own weight set, restaged into one slot from the fragment
+// images at `images` (GruSeparatedShape) at every agent's turn (gru_restage).
 template <class P, int H, bool EPISODES, bool CATEGORICAL = false, bool MAPPO = false, bool GRU = false,
-          bool CRITIC = false>
+          bool CRITIC = false, bool SEPARATED = false>
 __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEpisodeArgs *ea,
                                             const MlpCategoricalRecords *cr = nullptr, float ln_eps = 0.0f,
                                             uint32_t net_flags = 0, const MlpGruState *gs = nullptr,
-                                            const MlpCriticState *cs = nullptr) {
+                                            const MlpCriticState *cs = nullptr, const float *images = nullptr) {
     static_assert(!CRITIC || (MAPPO && !GRU), "the critic runs next to MAPPO's MLP actor");
+    static_assert(!SEPARATED || GRU, "per-agent weight sets are the recurrent actor's");
     static_assert(H == 32 || H == 64, "MLP policy rollout: hidden width 32 or 64");
     constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     using S = MlpShape<P, H>;
     constexpr int kWarps = [] {
-        if constexpr (GRU) return gru_block_warps<P>();
+        if constexpr (SEPARATED) return gru_separated_block_warps<P>();
+        else if constexpr (GRU) return gru_block_warps<P>();
         else if constexpr (CRITIC) return critic_block_warps<P, EPISODES>();
         else return mlp_block_warps<P, H, EPISODES | (MAPPO ? 2 : CATEGORICAL) << 1>();
     }();
+    constexpr int kSlotOff = SEPARATED ? 4 : 0;   // SEPARATED: the slot's mbarrier, then the slot (16-byte aligned)
     constexpr int kWeightFloats = [] {
-        if constexpr (GRU) return GruShape<P>::kWeightFloats;
+        if constexpr (SEPARATED) return kSlotOff + GruSeparatedShape<P>::kSlotFloats;
+        else if constexpr (GRU) return GruShape<P>::kWeightFloats;
         else return S::kWeightFloats;
     }();
     static_assert(kWarps >= 1 && (kWeightFloats + (CRITIC ? CriticShape<P>::kFloats : 0) + kWarps * S::kWarpFloats) * 4 <=
@@ -1888,7 +1980,11 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
     const StepArgs &a = pa.s;
     extern __shared__ __align__(16) float smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if constexpr (GRU) {   // ---- the one shared weight set -> TF32 B fragments in shared memory, once per block ----
+    uint64_t *const bar = reinterpret_cast<uint64_t *>(smem);   // SEPARATED: the slot's mbarrier
+    uint32_t phase = 0;                                          // SEPARATED: the block's turns mod 2
+    if constexpr (SEPARATED) {    // ---- no weights yet: agent 0's first turn stages them ----
+        if (threadIdx.x == 0) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(bar)) : "memory");
+    } else if constexpr (GRU) {   // ---- the one shared weight set -> TF32 B fragments in shared memory, once per block ----
         using G = GruShape<P>;
         constexpr int OD = P::obs_dim(0), AD = P::act_dim(0);
         stage_fragments<S::kt1(0), G::NT, false>(smem, pa.w1[0], 64, OD);
@@ -1946,7 +2042,16 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
     const int64_t n = a.n;
     const int64_t end = a.begin + a.count;
     const int64_t w0 = a.begin + (static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + warp) * 32;
-    if (w0 >= end) return;
+    if (w0 >= end) {
+        if constexpr (SEPARATED) {   // a warp without worlds still takes part in every turn's barrier
+#pragma unroll 1
+            for (int e = 0; e < (EPISODES ? ea->episodes : 1); ++e)
+#pragma unroll 1
+                for (int t = 0; t < pa.T; ++t)
+                    static_for<A>([&](auto ic) { gru_restage<P, decltype(ic)::value>(smem + kSlotOff, images, bar, phase); });
+        }
+        return;
+    }
     const int rows = (end - w0) < 32 ? static_cast<int>(end - w0) : 32;
     const bool active = lane < rows;
     const int64_t wi = w0 + (active ? lane : 0);   // idle lanes of a partial tile replay world w0: every tile row is finite
@@ -1988,8 +2093,9 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
             if constexpr (CRITIC) run_critics<P>(*cs, Wc, d, w, s_warp, lane, rows, ln_eps, net_flags, cs->values, tg, w0, n);   // V of the state the actors act on
             static_for<A>([&](auto ic) {
                 constexpr int i = decltype(ic)::value;
+                if constexpr (SEPARATED) gru_restage<P, i>(smem + kSlotOff, images, bar, phase);
                 const float2 u = mlp_agent<P, H, i, EPISODES, CATEGORICAL, MAPPO, GRU>(
-                    pa, w, GRU ? smem : smem + S::agent_off(i), s_warp, lane, tg, rows, active, w0, wi, cact, t,
+                    pa, w, GRU ? smem + kSlotOff : smem + S::agent_off(i), s_warp, lane, tg, rows, active, w0, wi, cact, t,
                     pa.epoch + e, cr, ln_eps, net_flags, gs);
                 ux[i] = u.x;
                 uy[i] = u.y;
@@ -2136,6 +2242,56 @@ __global__ void __launch_bounds__(gru_block_warps<P>() * 32)
     mlp_rollout<P, 64, true, true, true, true>(ga.m.c.e.p, &ga.m.c.e, &ga.m.c.c, ga.m.eps, ga.m.net_flags, &ga.g);
 }
 
+// Per-agent recurrent actors: agent i's weight set (GruAgentShape<P, i>) -> TF32 B fragments, the layout the shared
+// actor stages in shared memory, written to its image in global memory.  Block i writes agent i's image.
+template <class P, int I>
+__device__ __forceinline__ void stage_gru_agent(float *dst, const float *const (&w)[10]) {
+    using G = GruAgentShape<P, I>;
+    using S = MlpShape<P, 64>;
+    constexpr int OD = P::obs_dim(I), AD = P::act_dim(I);
+    stage_fragments<S::kt1(I), G::NT, false>(dst, w[0], 64, OD);
+    stage_fragments<G::NT, G::NT, true>(dst + G::w2_off, w[2], 64, 64);
+    stage_fragments<G::NT, G::NG, true>(dst + G::wih_off, w[4], 192, 64);
+    stage_fragments<G::NT, G::NG, true>(dst + G::whh_off, w[6], 192, 64);
+    stage_fragments<G::NT, S::nout(I) / 8, true>(dst + G::w3_off, w[8], AD, 64);
+    for (int q = threadIdx.x; q < 64; q += blockDim.x) {
+        dst[G::b1_off + q] = w[1][q];
+        dst[G::b2_off + q] = w[3][q];
+    }
+    for (int q = threadIdx.x; q < 192; q += blockDim.x) {
+        dst[G::bih_off + q] = w[5][q];
+        dst[G::bhh_off + q] = w[7][q];
+    }
+    for (int q = threadIdx.x; q < G::kImageFloats - G::b3_off; q += blockDim.x) dst[G::b3_off + q] = q < AD ? w[9][q] : 0.0f;
+}
+constexpr int kGruImageThreads = 256;
+template <class P>
+__global__ void __launch_bounds__(kGruImageThreads) mpe_gru_image_kernel(const __grid_constant__ GruImageArgs ia) {
+    static_for<P::A>([&](auto ic) {
+        constexpr int i = decltype(ic)::value;
+        static_assert(GruSeparatedShape<P>::image_floats(i) == GruAgentShape<P, i>::kImageFloats, "one image layout");
+        if (blockIdx.x == i) {
+            const float *const w[10] = {ia.w[0][i], ia.w[1][i], ia.w[2][i], ia.w[3][i], ia.w[4][i],
+                                        ia.w[5][i], ia.w[6][i], ia.w[7][i], ia.w[8][i], ia.w[9][i]};
+            stage_gru_agent<P, i>(ia.images + GruSeparatedShape<P>::image_off(i), w);
+        }
+    });
+}
+
+template <class P>
+__global__ void __launch_bounds__(gru_separated_block_warps<P>() * 32)
+    mpe_policy_gru_separated_kernel(const __grid_constant__ MlpGruSeparatedArgs sa) {
+    mlp_rollout<P, 64, false, true, true, true, false, true>(sa.g.m.c.p, nullptr, &sa.g.m.c.c, sa.g.m.eps, sa.g.m.net_flags,
+                                                             &sa.g.g, nullptr, sa.images);
+}
+
+template <class P>
+__global__ void __launch_bounds__(gru_separated_block_warps<P>() * 32)
+    mpe_policy_gru_separated_episode_kernel(const __grid_constant__ MlpGruSeparatedEpisodeArgs sa) {
+    mlp_rollout<P, 64, true, true, true, true, false, true>(sa.g.m.c.e.p, &sa.g.m.c.e, &sa.g.m.c.c, sa.g.m.eps,
+                                                            sa.g.m.net_flags, &sa.g.g, nullptr, sa.images);
+}
+
 // The recurrent actor's two kernels of program P (episodes = 0, 1).  mpe_gru.cu defines it and so instantiates the 14
 // kernels in a translation unit of their own, which the Makefile compiles alongside this one: in one unit the library
 // took half as long again to build.
@@ -2148,6 +2304,11 @@ const void *critic_kernel(int episodes);
 // instantiates it for the programs of GruBuilt
 template <class P>
 const void *critic_gru_kernel();
+// The per-agent recurrent actors' kernels of program P: 0 the fragment images, 1 the rollout, 2 its episode form, 3
+// rMAPPO's per-agent recurrent critics (RCriticSeparatedArgs).  mpe_gru_separated.cu defines and instantiates it for the
+// programs of GruSeparatedBuilt.
+template <class P>
+const void *gru_separated_kernel(int which);
 
 // MAPPO's GAE over a finished buffer (mpe_gae): one thread per (agent, world) column of [T][A][N], walking t backwards.
 // mpe_gae.cu defines the kernels; gae_kernel(0) is the scan, gae_kernel(1) the scan that also sums the advantages and
@@ -2367,6 +2528,12 @@ struct Program {
     int mlp_weight_floats[2], mlp_warp_floats[2], gru_weight_floats, critic_floats;
     const void *critic_gru_fn;   // rMAPPO's recurrent critic (kRCriticWarps per block), its weights critic_gru_floats
     int critic_gru_floats;
+    // per-agent recurrent actors and critics (GruSeparatedBuilt, gru_separated_kernel): the fragment images' kernel, the
+    // rollout's two forms (kGruWarps per block, a 4-float mbarrier header and gru_sep_slot_floats of slot), the critics
+    // (kRCriticWarps per block, critic_gru_floats each); null where not built
+    const void *gru_sep_fn[4];
+    int gru_sep_slot_floats;
+    int64_t gru_sep_image_bytes;   // all agents' fragment images, the workspace the rollout needs
     int mlp_explore_stride;           // Philox blocks per (step, agent) of its exploration noise
     void (*rollout_fn)(RolloutArgs);   // K-step open-loop rollout
     int rollout_smem;   // dynamic shared memory per WARP of the rollout kernel
@@ -2427,6 +2594,12 @@ static Program make_program() {
     }
     if constexpr (GruBuilt<P>::value) {
         p.critic_gru_fn = critic_gru_kernel<P>();
+        p.critic_gru_floats = RCriticShape<P>::kFloats;
+    }
+    if constexpr (GruSeparatedBuilt<P>::value) {
+        for (int j = 0; j < 4; ++j) p.gru_sep_fn[j] = gru_separated_kernel<P>(j);
+        p.gru_sep_slot_floats = GruSeparatedShape<P>::kSlotFloats;
+        p.gru_sep_image_bytes = static_cast<int64_t>(GruSeparatedShape<P>::kImagesFloats) * 4;
         p.critic_gru_floats = RCriticShape<P>::kFloats;
     }
     p.smem_bytes = Shape<P>::kWarpBytes;  // per warp
@@ -2572,6 +2745,13 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
         if (prog->critic_gru_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->critic_gru_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->critic_gru_floats * 4));
+        for (int j = 1; j < 3; ++j)
+            if (prog->gru_sep_fn[j])
+                CUDA_TRY(cudaFuncSetAttribute(prog->gru_sep_fn[j], cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (4 + prog->gru_sep_slot_floats + kGruWarps * prog->mlp_warp_floats[1]) * 4));
+        if (prog->gru_sep_fn[3])
+            CUDA_TRY(cudaFuncSetAttribute(prog->gru_sep_fn[3], cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          prog->critic_gru_floats * 4));
         if (prog->rollout_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->rollout_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->rollout_smem * max_warps_per_block(prog->rollout_smem)));
@@ -2674,13 +2854,13 @@ extern "C" int64_t mpe_bytes_per_env_step(mpe_handle h) {
 // serialization: the kernel may start while the previous one on the stream is finishing (the step kernels wait for it
 // with griddepcontrol.wait before touching global memory).
 static int launch_kernel(mpe_handle h, const void *fn, int64_t blocks, int threads, size_t smem, void *stream,
-                         void **params, bool pdl, const char *what) {
+                         void **params, bool pdl, const char *what, unsigned blocks_y = 1) {
     if (blocks > 0x7fffffffLL) return MPE_ERR_BAD_ARG;
     int prev = 0;
     CUDA_TRY(cudaGetDevice(&prev));
     if (prev != h->device) CUDA_TRY(cudaSetDevice(h->device));
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(blocks));
+    cfg.gridDim = dim3(static_cast<unsigned>(blocks), blocks_y);
     cfg.blockDim = dim3(static_cast<unsigned>(threads));
     cfg.dynamicSmemBytes = smem;
     cfg.stream = static_cast<cudaStream_t>(stream);
@@ -2933,6 +3113,12 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
 struct MlpCall {
     int form;
     MlpGruState gru;
+    // per-agent recurrent actors (forms 6 and 7 with separated): W_ih, b_ih, W_hh, b_hh one pointer per agent each (the
+    // base and head in w), and the workspace of their fragment images
+    bool separated;
+    const float *const *gru_w[4];
+    void *workspace;
+    int64_t workspace_bytes;
     MlpCriticState critic;
     uint32_t net_flags;
     float ln_eps;
@@ -2967,13 +3153,17 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
         {"mpe_rollout_policy_mappo_critic_episodes", "cudaLaunchKernelExC(rollout_policy_mappo_critic_episodes)"}};
     const bool episodes = c.form & 1, categorical = c.form >= 2, mappo = c.form >= 4;
     const bool gru = c.form == kMlpForms || c.form == kMlpForms + 1, critic = c.form >= kMlpForms + 2;
-    const bool no_weights = !c.w[0] || !c.w[1] || !c.w[2] || !c.w[3] || !c.w[4] || !c.w[5];
+    const bool no_weights = !c.w[0] || !c.w[1] || !c.w[2] || !c.w[3] || !c.w[4] || !c.w[5] ||
+                            (c.separated && (!c.gru_w[0] || !c.gru_w[1] || !c.gru_w[2] || !c.gru_w[3]));
     // the single-episode forms refuse a negative n_steps and null weight arrays before anything else, the episode forms
     // after the device, program and length checks
     if (!h || (!episodes && (c.T < 0 || no_weights))) return MPE_ERR_BAD_ARG;
     if (h->device < 0) return MPE_ERR_NO_DEVICE;
     const int k = c.hidden == 32 ? 0 : (c.hidden == 64 ? 1 : -1);
-    if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || h->prog->mlp[c.form][k].fn == nullptr) return MPE_ERR_UNSUPPORTED;
+    // the per-agent recurrent actors' rollout (hidden width 64 only), else the form's kernel
+    const void *const fn = k < 0 ? nullptr
+                         : c.separated ? (k == 1 ? h->prog->gru_sep_fn[1 + episodes] : nullptr) : h->prog->mlp[c.form][k].fn;
+    if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || fn == nullptr) return MPE_ERR_UNSUPPORTED;
     // 1 (shared) or A critics, whose weights must leave room for a warp's tiles next to the actor's
     int critic_cap = 0;
     if (critic) {
@@ -2993,8 +3183,8 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     if (c.explore && static_cast<int64_t>(c.T) * h->prog->A * h->prog->mlp_explore_stride > static_cast<int64_t>(kExploreTag))
         return MPE_ERR_BAD_ARG;
     if (no_weights || (c.rew_steps != nullptr && !ok4(c.rew_steps))) return MPE_ERR_BAD_ARG;
-    if (gru && (!ok4(c.gru.w_ih) || !ok4(c.gru.b_ih) || !ok4(c.gru.w_hh) || !ok4(c.gru.b_hh) || !ok8(c.gru.h) ||
-                (c.gru.h_rec != nullptr && !ok8(c.gru.h_rec))))
+    if (gru && ((!c.separated && (!ok4(c.gru.w_ih) || !ok4(c.gru.b_ih) || !ok4(c.gru.w_hh) || !ok4(c.gru.b_hh))) ||
+                !ok8(c.gru.h) || (c.gru.h_rec != nullptr && !ok8(c.gru.h_rec))))
         return MPE_ERR_BAD_ARG;
     if (critic) {
         if (!ok4(c.critic.values) || !ok4(c.critic.final_values)) return MPE_ERR_BAD_ARG;
@@ -3003,7 +3193,8 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
                 !ok4(c.critic.w3[q]) || !ok4(c.critic.b3[q]))
                 return MPE_ERR_BAD_ARG;
     }
-    NvtxRange range(kName[c.form][0]);
+    NvtxRange range(!c.separated ? kName[c.form][0]
+                                 : episodes ? "mpe_rollout_policy_gru_separated_episodes" : "mpe_rollout_policy_gru_separated");
     MlpCategoricalRecords cr{};
     if (categorical) {
         if (c.logp_steps != nullptr && !ok4(c.logp_steps)) return MPE_ERR_BAD_ARG;
@@ -3020,6 +3211,9 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     for (int i = 0; i < h->prog->A; ++i) {
         for (int j = 0; j < 6; ++j)
             if (!ok4(c.w[j][i])) return MPE_ERR_BAD_ARG;
+        if (c.separated)
+            for (int j = 0; j < 4; ++j)
+                if (!ok4(c.gru_w[j][i])) return MPE_ERR_BAD_ARG;
         pa.w1[i] = c.w[0][i]; pa.b1[i] = c.w[1][i]; pa.w2[i] = c.w[2][i]; pa.b2[i] = c.w[3][i]; pa.w3[i] = c.w[4][i]; pa.b3[i] = c.w[5][i];
         pa.act_rec[i] = c.act_record_n ? c.act_record_n[i] : nullptr;
         if (pa.act_rec[i] != nullptr && !ok4(pa.act_rec[i])) return MPE_ERR_BAD_ARG;
@@ -3028,6 +3222,8 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
         ea.final_obs[i] = c.final_obs_record_n ? c.final_obs_record_n[i] : nullptr;
         if (c.final_obs_record_n != nullptr && !ok16(ea.final_obs[i])) return MPE_ERR_BAD_ARG;   // every agent's, or none
     }
+    // the fragment images are read by 16-byte bulk copies
+    if (c.separated && (!ok16(c.workspace) || c.workspace_bytes < h->prog->gru_sep_image_bytes)) return MPE_ERR_BAD_ARG;
     pa.T = c.T;
     pa.explore = c.explore ? 1 : 0;
     pa.seed = c.explore_seed;
@@ -3048,14 +3244,34 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     MlpCriticArgs va{ma, c.critic};
     MlpCriticEpisodeArgs vea{mea, c.critic};
     void *const form_args[kMlpForms + 4] = {&pa, &ea, &ca, &cea, &ma, &mea, &ga, &gea, &va, &vea};
-    const void *const fn = h->prog->mlp[c.form][k].fn;
-    int cap = h->prog->mlp[c.form][k].warps;
+    const float *const images = static_cast<const float *>(c.workspace);
+    MlpGruSeparatedArgs sga{ga, images};
+    MlpGruSeparatedEpisodeArgs sgea{gea, images};
+    int cap = c.separated ? kGruWarps : h->prog->mlp[c.form][k].warps;
     if (critic && critic_cap < cap) cap = critic_cap;   // per-agent critics leave fewer warps than the shared one
     // every block stages all agents' weights once, so blocks are as large as possible while every SM still gets work
     const int64_t warps = (h->n + 31) / 32;
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
     if (wpb > cap) wpb = cap;
+    if (c.separated) {   // every agent's fragment image, then the rollout that restages them turn by turn
+        GruImageArgs ia{};
+        for (int i = 0; i < h->prog->A; ++i) {
+            const float *const *src[10] = {c.w[0], c.w[1], c.w[2], c.w[3], c.gru_w[0], c.gru_w[1], c.gru_w[2], c.gru_w[3],
+                                           c.w[4], c.w[5]};
+            for (int j = 0; j < 10; ++j) ia.w[j][i] = src[j][i];
+        }
+        ia.images = static_cast<float *>(c.workspace);
+        void *params[] = {&ia};
+        int r = launch_kernel(h, h->prog->gru_sep_fn[0], h->prog->A, kGruImageThreads, 0, c.stream, params, false,
+                              "cudaLaunchKernelExC(gru_images)");
+        if (r) return r;
+        return launch_persistent(h, fn, warps, wpb, static_cast<size_t>(4 + h->prog->gru_sep_slot_floats) * 4,
+                                 static_cast<size_t>(h->prog->mlp_warp_floats[k]) * 4,
+                                 episodes ? static_cast<void *>(&sgea) : static_cast<void *>(&sga), c.stream,
+                                 episodes ? "cudaLaunchKernelExC(rollout_policy_gru_separated_episodes)"
+                                          : "cudaLaunchKernelExC(rollout_policy_gru_separated)");
+    }
     const int weight_floats = gru ? h->prog->gru_weight_floats
                                   : h->prog->mlp_weight_floats[k] + (critic ? c.critic.count * h->prog->critic_floats : 0);
     return launch_persistent(h, fn, warps, wpb, static_cast<size_t>(weight_floats) * 4,
@@ -3234,6 +3450,68 @@ extern "C" int mpe_rollout_policy_gru_episodes(
     return rollout_policy_gru(h, c, {w1, b1, w2, b2, w_ih, b_ih, w_hh, b_hh, w3, b3}, rnn_state, rnn_state_record);
 }
 
+// Per-agent recurrent actors: the ten per-agent weight arrays -> c.w (base and head) and c.gru_w, and the workspace
+static int rollout_policy_gru_separated(mpe_handle h, MlpCall &c, const float *const *const (&wt)[10], float *rnn_state,
+                                        float *rnn_state_record, void *workspace, int64_t workspace_bytes) {
+    static const int kBaseHead[6] = {0, 1, 2, 3, 8, 9};
+    for (int j = 0; j < 6; ++j) c.w[j] = wt[kBaseHead[j]];
+    for (int j = 0; j < 4; ++j) c.gru_w[j] = wt[4 + j];
+    c.separated = true;
+    c.gru = MlpGruState{nullptr, nullptr, nullptr, nullptr, rnn_state, rnn_state_record};
+    c.workspace = workspace;
+    c.workspace_bytes = workspace_bytes;
+    return rollout_policy_mlp(h, c);
+}
+
+extern "C" int mpe_rollout_policy_gru_separated(
+    mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal, const float *const *w1_n,
+    const float *const *b1_n, const float *const *w2_n, const float *const *b2_n, const float *const *w_ih_n,
+    const float *const *b_ih_n, const float *const *w_hh_n, const float *const *b_hh_n, const float *const *w3_n,
+    const float *const *b3_n, int32_t hidden, int32_t n_steps, int32_t explore, uint64_t explore_seed,
+    uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n, float *rew_sum, float *rew_steps, float *logp_steps,
+    int32_t *const *act_index_record_n, float *const *obs_record_n, float *rnn_state, float *rnn_state_record,
+    void *workspace, int64_t workspace_bytes, uint32_t net_flags, float ln_eps, uint8_t *done, uint32_t flags,
+    void *stream) {
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = kMlpForms; c.T = n_steps; c.episodes = 1; c.rew = rew_sum;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    c.net_flags = net_flags; c.ln_eps = ln_eps;
+    return rollout_policy_gru_separated(h, c, {w1_n, b1_n, w2_n, b2_n, w_ih_n, b_ih_n, w_hh_n, b_hh_n, w3_n, b3_n},
+                                        rnn_state, rnn_state_record, workspace, workspace_bytes);
+}
+
+extern "C" int mpe_rollout_policy_gru_separated_episodes(
+    mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal, const float *const *w1_n, const float *const *b1_n,
+    const float *const *w2_n, const float *const *b2_n, const float *const *w_ih_n, const float *const *b_ih_n,
+    const float *const *w_hh_n, const float *const *b_hh_n, const float *const *w3_n, const float *const *b3_n,
+    int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore, uint64_t explore_seed,
+    uint64_t explore_epoch, uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n,
+    float *ep_rew, float *rew_steps, float *logp_steps, int32_t *const *act_index_record_n, float *const *obs_record_n,
+    float *const *final_obs_record_n, float *rnn_state, float *rnn_state_record, void *workspace, int64_t workspace_bytes,
+    uint32_t net_flags, float ln_eps, uint8_t *done, uint32_t flags, void *stream) {
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = kMlpForms + 1; c.T = episode_length; c.episodes = n_episodes; c.rew = ep_rew;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
+    c.net_flags = net_flags; c.ln_eps = ln_eps;
+    return rollout_policy_gru_separated(h, c, {w1_n, b1_n, w2_n, b2_n, w_ih_n, b_ih_n, w_hh_n, b_hh_n, w3_n, b3_n},
+                                        rnn_state, rnn_state_record, workspace, workspace_bytes);
+}
+
+extern "C" int64_t mpe_rollout_policy_gru_separated_workspace_bytes(mpe_handle h) {
+    if (!h) return MPE_ERR_BAD_ARG;
+    if (h->prog->scenario == MPE_SCN_CUSTOM || h->prog->gru_sep_fn[0] == nullptr) return MPE_ERR_UNSUPPORTED;
+    return h->prog->gru_sep_image_bytes;
+}
+
 // The critics' six weight arrays (W1, b1, W2, b2, W3, b3: critic_count pointers each) and value records -> c.critic
 static int rollout_policy_critic(mpe_handle h, MlpCall &c, int32_t critic_count, const float *const *const (&cw)[6],
                                  float *values, float *final_values) {
@@ -3289,45 +3567,88 @@ extern "C" int mpe_rollout_policy_mappo_critic_episodes(
     return rollout_policy_critic(h, c, critic_count, {cw1, cb1, cw2, cb2, cw3, cb3}, values, final_values);
 }
 
-extern "C" int mpe_critic_gru(mpe_handle h, const float *const *obs_record_n, const float *const *final_obs_n,
-                              int32_t n_steps, int32_t episode_length, const float *w1, const float *b1, const float *w2,
-                              const float *b2, const float *w_ih, const float *b_ih, const float *w_hh, const float *b_hh,
-                              const float *w3, const float *b3, float *rnn_state, float *rnn_state_record, float *values,
-                              float *final_values, uint32_t net_flags, float ln_eps, void *stream) {
+// The checks of the recurrent critics' entry points, in their documented order, and RCriticArgs but for the weights.
+// fn: the program's kernel; weights_ok: every weight pointer non-null and 4-byte aligned.
+static int rcritic_args(mpe_handle h, const void *fn, const float *const *obs_record_n, const float *const *final_obs_n,
+                        int32_t n_steps, int32_t episode_length, bool weights_ok, float *rnn_state,
+                        float *rnn_state_record, float *values, float *final_values, uint32_t net_flags, float ln_eps,
+                        RCriticArgs &a) {
     if (!h || n_steps < 0) return MPE_ERR_BAD_ARG;
     if (h->device < 0) return MPE_ERR_NO_DEVICE;
     const Program *p = h->prog;
-    if (p->scenario == MPE_SCN_CUSTOM || p->critic_gru_fn == nullptr) return MPE_ERR_UNSUPPORTED;
+    if (p->scenario == MPE_SCN_CUSTOM || fn == nullptr) return MPE_ERR_UNSUPPORTED;
     if (episode_length < 0 || (episode_length > 0 && (n_steps < 1 || n_steps % episode_length != 0)))
         return MPE_ERR_BAD_ARG;
     // unknown network flags, or an eps that is negative, NaN or infinite
     if ((net_flags & ~(kMappoFeatureNorm | kMappoTanh)) || !(ln_eps >= 0.0f && ln_eps <= 3.4e38f)) return MPE_ERR_BAD_ARG;
-    const float *const wt[10] = {w1, b1, w2, b2, w_ih, b_ih, w_hh, b_hh, w3, b3};
-    for (int j = 0; j < 10; ++j)
-        if (!ok4(wt[j])) return MPE_ERR_BAD_ARG;
+    if (!weights_ok) return MPE_ERR_BAD_ARG;
     if (!ok8(rnn_state) || (rnn_state_record != nullptr && !ok8(rnn_state_record)) || !ok4(final_values) || !final_obs_n)
         return MPE_ERR_BAD_ARG;
     if (n_steps > 0 && (!ok4(values) || !obs_record_n)) return MPE_ERR_BAD_ARG;
-    RCriticArgs a{};
     for (int i = 0; i < p->A; ++i) {
         if (!ok4(final_obs_n[i]) || (n_steps > 0 && !ok4(obs_record_n[i]))) return MPE_ERR_BAD_ARG;
         a.obs[i] = n_steps > 0 ? obs_record_n[i] : nullptr;
         a.final_obs[i] = final_obs_n[i];
     }
-    a.w1 = w1; a.b1 = b1; a.w2 = w2; a.b2 = b2; a.w_ih = w_ih; a.b_ih = b_ih; a.w_hh = w_hh; a.b_hh = b_hh;
-    a.w3 = w3; a.b3 = b3;
     a.h = rnn_state; a.h_rec = rnn_state_record; a.values = values; a.final_values = final_values;
     a.n = h->n; a.T = n_steps; a.L = episode_length;
     a.net_flags = net_flags; a.ln_eps = ln_eps;
-    NvtxRange range("mpe_critic_gru");
-    const int64_t warps = (h->n + 15) / 16;   // one warp per 16 worlds
+    return MPE_OK;
+}
+
+// one warp per 16 worlds, blocks_y critics
+static int launch_rcritic(mpe_handle h, const void *fn, void *args, unsigned blocks_y, void *stream, const char *what) {
+    const int64_t warps = (h->n + 15) / 16;
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
     if (wpb > kRCriticWarps) wpb = kRCriticWarps;
-    void *params[] = {&a};
-    return launch_kernel(h, p->critic_gru_fn, (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb),
-                         static_cast<size_t>(p->critic_gru_floats) * 4, stream, params, false,
-                         "cudaLaunchKernelExC(critic_gru)");
+    void *params[] = {args};
+    return launch_kernel(h, fn, (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb),
+                         static_cast<size_t>(h->prog->critic_gru_floats) * 4, stream, params, false, what, blocks_y);
+}
+
+extern "C" int mpe_critic_gru(mpe_handle h, const float *const *obs_record_n, const float *const *final_obs_n,
+                              int32_t n_steps, int32_t episode_length, const float *w1, const float *b1, const float *w2,
+                              const float *b2, const float *w_ih, const float *b_ih, const float *w_hh, const float *b_hh,
+                              const float *w3, const float *b3, float *rnn_state, float *rnn_state_record, float *values,
+                              float *final_values, uint32_t net_flags, float ln_eps, void *stream) {
+    const float *const wt[10] = {w1, b1, w2, b2, w_ih, b_ih, w_hh, b_hh, w3, b3};
+    bool weights_ok = true;
+    for (int j = 0; j < 10; ++j) weights_ok = weights_ok && ok4(wt[j]);
+    RCriticArgs a{};
+    int r = rcritic_args(h, h ? h->prog->critic_gru_fn : nullptr, obs_record_n, final_obs_n, n_steps, episode_length,
+                         weights_ok, rnn_state, rnn_state_record, values, final_values, net_flags, ln_eps, a);
+    if (r) return r;
+    a.w1 = w1; a.b1 = b1; a.w2 = w2; a.b2 = b2; a.w_ih = w_ih; a.b_ih = b_ih; a.w_hh = w_hh; a.b_hh = b_hh;
+    a.w3 = w3; a.b3 = b3;
+    NvtxRange range("mpe_critic_gru");
+    return launch_rcritic(h, h->prog->critic_gru_fn, &a, 1, stream, "cudaLaunchKernelExC(critic_gru)");
+}
+
+extern "C" int mpe_critic_gru_separated(mpe_handle h, const float *const *obs_record_n, const float *const *final_obs_n,
+                                        int32_t n_steps, int32_t episode_length, const float *const *w1_n,
+                                        const float *const *b1_n, const float *const *w2_n, const float *const *b2_n,
+                                        const float *const *w_ih_n, const float *const *b_ih_n,
+                                        const float *const *w_hh_n, const float *const *b_hh_n,
+                                        const float *const *w3_n, const float *const *b3_n, float *rnn_state,
+                                        float *rnn_state_record, float *values, float *final_values, uint32_t net_flags,
+                                        float ln_eps, void *stream) {
+    const float *const *const wt[10] = {w1_n, b1_n, w2_n, b2_n, w_ih_n, b_ih_n, w_hh_n, b_hh_n, w3_n, b3_n};
+    RCriticSeparatedArgs sa{};
+    bool weights_ok = h != nullptr;
+    for (int j = 0; j < 10 && weights_ok; ++j) {
+        weights_ok = wt[j] != nullptr;
+        for (int k = 0; weights_ok && k < h->prog->A; ++k) {
+            weights_ok = ok4(wt[j][k]);
+            sa.w[j][k] = wt[j][k];
+        }
+    }
+    int r = rcritic_args(h, h ? h->prog->gru_sep_fn[3] : nullptr, obs_record_n, final_obs_n, n_steps, episode_length,
+                         weights_ok, rnn_state, rnn_state_record, values, final_values, net_flags, ln_eps, sa.c);
+    if (r) return r;
+    NvtxRange range("mpe_critic_gru_separated");
+    return launch_rcritic(h, h->prog->gru_sep_fn[3], &sa, static_cast<unsigned>(h->prog->A), stream,
+                          "cudaLaunchKernelExC(critic_gru_separated)");
 }
 
 static int64_t gae_scan_blocks(const mpe_env *h) { return (h->prog->A * h->n + kGaeThreads - 1) / kGaeThreads; }

@@ -324,6 +324,16 @@ class MultiAgentEnv(_Env):
         None -- T * n * N * 256 bytes.  Records, sampling, log-probabilities, episodes and epochs are the categorical
         mode's.  rnn_states or record_rnn_states with any other actor raise ValueError.
 
+        Per-agent recurrent actors (mpe_rollout_policy_gru_separated, rMAPPO's separated runner): on a program whose
+        agents observe or act differently -- built for simple_speaker_listener -- distinct tuples give every agent its
+        own (base, gru, norm, head), each of the form above for its own obs_dim_i and act_dim_i and folded by
+        rmappo_actor_params([policies[i]], [obs_dim_i], [act_dim_i]) (ValueError naming the agent); the activation,
+        input LayerNorm and eps must be the same for all (ValueError).  rnn_states, the records, extras and episodes are
+        the shared actor's, row i being agent i's h.  Every agent's weights do not fit in shared memory at once, so the
+        call first writes each agent's TF32 fragment image to a workspace and the kernel copies agent i's into shared
+        memory at its turn of every step.  On any other program distinct tuples keep the shared actor's refusal (one
+        shared tuple on speaker_listener raises MpeError).  Every refusal happens before the world is bound.
+
         critic (MAPPO's MLP actor only, mpe_rollout_policy_mappo_critic[_episodes]) evaluates MAPPO's centralized critic
         in the same launch: R_Critic with use_centralized_V and no recurrence, `nn.Sequential([LayerNorm(D)], Linear(D,
         64), Act, LayerNorm(64), Linear(64, 64), Act, LayerNorm(64), Linear(64, 1))`, whose input is share_obs -- every
@@ -360,7 +370,11 @@ class MultiAgentEnv(_Env):
         else is bit-identical to the same call without a critic.  A recurrent critic with any other actor, an
         nn.Sequential critic with the recurrent actor (rMAPPO pairs the actor's and the critic's recurrence) and
         distinct per-agent recurrent critics raise NotImplementedError; critic_rnn_states or record_critic_rnn_states
-        without a recurrent critic raise ValueError."""
+        without a recurrent critic raise ValueError.  With per-agent recurrent actors the critic is a list of n recurrent
+        tuples, one per agent (mpe_critic_gru_separated, the separated runner's R_Critic per agent on share_obs), each
+        folded by rmappo_critic_params: agent k's values and final values come from critic k, critic_rnn_states and
+        extras["final_critic_rnn_states"] are [n, N, 64] and extras["critic_rnn_states"] [T, n, N, 64] (MAPPO's
+        separated rnn_states_critic); a single tuple or a list of another length raises ValueError."""
         import torch
         world = self.world
         if action_mode not in ("softmax", "categorical"):
@@ -405,9 +419,12 @@ class MultiAgentEnv(_Env):
             if critic_rnn_states is not None and episode_length is not None:
                 raise ValueError("rollout_policy: critic_rnn_states cannot be combined with episode_length (every "
                                  "episode starts from h = 0)")
+            sep = None   # rMAPPO's separated runner: distinct tuples on a program with per-agent recurrent actors
+            if any(p is not policies[0] for p in policies) and self._has_gru_separated():
+                sep = self._gru_separated_fold(policies, critic, rnn_states, critic_rnn_states)
             return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
                                             explore_seed, episode_length, True, record_log_probs, mappo=True,
-                                            gru=(rnn_states, record_rnn_states),
+                                            gru=(rnn_states, record_rnn_states, sep),
                                             rcritic=(critic, critic_rnn_states, record_critic_rnn_states)
                                             if critic is not None else None)
         if rnn_states is not None or record_rnn_states:
@@ -466,6 +483,61 @@ class MultiAgentEnv(_Env):
         world._obs_valid = False
         info_n = {'n': [{} for _ in range(self.n)]}
         return list(out.obs), list(out.rew_list), list(out.done_list), info_n, {"actions": actions, "rewards": rew_steps}
+
+    def _has_gru_separated(self):
+        """does the library have per-agent recurrent actors for this program?  (Asked without a device.)"""
+        try:
+            self.world.native_shapes().require_gru_separated()
+        except _lib.MpeError:
+            return False
+        return True
+
+    def _device(self):
+        """the env's device as bind() resolves it, without binding"""
+        import torch
+        world = self.world
+        if world._native is not None:
+            return world._native.device
+        device = torch.device(world.device if world.device is not None else "cuda")
+        if device.type == "cuda" and device.index is None and torch.cuda.is_available():
+            device = torch.device("cuda", torch.cuda.current_device())
+        return device
+
+    def _gru_separated_fold(self, policies, critic, rnn_states, critic_rnn_states):
+        """rMAPPO's separated runner, checked before the world is bound: every agent's actor folded by
+        rmappo_actor_params on its own sizes, every agent's critic (a list of n recurrent tuples) by
+        rmappo_critic_params, one activation, input LayerNorm and eps for all, and the two state tensors [n, N, 64].
+        Returns (actor params per agent, (tanh, feature_norm, eps), critic params per agent or None)."""
+        import torch
+        shapes = self.world.native_shapes()
+        n, N = self.n, shapes.n_env
+        actors = []
+        for i, pol in enumerate(policies):
+            try:
+                actors.append(rmappo_actor_params([pol], [shapes.obs_dims[i]], [shapes.act_dims[i]]))
+            except ValueError as e:
+                raise ValueError("rollout_policy: agent %d's recurrent actor: %s" % (i, e)) from None
+        net = actors[0][1:]
+        if any(a[1:] != net for a in actors):
+            raise ValueError("rollout_policy: every agent's recurrent actor must use the same activation, input "
+                             "LayerNorm and eps; got %s" % [("Tanh" if a[1] else "ReLU", a[2], a[3]) for a in actors])
+        critics = None
+        if critic is not None:
+            if _is_recurrent(critic) or not (isinstance(critic, (list, tuple)) and len(critic) == n):
+                raise ValueError("rollout_policy: per-agent recurrent actors take a list of %d recurrent critics, one "
+                                 "per agent (rMAPPO's separated runner)" % n)
+            critics = [rmappo_critic_params(c, shapes.obs_dims) for c in critic]
+            if any(c[1:] != net for c in critics):
+                raise ValueError("rollout_policy: every critic must use the actors' activation, input LayerNorm and "
+                                 "eps (%s, %s, %g)" % ("Tanh" if net[0] else "ReLU", net[1], net[2]))
+        device = self._device()
+        for name, t in (("rnn_states", rnn_states), ("critic_rnn_states", critic_rnn_states)):
+            if t is not None and not (torch.is_tensor(t) and tuple(t.shape) == (n, N, MAPPO_HIDDEN)
+                                      and t.dtype == torch.float32 and t.device == device):
+                raise ValueError("rollout_policy: %s must be a float32 tensor %s on %s; got %s"
+                                 % (name, [n, N, MAPPO_HIDDEN], device, (tuple(t.shape), t.dtype, t.device)
+                                    if torch.is_tensor(t) else type(t).__name__))
+        return [a[0] for a in actors], net, (None if critics is None else [c[0] for c in critics])
 
     def compute_gae(self, rewards, values, final_values=None, gamma=0.99, gae_lambda=0.95, episode_length=None,
                     bootstrap=True, value_norm=None, normalize_advantages=False):
@@ -537,12 +609,7 @@ class MultiAgentEnv(_Env):
             per_agent = torch.is_tensor(value_norm) and value_norm.dim() == 2
             check_tensor("value_norm", value_norm, (n, 2) if per_agent else (2,))
         # the env's device as bind() resolves it, so that wrong-device tensors are refused before the world is allocated
-        if world._native is not None:
-            device = world._native.device
-        else:
-            device = torch.device(world.device if world.device is not None else "cuda")
-            if device.type == "cuda" and device.index is None and torch.cuda.is_available():
-                device = torch.device("cuda", torch.cuda.current_device())
+        device = self._device()
         for name, t in (("rewards", rewards), ("values", values), ("final_values", final_values),
                         ("value_norm", value_norm)):
             if t is not None and not (t.is_cuda and t.device == device):
@@ -568,13 +635,16 @@ class MultiAgentEnv(_Env):
         N, T = nw.n_env, int(n_steps)
         nw.require_mlp_actor()   # a program without the kernel is refused as such, before its heads are checked
         rnn = None
-        if gru is not None:      # MAPPO's recurrent actor: gru = (rnn_states, record_rnn_states)
-            nw.require_gru_actor()
-            params, tanh, feature_norm, eps = rmappo_actor_params(policies, nw.obs_dims, nw.act_dims)
-            params = [params]    # one shared set
+        if gru is not None:      # MAPPO's recurrent actor: gru = (rnn_states, record_rnn_states, separated fold)
+            h0, record, sep = gru
+            if sep is None:
+                nw.require_gru_actor()
+                params, tanh, feature_norm, eps = rmappo_actor_params(policies, nw.obs_dims, nw.act_dims)
+                params = [params]    # one shared set
+            else:                # every agent's own set (_gru_separated_fold)
+                params, (tanh, feature_norm, eps), rparams = sep
             hidden = MAPPO_HIDDEN
             net = ((_lib.MAPPO_FEATURE_NORM if feature_norm else 0) | (_lib.MAPPO_TANH if tanh else 0), eps)
-            h0, record = gru
             shape = (self.n, N, MAPPO_HIDDEN)
             if h0 is not None:
                 if not (torch.is_tensor(h0) and tuple(h0.shape) == shape and h0.dtype == torch.float32
@@ -588,16 +658,19 @@ class MultiAgentEnv(_Env):
             else:                # every episode starts from h = 0 without reading the buffer
                 h = torch.empty(shape, dtype=torch.float32, device=nw.device)
             rnn = (h, torch.empty((T,) + shape, dtype=torch.float32, device=nw.device) if record else None)
+            if sep is not None:  # the workspace of the agents' fragment images
+                rnn += (torch.empty(nw.gru_separated_workspace_bytes() // 4, dtype=torch.float32, device=nw.device),)
             if rcritic is not None:   # rMAPPO's recurrent critic: rcritic = (critic, critic_rnn_states, record)
                 rmodule, ch0, crecord = rcritic
-                rparams, ctanh, cfn, ceps = rmappo_critic_params(rmodule, nw.obs_dims)
-                if (ctanh, cfn, ceps) != (tanh, feature_norm, eps):
-                    raise ValueError("rollout_policy: the critic must use the actor's activation, input LayerNorm and "
-                                     "eps (%s, %s, %g); got (%s, %s, %g)"
-                                     % ("Tanh" if tanh else "ReLU", feature_norm, eps, "Tanh" if ctanh else "ReLU", cfn,
-                                        ceps))
-                nw.require_critic_gru()
-                cshape = (N, MAPPO_HIDDEN)
+                if sep is None:
+                    rparams, ctanh, cfn, ceps = rmappo_critic_params(rmodule, nw.obs_dims)
+                    if (ctanh, cfn, ceps) != (tanh, feature_norm, eps):
+                        raise ValueError("rollout_policy: the critic must use the actor's activation, input LayerNorm "
+                                         "and eps (%s, %s, %g); got (%s, %s, %g)"
+                                         % ("Tanh" if tanh else "ReLU", feature_norm, eps, "Tanh" if ctanh else "ReLU",
+                                            cfn, ceps))
+                    nw.require_critic_gru()
+                cshape = (N, MAPPO_HIDDEN) if sep is None else (self.n, N, MAPPO_HIDDEN)
                 if ch0 is not None:
                     if not (torch.is_tensor(ch0) and tuple(ch0.shape) == cshape and ch0.dtype == torch.float32
                             and ch0.device == torch.device(nw.device)):
@@ -609,7 +682,11 @@ class MultiAgentEnv(_Env):
                     ch = torch.zeros(cshape, dtype=torch.float32, device=nw.device)
                 else:            # every episode starts from h = 0 without reading the buffer
                     ch = torch.empty(cshape, dtype=torch.float32, device=nw.device)
-                rkeep = [t.to(device=nw.device, dtype=torch.float32).contiguous() for t in rparams]
+                if sep is None:
+                    rkeep = [t.to(device=nw.device, dtype=torch.float32).contiguous() for t in rparams]
+                else:            # critic k's ten weights; the kernel takes one pointer array per weight
+                    ckeep = [[t.to(device=nw.device, dtype=torch.float32).contiguous() for t in p] for p in rparams]
+                    rkeep = [_lib.ptr_array([ckeep[k][j].data_ptr() for k in range(self.n)]) for j in range(10)]
                 rcrit = (ch, torch.empty((T,) + cshape, dtype=torch.float32, device=nw.device) if crecord else None)
         elif mappo:
             params, tanh, feature_norm, eps = mappo_actor_params(policies, nw.obs_dims, nw.act_dims)
@@ -627,10 +704,10 @@ class MultiAgentEnv(_Env):
             params, hidden = mlp_actor_params(policies, nw.obs_dims, nw.act_dims)
             net = None
         keep = [[t.detach().to(device=nw.device, dtype=torch.float32).contiguous() for t in p] for p in params]
-        if rnn is not None:
+        if rnn is not None and len(rnn) == 2:
             w_ptrs = [t.data_ptr() for t in keep[0]]
-        else:
-            w_ptrs = [_lib.ptr_array([keep[i][j].data_ptr() for i in range(self.n)]) for j in range(6)]
+        else:   # one pointer per agent for each weight
+            w_ptrs = [_lib.ptr_array([keep[i][j].data_ptr() for i in range(self.n)]) for j in range(len(keep[0]))]
         out = nw.out if self.reuse_buffers else nw.new_outputs()
         dev = dict(dtype=torch.float32, device=nw.device)
         crit = None
@@ -667,13 +744,17 @@ class MultiAgentEnv(_Env):
                               logp_steps=log_probs, ep_rew=ep_rew, explore_seed=seed, explore_epoch=self.explore_epoch,
                               mappo=net, gru=rnn, critic=crit)
         if rnn is not None:
-            extras["final_rnn_states"], extras["rnn_states"] = rnn
+            extras["final_rnn_states"], extras["rnn_states"] = rnn[:2]
         if rcritic is not None:   # on the same stream, after the rollout that wrote its input records
             values = torch.empty((T, self.n, N), **dev)
             final_values = torch.empty((self.n, N) if episode_length is None else (E, self.n, N), **dev)
-            nw.critic_gru([t.data_ptr() for t in rkeep], obs_ptrs,
-                          out.obs_ptrs if final is None else _lib.ptr_array([o.data_ptr() for o in final]), T,
-                          episode_length, rcrit[0], rcrit[1], values, final_values, net)
+            final_ptrs = out.obs_ptrs if final is None else _lib.ptr_array([o.data_ptr() for o in final])
+            if sep is None:
+                nw.critic_gru([t.data_ptr() for t in rkeep], obs_ptrs, final_ptrs, T, episode_length, rcrit[0],
+                              rcrit[1], values, final_values, net)
+            else:
+                nw.critic_gru_separated(rkeep, obs_ptrs, final_ptrs, T, episode_length, rcrit[0], rcrit[1], values,
+                                        final_values, net)
             extras["values"], extras["final_values"] = values, final_values
             extras["final_critic_rnn_states"], extras["critic_rnn_states"] = rcrit
         if crit is not None:

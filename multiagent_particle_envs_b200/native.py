@@ -41,6 +41,17 @@ class ShapeHandle(object):
         self.bytes_per_env_step = lib.mpe_bytes_per_env_step(h)
         self._speakers = [i for i in range(self.n_agents) if not desc.agent_silent[i]]
 
+    def gru_separated_workspace_bytes(self):
+        """bytes of the per-agent recurrent actors' workspace, every agent's fragment image
+        (mpe_rollout_policy_gru_separated_workspace_bytes); MpeError for a program without them.  Needs no device."""
+        return check(self.lib.mpe_rollout_policy_gru_separated_workspace_bytes(self.handle),
+                     "mpe_rollout_policy_gru_separated_workspace_bytes")
+
+    def require_gru_separated(self):
+        """MpeError unless the library has per-agent recurrent actors and critics (rMAPPO's separated runner) for this
+        program.  The device-less workspace query answers it."""
+        self.gru_separated_workspace_bytes()
+
     def speaker_slot(self, agent_index):
         """row block of agent `agent_index` in the comm tensors, or -1 if the agent is silent"""
         try:
@@ -323,6 +334,18 @@ class NativeWorld(ShapeHandle):
                                      self._stream())
         check(rc, "mpe_critic_gru")
 
+    def critic_gru_separated(self, w_ptrs, obs_rec_ptrs, final_obs_ptrs, n_steps, episode_length, rnn_state, rnn_record,
+                             values, final_values, net):
+        """rMAPPO's per-agent recurrent critics (mpe_critic_gru_separated) as critic_gru, but w_ptrs are ten pointer
+        arrays (critic k's weight at entry k), rnn_state is float32 [A, N, 64] and rnn_record [n_steps, A, N, 64] or
+        None, and critic k writes only agent k's values."""
+        rc = self.lib.mpe_critic_gru_separated(self.handle, obs_rec_ptrs, final_obs_ptrs, int(n_steps),
+                                               int(episode_length or 0), *w_ptrs, rnn_state.data_ptr(),
+                                               rnn_record.data_ptr() if rnn_record is not None else None,
+                                               values.data_ptr(), final_values.data_ptr(), int(net[0]), float(net[1]),
+                                               self._stream())
+        check(rc, "mpe_critic_gru_separated")
+
     def gae_workspace_bytes(self):
         """bytes of the workspace gae needs to normalise the advantages (mpe_gae_workspace_bytes)"""
         return check(self.lib.mpe_gae_workspace_bytes(self.handle), "mpe_gae_workspace_bytes")
@@ -365,7 +388,9 @@ class NativeWorld(ShapeHandle):
         then the ten device pointers of its one shared folded weight set (W1, b1, W2, b2, W_ih, b_ih, W_hh, b_hh, W3,
         b3; environment.rmappo_actor_params); rnn_state, a float32 [A, N, 64] CUDA tensor, holds the initial hidden
         state and receives the final one, and rnn_record (float32 [n_steps, A, N, 64], or None) the h each step
-        consumed.
+        consumed.  gru=(rnn_state, rnn_record, workspace) (mpe_rollout_policy_gru_separated[_episodes]): every agent's
+        own recurrent actor; w_ptrs is then ten pointer arrays, agent i's folded weight at entry i, and workspace a
+        16-byte aligned CUDA tensor of at least gru_separated_workspace_bytes() bytes.
 
         critic=(count, cw_ptrs, values, final_values) with mappo (mpe_rollout_policy_mappo_critic[_episodes]): MAPPO's
         centralized critic next to the actor.  count is 1 (one shared critic) or A; cw_ptrs the six pointer arrays of
@@ -393,9 +418,12 @@ class NativeWorld(ShapeHandle):
             net = (int(mappo[0]), float(mappo[1]), int(critic[0]), *critic[1], critic[2].data_ptr(),
                    critic[3].data_ptr())
         elif gru is not None:
-            name = "mpe_rollout_policy_gru" + ("_episodes" if episodes else "")
+            separated = len(gru) == 3
+            name = "mpe_rollout_policy_gru" + ("_separated" if separated else "") + ("_episodes" if episodes else "")
             net = (int(mappo[0]), float(mappo[1]))
             rnn = (gru[0].data_ptr(), gru[1].data_ptr() if gru[1] is not None else None)
+            if separated:
+                rnn += (gru[2].data_ptr(), gru[2].numel() * gru[2].element_size())
         elif mappo is not None:
             name = "mpe_rollout_policy_mappo" + ("_episodes" if episodes else "")
             net = (int(mappo[0]), float(mappo[1]))

@@ -27,6 +27,11 @@
       "kernel_then_torch_critic" (that rollout, then the torch critic under no_grad in its fastest form: base over
       [T N, D] in one call, one cuDNN nn.GRU call over the [T, N, 64] sequence, norm and v_out, plus the bootstrap step
       on the returned observations);
+      --separated (with --actor rmappo, simple_speaker_listener): rMAPPO's separated runner, a distinct tuple per agent
+      (mpe_rollout_policy_gru_separated, which restages each agent's weights into shared memory at its turn), and with
+      --critic recurrent a distinct critic per agent (mpe_critic_gru_separated; the torch arm runs each critic in turn).
+      The restaging traffic per step is reported as computed, not measured: blocks x the sum of the agents' fragment
+      image bytes (restage_bytes_per_step);
   (b) the same actors as torch modules + env.step, all captured in one CUDA graph (rollout.GraphedRollout); with
       --categorical the graphed policy takes argmax(logits - log(-log u)) per sub-space, its one_hot and
       log_softmax(logits).gather(k) for the log-probabilities.  With --actor rmappo the graphed policy evaluates the
@@ -122,10 +127,14 @@ def time_rcritic(args, env, mods, kw, res, e0, e1):
     n, T, H, D = args.num_envs, args.steps, args.hidden, sum(nw.obs_dims)
     dev = mods[0][0][-1].weight.device
     Act = nn.Tanh if args.tanh else nn.ReLU
-    base = nn.Sequential(*(([nn.LayerNorm(D)] if args.feature_norm else []) +
-                           [nn.Linear(D, H), Act(), nn.LayerNorm(H), nn.Linear(H, H), Act(), nn.LayerNorm(H)]))
-    critic = tuple(m.to(dev) for m in (base, nn.GRU(H, H), nn.LayerNorm(H), nn.Linear(H, 1)))
-    b, gru, norm, v_out = critic
+
+    def make():
+        base = nn.Sequential(*(([nn.LayerNorm(D)] if args.feature_norm else []) +
+                               [nn.Linear(D, H), Act(), nn.LayerNorm(H), nn.Linear(H, H), Act(), nn.LayerNorm(H)]))
+        return tuple(m.to(dev) for m in (base, nn.GRU(H, H), nn.LayerNorm(H), nn.Linear(H, 1)))
+
+    crits = [make() for _ in (nw.obs_dims if args.separated else [0])]   # one per agent, or one shared
+    critic = crits if args.separated else crits[0]
     h0 = torch.zeros(1, n, H, device=dev)
 
     def in_kernel():
@@ -138,10 +147,11 @@ def time_rcritic(args, env, mods, kw, res, e0, e1):
         obs_n, _, _, _, ex = recording()
         x = torch.cat(ex["observations"], -1).reshape(T * n, D)
         with torch.no_grad():
-            out, hT = gru(b(x).reshape(T, n, H), h0)
-            v_out(norm(out))
-            _, hb = gru(b(torch.cat(list(obs_n), -1))[None], hT)
-            v_out(norm(hb[0]))
+            for b, gru, norm, v_out in crits:
+                out, hT = gru(b(x).reshape(T, n, H), h0)
+                v_out(norm(out))
+                _, hb = gru(b(torch.cat(list(obs_n), -1))[None], hT)
+                v_out(norm(hb[0]))
 
     def timed(fn):
         for _ in range(2):
@@ -184,6 +194,8 @@ def main():
                          "--categorical)")
     ap.add_argument("--tanh", action="store_true", help="MAPPO's actor with Tanh instead of ReLU")
     ap.add_argument("--feature-norm", action="store_true", help="MAPPO's actor with the input LayerNorm")
+    ap.add_argument("--separated", action="store_true",
+                    help="rMAPPO's separated runner: one recurrent actor (and critic) per agent (--actor rmappo)")
     ap.add_argument("--critic", choices=("shared", "separated", "recurrent"),
                     help="time MAPPO's centralized critic in-kernel against the torch critic after the rollout "
                          "(shared, separated: --actor mappo; recurrent: --actor rmappo)")
@@ -192,6 +204,8 @@ def main():
         ap.error("--critic shared|separated needs --actor mappo")
     if args.critic == "recurrent" and args.actor != "rmappo":
         ap.error("--critic recurrent needs --actor rmappo")
+    if args.separated and args.actor != "rmappo":
+        ap.error("--separated needs --actor rmappo")
     if args.actor in ("mappo", "rmappo"):
         args.layers, args.categorical = 3, True
     elif args.tanh or args.feature_norm:
@@ -234,11 +248,16 @@ def main():
         nn = torch.nn
         torch.set_float32_matmul_precision("highest")
         Act = nn.Tanh if args.tanh else nn.ReLU
-        od, ad = nw.obs_dims[0], nw.act_dims[0]
-        base = nn.Sequential(*(([nn.LayerNorm(od)] if args.feature_norm else []) +
-                               [nn.Linear(od, H), Act(), nn.LayerNorm(H), nn.Linear(H, H), Act(), nn.LayerNorm(H)]))
-        actor = tuple(m.to(dev) for m in (base, nn.GRU(H, H), nn.LayerNorm(H), nn.Linear(H, ad)))
-        mods = [actor] * len(nw.obs_dims)
+
+        def make(od, ad):
+            base = nn.Sequential(*(([nn.LayerNorm(od)] if args.feature_norm else []) +
+                                   [nn.Linear(od, H), Act(), nn.LayerNorm(H), nn.Linear(H, H), Act(), nn.LayerNorm(H)]))
+            return tuple(m.to(dev) for m in (base, nn.GRU(H, H), nn.LayerNorm(H), nn.Linear(H, ad)))
+
+        if args.separated:
+            mods = [make(od, ad) for od, ad in zip(nw.obs_dims, nw.act_dims)]
+        else:
+            mods = [make(nw.obs_dims[0], nw.act_dims[0])] * len(nw.obs_dims)
         rnn = torch.zeros(len(nw.obs_dims) * n, H, device=dev)    # the graphed loop's carried h, agents stacked
     segs = sub_spaces(env.world) if args.layers == 3 else [[5]] * len(nw.obs_dims)
     res = {"config": {"scenario": args.scenario, "scenario_kwargs": skw, "n_env": n, "T": T, "hidden": H}}
@@ -247,6 +266,12 @@ def main():
                              torch_float32_matmul_precision=torch.get_float32_matmul_precision())
     if args.actor in ("mappo", "rmappo"):
         res["config"].update(actor=args.actor, tanh=args.tanh, feature_norm=args.feature_norm)
+    if args.separated:   # computed from the launch shape the library picks (8-warp blocks), not measured
+        warps, sms = (n + 31) // 32, torch.cuda.get_device_properties(dev).multi_processor_count
+        wpb = min(8, max(1, (warps + sms - 1) // sms))
+        image_bytes = nw.gru_separated_workspace_bytes()
+        res["config"].update(separated=True, image_bytes=image_bytes,
+                             restage_bytes_per_step=(warps + wpb - 1) // wpb * image_bytes)
     kw = {"explore_seed": 1} if args.explore else {}
     if args.categorical:
         kw.update(action_mode="categorical", record_actions=True, record_log_probs=True)
@@ -267,8 +292,10 @@ def main():
     if args.critic:
         res["config"].update(critic=args.critic)
         timer = time_rcritic if args.critic == "recurrent" else time_critic
-        print(json.dumps(timer(args, env, mods, kw, res, e0, e1)))
-        return
+        res = timer(args, env, mods, kw, res, e0, e1)
+        if not args.separated:   # the separated runner's critic arms go with its rollout arms, in the same run
+            print(json.dumps(res))
+            return
     sec = time_in_kernel(mods)
     res["in_kernel"] = {"us_per_step": 1e6 * sec, "env_steps_per_sec": n / sec}
     if maddpg_mods is not None:   # the MADDPG categorical kernel on the same env, same sizes
@@ -298,9 +325,24 @@ def main():
 
     logps = []   # the graph's log-probability outputs, kept as a trainer would keep them
 
+    def separated_policy(obs_n):   # each agent's own tuple on its own observations and its slice of rnn
+        F = torch.nn.functional
+        out = []
+        for i, ((base, gru, norm, head), o, seg) in enumerate(zip(mods, obs_n, segs)):
+            h = rnn[i * n:(i + 1) * n]
+            gi = F.linear(base(o), gru.weight_ih_l0, gru.bias_ih_l0).chunk(3, 1)
+            gh = F.linear(h, gru.weight_hh_l0, gru.bias_hh_l0).chunk(3, 1)
+            r, z = torch.sigmoid(gi[0] + gh[0]), torch.sigmoid(gi[1] + gh[1])
+            hn = (1 - z) * torch.tanh(gi[2] + r * gh[2]) + z * h
+            h.copy_(hn)
+            out.append(categorical(head(norm(hn)), seg))
+        return out
+
     def recurrent_policy(obs_n):
         # torch's GRU step written out (F.linear GEMMs and pointwise kernels capture in a graph on every backend)
         F = torch.nn.functional
+        if args.separated:
+            return separated_policy(obs_n)
         base, gru, norm, head = mods[0]
         gi = F.linear(base(torch.cat(obs_n, 0)), gru.weight_ih_l0, gru.bias_ih_l0).chunk(3, 1)
         gh = F.linear(rnn, gru.weight_hh_l0, gru.bias_hh_l0).chunk(3, 1)
