@@ -440,6 +440,34 @@ MPE_API int mpe_rollout_policy_mappo_critic_episodes(
     uint32_t net_flags, float ln_eps, int32_t critic_count, const float *const *cw1_n, const float *const *cb1_n,
     const float *const *cw2_n, const float *const *cb2_n, const float *const *cw3_n, const float *const *cb3_n,
     float *values_dev, float *final_values_dev, uint8_t *done_dev, uint32_t flags, void *stream);
+/* MAPPO's MLP actor with IPPO's local critics (MAPPO with use_centralized_V = False) in the same launch: agent k's
+ * critic is the critic above on its own raw observation, D = obs_dim_k (cw1_n[k] is [64][obs_dim_k]).  critic_count 1:
+ * one shared critic evaluated once per agent on that agent's observation, which needs every obs_dim_i equal;
+ * critic_count A: agent k's own critic.  values_dev[t][k][w] = V_k(o_t^k), final_values_dev as
+ * mpe_rollout_policy_mappo_critic[_episodes]'s.  Parameters, semantics and return codes are
+ * mpe_rollout_policy_mappo_critic[_episodes]'s, in the same order, except that MPE_ERR_UNSUPPORTED names a program
+ * without these kernels (simple_tag 4+2 and 6+2, simple_world_comm) or critics that leave no room for a warp
+ * (critic_count A on simple_spread N = 5 and 6), and that MPE_ERR_BAD_ARG at the critic_count check also refuses
+ * critic_count 1 on a program whose agents' obs_dims differ. */
+MPE_API int mpe_rollout_policy_mappo_local_critic(
+    mpe_handle h, void *agent_pv_dev, const void *lm_p_dev, float *comm_dev, const int32_t *goal_dev,
+    const float *const *w1_n, const float *const *b1_n, const float *const *w2_n, const float *const *b2_n,
+    const float *const *w3_n, const float *const *b3_n, int32_t hidden, int32_t n_steps, int32_t explore,
+    uint64_t explore_seed, uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n_dev, float *rew_sum_dev,
+    float *rew_steps_dev, float *logp_steps_dev, int32_t *const *act_index_record_n, float *const *obs_record_n,
+    uint32_t net_flags, float ln_eps, int32_t critic_count, const float *const *cw1_n, const float *const *cb1_n,
+    const float *const *cw2_n, const float *const *cb2_n, const float *const *cw3_n, const float *const *cb3_n,
+    float *values_dev, float *final_values_dev, uint8_t *done_dev, uint32_t flags, void *stream);
+MPE_API int mpe_rollout_policy_mappo_local_critic_episodes(
+    mpe_handle h, void *agent_pv_dev, void *lm_p_dev, float *comm_dev, int32_t *goal_dev, const float *const *w1_n,
+    const float *const *b1_n, const float *const *w2_n, const float *const *b2_n, const float *const *w3_n,
+    const float *const *b3_n, int32_t hidden, int32_t episode_length, int32_t n_episodes, int32_t explore,
+    uint64_t explore_seed, uint64_t explore_epoch, uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset,
+    float *const *obs_n_dev, float *ep_rew_dev, float *rew_steps_dev, float *logp_steps_dev,
+    int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n,
+    uint32_t net_flags, float ln_eps, int32_t critic_count, const float *const *cw1_n, const float *const *cb1_n,
+    const float *const *cw2_n, const float *const *cb2_n, const float *const *cw3_n, const float *const *cb3_n,
+    float *values_dev, float *final_values_dev, uint8_t *done_dev, uint32_t flags, void *stream);
 
 /* rMAPPO's recurrent centralized critic (R_Critic with use_recurrent_policy, recurrent_N = 1, use_centralized_V,
  * hidden width 64), ONE weight set shared by every agent, run as a kernel of its own after
@@ -479,6 +507,18 @@ MPE_API int mpe_critic_gru_separated(mpe_handle h, const float *const *obs_recor
                                      const float *const *b_hh_n, const float *const *w3_n, const float *const *b3_n,
                                      float *rnn_state_dev, float *rnn_state_record_dev, float *values_dev,
                                      float *final_values_dev, uint32_t net_flags, float ln_eps, void *stream);
+/* rIPPO's recurrent local critic (R_Critic with use_centralized_V = False): ONE weight set shared by every agent, run on
+ * agent k's own observation record for k = 0 .. A-1 in one launch, w1 [64][obs_dim] (every agent observes alike on
+ * these programs).  As mpe_critic_gru but: agent k's critic reads obs_record_n[k] and final_obs_n[k] only,
+ * rnn_state_dev is [A][N][64] (agent k's h at row k), rnn_state_record_dev [n_steps][A][N][64], and values_dev[t][k]
+ * and final_values_dev[e][k] receive agent k's own value.  Return codes and their order are mpe_critic_gru's
+ * (MPE_ERR_UNSUPPORTED: built for simple, simple_spread N = 2..6 and simple_reference). */
+MPE_API int mpe_critic_gru_local(mpe_handle h, const float *const *obs_record_n, const float *const *final_obs_n,
+                                 int32_t n_steps, int32_t episode_length, const float *w1, const float *b1,
+                                 const float *w2, const float *b2, const float *w_ih, const float *b_ih,
+                                 const float *w_hh, const float *b_hh, const float *w3, const float *b3,
+                                 float *rnn_state_dev, float *rnn_state_record_dev, float *values_dev,
+                                 float *final_values_dev, uint32_t net_flags, float ln_eps, void *stream);
 
 /* flags of mpe_gae */
 enum mpe_gae_flags {

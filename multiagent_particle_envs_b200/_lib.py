@@ -154,6 +154,8 @@ _SIGNATURES = {
                                                                 ctypes.c_uint32, _P]),
     "mpe_critic_gru": (ctypes.c_int, [_P, _PP, _PP, ctypes.c_int32, ctypes.c_int32] + [_P] * 10 +
                        [_P, _P, _P, _P, ctypes.c_uint32, ctypes.c_float, _P]),
+    "mpe_critic_gru_local": (ctypes.c_int, [_P, _PP, _PP, ctypes.c_int32, ctypes.c_int32] + [_P] * 10 +
+                             [_P, _P, _P, _P, ctypes.c_uint32, ctypes.c_float, _P]),
     "mpe_critic_gru_separated": (ctypes.c_int, [_P, _PP, _PP, ctypes.c_int32, ctypes.c_int32] + [_PP] * 10 +
                                  [_P, _P, _P, _P, ctypes.c_uint32, ctypes.c_float, _P]),
     "mpe_gae": (ctypes.c_int, [_P, _P, _P, _P, ctypes.c_int32, ctypes.c_int32, ctypes.c_float, ctypes.c_float,
@@ -167,6 +169,9 @@ _SIGNATURES = {
     "mpe_kernel_launches": (ctypes.c_int64, []),
     "mpe_probe_stream": (ctypes.c_int, [ctypes.c_int, _P, ctypes.c_int64, _P, ctypes.c_int64, ctypes.c_int64, _P]),
 }
+# IPPO's local critics take exactly the parameter lists of the centralized critic's entry points
+_SIGNATURES["mpe_rollout_policy_mappo_local_critic"] = _SIGNATURES["mpe_rollout_policy_mappo_critic"]
+_SIGNATURES["mpe_rollout_policy_mappo_local_critic_episodes"] = _SIGNATURES["mpe_rollout_policy_mappo_critic_episodes"]
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 
 _lib = None

@@ -1,6 +1,6 @@
 // mpe_critic_gru.cuh -- one evaluation and the value store of rMAPPO's recurrent centralized critic (RCriticArgs,
-// RCriticShape in mpe_kernels.cu), shared by the one shared critic (mpe_critic_gru.cu) and the per-agent critics of the
-// separated runner (mpe_gru_separated.cu).  Included after mpe_kernels.cu's templates.
+// RCriticShape in mpe_kernels.cu), shared by the one shared critic (mpe_critic_gru.cu), the per-agent critics of the
+// separated runner (mpe_gru_separated.cu) and IPPO's recurrent local critic (mpe_critic_local.cu).  Included after mpe_kernels.cu's templates.
 #pragma once
 
 namespace mpe {
@@ -11,12 +11,13 @@ namespace mpe {
 // fp32 two-pass statistics over all D entries come from the A fragments themselves (a row's entries are spread over
 // the 4 lanes of a quad); the records are then read a third time, normalised, rounded to TF32 and multiplied by agent
 // i's k-tiles of W1.  Layers 2 and 3 are MAPPO's (act_norm_tf32_frags), the cell the recurrent actor's (gru_cell).
-template <class P>
+// K >= 0: IPPO's local critic on agent K's columns alone (RCriticShape<P, K>), src[K] its observations.
+template <class P, int K = -1>
 __device__ __forceinline__ void rcritic_eval(const float *__restrict__ Wsm, const float *const (&src)[P::A], int64_t wa,
                                              int64_t wb, const RCriticArgs &ca, int lane, const float (&h)[8][4],
                                              float (&hn)[8][4], float (&v)[4]) {
-    using R = RCriticShape<P>;
-    using C = CriticShape<P>;
+    using R = RCriticShape<P, K>;
+    using C = CriticShape<P, K>;
     constexpr int NT = 8, D = C::in_dim();
     const int tq = lane & 3;
     const bool tanh_act = ca.net_flags & kMappoTanh, feature_norm = ca.net_flags & kMappoFeatureNorm;
@@ -33,11 +34,13 @@ __device__ __forceinline__ void rcritic_eval(const float *__restrict__ Wsm, cons
     if (feature_norm) {   // k-tile by k-tile (not unrolled: spread N=6 would hoist its 120 loads and spill)
         float s0 = 0.0f, s1 = 0.0f;
         static_for<P::A>([&](auto ic) {
+            if constexpr (K < 0 || decltype(ic)::value == K) {
 #pragma unroll 1
             for (int kt = 0; kt < MlpShape<P, 64>::kt1(decltype(ic)::value); ++kt) {
                 float q[4];
                 load(ic, kt, q);
                 s0 += q[0] + q[2]; s1 += q[1] + q[3];
+            }
             }
         });
         s0 += __shfl_xor_sync(0xffffffffu, s0, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
@@ -46,12 +49,14 @@ __device__ __forceinline__ void rcritic_eval(const float *__restrict__ Wsm, cons
         float v0 = 0.0f, v1 = 0.0f;
         static_for<P::A>([&](auto ic) {
             constexpr int I = decltype(ic)::value, OD = P::obs_dim(I);
+            if constexpr (K < 0 || I == K) {
 #pragma unroll 1
             for (int kt = 0; kt < MlpShape<P, 64>::kt1(I); ++kt) {
                 float q[4];
                 load(ic, kt, q);
                 if (kt * 8 + tq < OD) { const float d0 = q[0] - mu0, d1 = q[1] - mu1; v0 += d0 * d0; v1 += d1 * d1; }
                 if (kt * 8 + tq + 4 < OD) { const float d0 = q[2] - mu0, d1 = q[3] - mu1; v0 += d0 * d0; v1 += d1 * d1; }
+            }
             }
         });
         v0 += __shfl_xor_sync(0xffffffffu, v0, 1); v1 += __shfl_xor_sync(0xffffffffu, v1, 1);
@@ -67,6 +72,7 @@ __device__ __forceinline__ void rcritic_eval(const float *__restrict__ Wsm, cons
     }
     static_for<P::A>([&](auto ic) {
         constexpr int I = decltype(ic)::value, OD = P::obs_dim(I);
+        if constexpr (K < 0 || I == K) {
         const float *W1 = Wsm + C::w1_off(I);
 #pragma unroll
         for (int kt = 0; kt < MlpShape<P, 64>::kt1(I); ++kt) {
@@ -80,6 +86,7 @@ __device__ __forceinline__ void rcritic_eval(const float *__restrict__ Wsm, cons
 #pragma unroll
             for (int nt = 0; nt < NT; ++nt)
                 mma_tf32(c[nt], a, *reinterpret_cast<const float2 *>(W1 + ((kt * NT + nt) * 32 + lane) * 2));
+        }
         }
     });
     // ---- layer 2 and the base's last LayerNorm -> x ----
@@ -125,6 +132,15 @@ __device__ __forceinline__ void rcritic_store(float *rec, int64_t n, int64_t w0,
         if (ra < rows) rec[s * n + w0 + ra] = v[0];
         if (rb < rows) rec[s * n + w0 + rb] = v[2];
     }
+}
+
+// the warp's values into one agent's row rec [n] (column 0 of rows g and g + 8 in elements 0 and 2 of the quad's first
+// lane)
+__device__ __forceinline__ void rcritic_store_one(float *rec, int64_t w0, int lane, int rows, const float (&v)[4]) {
+    const int ra = lane >> 2, rb = ra + 8;
+    if ((lane & 3) != 0) return;
+    if (ra < rows) rec[w0 + ra] = v[0];
+    if (rb < rows) rec[w0 + rb] = v[2];
 }
 
 }  // namespace mpe

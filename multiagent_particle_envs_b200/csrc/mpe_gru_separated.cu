@@ -8,15 +8,6 @@
 
 namespace mpe {
 
-// the warp's values into one agent's row rec [n] (column 0 of rows g and g + 8 in elements 0 and 2 of the quad's first
-// lane)
-__device__ __forceinline__ void rcritic_store_one(float *rec, int64_t w0, int lane, int rows, const float (&v)[4]) {
-    const int ra = lane >> 2, rb = ra + 8;
-    if ((lane & 3) != 0) return;
-    if (ra < rows) rec[w0 + ra] = v[0];
-    if (rb < rows) rec[w0 + rb] = v[2];
-}
-
 // rMAPPO's per-agent recurrent critics (RCriticSeparatedArgs): block (x, k) stages critic k's weights once and scans
 // its warps' worlds as mpe_critic_gru_kernel does (rcritic_eval), with critic k's state (slice k of h and h_rec) and only
 // agent k's row of the values.  The critics do not affect the trajectory, so they run after the rollout over its

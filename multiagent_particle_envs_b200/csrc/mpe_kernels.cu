@@ -1139,15 +1139,25 @@ static_assert((GruSeparatedShape<SpeakerListener>::kSlotFloats + kGruWarps * Mlp
 // One critic's weights in shared memory, in floats: B fragments [k-tile][n-tile][lane][2] of W1, agent by agent (agent
 // i's obs_dim_i columns zero-padded to whole k-tiles, so that layer 1 is a sum of k-slices over the agents'
 // observation tiles), then of W2 and W3 (one n-tile, its one real column first), then b1 [64], b2 [64], b3 [8].  They
-// follow the actor's weights (MlpShape), count sets in a row; the warps' tiles are the actor's.
-template <class P>
+// follow the actor's weights (MlpShape), count sets in a row; the warps' tiles are the actor's.  K >= 0 is IPPO's local
+// critic of agent K, whose input is obs_K alone: W1 has agent K's k-tiles only, at offset 0.
+template <class P, int K = -1>
 struct CriticShape {
     using M = MlpShape<P, 64>;
     static constexpr int NT = 8;
-    __host__ __device__ static constexpr int in_dim() { int s = 0; for (int i = 0; i < P::A; ++i) s += P::obs_dim(i); return s; }
-    __host__ __device__ static constexpr int col_off(int i) { int s = 0; for (int j = 0; j < i; ++j) s += P::obs_dim(j); return s; }
-    __host__ __device__ static constexpr int w1_off(int i) { int s = 0; for (int j = 0; j < i; ++j) s += 64 * M::kt1(j) * NT; return s; }
-    static constexpr int w2_off = w1_off(P::A);
+    __host__ __device__ static constexpr int in_dim() {
+        if (K >= 0) return P::obs_dim(K);
+        int s = 0; for (int i = 0; i < P::A; ++i) s += P::obs_dim(i); return s;
+    }
+    __host__ __device__ static constexpr int col_off(int i) {
+        if (K >= 0) return 0;
+        int s = 0; for (int j = 0; j < i; ++j) s += P::obs_dim(j); return s;
+    }
+    __host__ __device__ static constexpr int w1_off(int i) {
+        if (K >= 0) return 0;
+        int s = 0; for (int j = 0; j < i; ++j) s += 64 * M::kt1(j) * NT; return s;
+    }
+    static constexpr int w2_off = K >= 0 ? 64 * M::kt1(K) * NT : w1_off(P::A);
     static constexpr int w3_off = w2_off + 64 * NT * NT;
     static constexpr int b1_off = w3_off + 64 * NT;
     static constexpr int b2_off = b1_off + 64;
@@ -1198,6 +1208,65 @@ static_assert(critic_smem_warps<Adversary<1, 3, 3>>(4) < 1 && critic_smem_warps<
 static_assert(!critic_built<Spread<6>>() && !critic_built<Tag<6, 2, 3>>() && critic_built<Tag<4, 2, 2>>(),
               "no critic kernel for spread N=6 and tag 6+2");
 
+// IPPO's local critics (MAPPO with use_centralized_V = False, next to MAPPO's actor, MlpCriticArgs): agent k's critic is
+// the critic above on obs_k alone (share_obs = obs), laid out as CriticShape<P, k>.  count = 1: one shared critic, which
+// needs every obs_dim_i equal, evaluated once per agent on that agent's observation; count = A: critic k evaluates agent
+// k's, the sets back to back (LocalCriticShape::critic_off).  Agent k's values go to row k of values and final_values.
+template <class P>
+struct LocalCriticShape {
+    __host__ __device__ static constexpr int floats(int k) {   // CriticShape<P, k>::kFloats for a run-time k
+        return 64 * MlpShape<P, 64>::kt1(k) * 8 + 64 * 8 * 8 + 64 * 8 + 64 + 64 + 8;
+    }
+    __host__ __device__ static constexpr int critic_off(int k) { int s = 0; for (int j = 0; j < k; ++j) s += floats(j); return s; }
+    __host__ __device__ static constexpr bool shared_ok() {
+        for (int i = 1; i < P::A; ++i)
+            if (P::obs_dim(i) != P::obs_dim(0)) return false;
+        return true;
+    }
+    // the weights of `count` critics (1 or A)
+    __host__ __device__ static constexpr int weight_floats(int count) { return count == 1 ? floats(0) : critic_off(P::A); }
+    // the smallest set a call may pass: one shared critic where the agents observe alike, else A
+    static constexpr int kMinFloats = weight_floats(shared_ok() ? 1 : P::A);
+};
+template <class P>
+__host__ __device__ constexpr int local_critic_smem_warps(int count) {
+    return (kMlpSmemBytes / 4 - MlpShape<P, 64>::kWeightFloats - LocalCriticShape<P>::weight_floats(count)) /
+           MlpShape<P, 64>::kWarpFloats;
+}
+// Built where the smallest set leaves room for a warp: every MAPPO program but tag 4+2 (per-agent critics only, 150 720
+// B of them with 81 728 B free) and tag 6+2 (15 104 B free next to its actor)
+template <class P>
+__host__ __device__ constexpr bool local_critic_built() {
+    return MlpBuilt<P>::value && local_critic_smem_warps<P>(LocalCriticShape<P>::shared_ok() ? 1 : P::A) >= 1;
+}
+// The compile-time cap of the two local-critic kernels: MAPPO's register rule for its form unless an exception below
+// holds (ptxas -v: no spills and no stack), lowered to what the smallest set leaves in shared memory.  The launcher
+// lowers it at run time to local_critic_smem_warps(count).  Forms by MAPPO's bits; the stack ptxas -v showed without
+// the exception.
+template <class P> struct LocalCriticRegisterException : MlpException<0, 0> {};
+template <> struct LocalCriticRegisterException<Simple<1, 1>> : MlpException<kFormM, 12> {};                 // 16 at 128
+template <> struct LocalCriticRegisterException<Push<1, 1, 2>> : MlpException<kFormM | kFormME, 12> {};      // 40, 48 at 128
+template <> struct LocalCriticRegisterException<Crypto> : MlpException<kFormME, 12> {};                      // 56 at 128
+template <> struct LocalCriticRegisterException<Reference> : MlpException<kFormME, 8> {};                    // 32 at 168
+template <> struct LocalCriticRegisterException<Spread<4>> : MlpException<kFormM | kFormME, 8> {};           // 8, 8 at 168
+template <> struct LocalCriticRegisterException<Spread<5>> : MlpException<kFormM, 8> {};                     // 8 at 168
+template <> struct LocalCriticRegisterException<Adversary<1, 3, 3>> : MlpException<kFormM | kFormME, 8> {};  // 16, 8 at 168
+template <class P, bool EPISODES>
+__host__ __device__ constexpr int local_critic_block_warps() {
+    using X = LocalCriticRegisterException<P>;
+    constexpr int r = (X::forms >> (EPISODES ? 5 : 4) & 1) ? X::warps : mlp_register_warps<P, 64, EPISODES ? 5 : 4>();
+    constexpr int s = local_critic_smem_warps<P>(LocalCriticShape<P>::shared_ok() ? 1 : P::A);
+    return r < s ? r : s;
+}
+static_assert(LocalCriticShape<Spread<3>>::floats(0) * 4 == 25120 && local_critic_smem_warps<Spread<3>>(3) == 23,
+              "spread N=3: 3 x 25 120 B of critics next to 75 360 B of actor, 23 warps");
+static_assert(LocalCriticShape<Spread<6>>::floats(0) * 4 == 29216 && local_critic_smem_warps<Spread<6>>(1) == 4 &&
+              local_critic_smem_warps<Spread<6>>(6) < 1, "spread N=6: one shared 29 216 B critic, 4 warps");
+static_assert(local_critic_smem_warps<Spread<5>>(1) >= 1 && local_critic_smem_warps<Spread<5>>(5) < 1,
+              "spread N=5: a shared critic fits, five do not");
+static_assert(kMlpSmemBytes - MlpShape<Tag<6, 2, 3>, 64>::kWeightFloats * 4 == 15104 && !local_critic_built<Tag<6, 2, 3>>(),
+              "tag 6+2: 15 104 B free, no local critic");
+
 // rMAPPO's recurrent centralized critic (R_Critic with use_recurrent_policy, recurrent_N = 1, use_centralized_V), one
 // weight set shared by every agent, in a kernel of its own that runs after the recurrent actor's rollout and reads its
 // observation records:
@@ -1232,10 +1301,11 @@ static_assert(sizeof(RCriticSeparatedArgs) <= 4096, "kernel parameter space");
 // Its weights in shared memory, in floats: W1's B fragments agent by agent as the MLP critic's (CriticShape::w1_off,
 // stage_critic_w1), then W2, W_ih and W_hh (GruShape's layout), W3 (one n-tile, its one real column first), b1 [64],
 // b2 [64], b_ih [192], b_hh [192], b3 [8]: 512 sum(kt1_i) + 29 704 floats.  The records stream through registers (no
-// per-warp tile), so the rest of shared memory is the L1 cache that serves their second and third reads.
-template <class P>
+// per-warp tile), so the rest of shared memory is the L1 cache that serves their second and third reads.  K >= 0: the
+// local critic of IPPO on agent K's observation alone (CriticShape<P, K>'s W1), 512 kt1_K + 29 704 floats.
+template <class P, int K = -1>
 struct RCriticShape {
-    using C = CriticShape<P>;
+    using C = CriticShape<P, K>;
     static constexpr int NT = 8, NG = 24;
     static constexpr int w2_off = C::w2_off;
     static constexpr int wih_off = w2_off + 64 * NT * NT;
@@ -1800,10 +1870,11 @@ struct SqDevWriter {
 };
 
 // Critic W1's columns of agent I ([64][D] torch layout, global) -> TF32 B fragments of its kt1(I) k-tiles, as
-// stage_fragments (PERM = false) lays them out; columns beyond obs_dim_I are zero
-template <class P, int I>
+// stage_fragments (PERM = false) lays them out; columns beyond obs_dim_I are zero.  K = I: a local critic's W1
+// ([64][obs_dim_I]).
+template <class P, int I, int K = -1>
 __device__ __forceinline__ void stage_critic_w1(float *dst, const float *__restrict__ W) {
-    using C = CriticShape<P>;
+    using C = CriticShape<P, K>;
     constexpr int KT = MlpShape<P, 64>::kt1(I), OD = P::obs_dim(I), D = C::in_dim(), OFF = C::col_off(I);
     for (int q = threadIdx.x; q < KT * C::NT * 64; q += blockDim.x) {
         const int j = q & 1, l = (q >> 1) & 31, tile = q >> 6;
@@ -1819,22 +1890,27 @@ __device__ __forceinline__ void stage_critic_w1(float *dst, const float *__restr
 // fp32 passes of register-only writers over every agent's observation; layer 1 then sums, agent by agent, that agent's
 // observation in the warp's observation tile, normalised in place, times its k-tiles of W1.  Layers 2 and 3 run as
 // MAPPO's actor runs them, one m-tile at a time, with act_norm_tf32_frags; layer 3 has one real output column.  Called
-// by all 32 lanes; the tile is free on entry and on return.
-template <class P>
+// by all 32 lanes; the tile is free on entry and on return.  K >= 0: IPPO's local critic of agent K (CriticShape<P,
+// K>), the same arithmetic on obs_K alone.
+template <class P, int K = -1>
 __device__ __forceinline__ void mlp_critic(const float *__restrict__ Wc, const DevDesc &d, const typename P::W &w,
                                            float *tile, int lane, int rows, float ln_eps, uint32_t net_flags, float *dst,
                                            int slots, int64_t n) {
-    using C = CriticShape<P>;
+    using C = CriticShape<P, K>;
     constexpr int NT = C::NT, D = C::in_dim();
     const int gq = lane >> 2, tq = lane & 3;
     const bool feature_norm = net_flags & kMappoFeatureNorm;
     float mu = 0.0f, rstd = 1.0f;
     if (feature_norm) {
         SumWriter sw;
-        static_for<P::A>([&](auto ic) { P::template observe<decltype(ic)::value>(d, w, sw); });
+        static_for<P::A>([&](auto ic) {
+            if constexpr (K < 0 || decltype(ic)::value == K) P::template observe<decltype(ic)::value>(d, w, sw);
+        });
         mu = sw.s / static_cast<float>(D);
         SqDevWriter vw{mu};
-        static_for<P::A>([&](auto ic) { P::template observe<decltype(ic)::value>(d, w, vw); });
+        static_for<P::A>([&](auto ic) {
+            if constexpr (K < 0 || decltype(ic)::value == K) P::template observe<decltype(ic)::value>(d, w, vw);
+        });
         rstd = rsqrtf(vw.s / static_cast<float>(D) + ln_eps);
     }
     // ---- layer 1: sum over agents of [32 x K1_i] . W1[:, agent i's columns]^T, + b1 ----
@@ -1848,6 +1924,7 @@ __device__ __forceinline__ void mlp_critic(const float *__restrict__ Wc, const D
     static_for<P::A>([&](auto ic) {
         constexpr int I = decltype(ic)::value;
         constexpr int OD = P::obs_dim(I), KT1 = MlpShape<P, 64>::kt1(I), PITCH = ObsTile<OD>::kPitch;
+        if constexpr (K < 0 || I == K) {
         {
             TileWriter<OD> o(tile, lane);
             P::template observe<I>(d, w, o);
@@ -1878,6 +1955,7 @@ __device__ __forceinline__ void mlp_critic(const float *__restrict__ Wc, const D
             }
         }
         __syncwarp();   // every lane has read the tile before the next observation overwrites it
+        }
     });
     uint32_t x1[2][NT][4];
 #pragma unroll
@@ -1914,16 +1992,30 @@ __device__ __forceinline__ void mlp_critic(const float *__restrict__ Wc, const D
 }
 
 // every critic's values of the current state into record row `row` of rec (values [T][A][n] or final_values):
-// a shared critic's (count 1) for every agent, else critic k's for agent k
-template <class P>
+// a shared critic's (count 1) for every agent, else critic k's for agent k.  LOCAL: agent k's value is V_k(obs_k), from
+// the shared critic (count 1) or critic k (LocalCriticShape).
+template <class P, bool LOCAL = false>
 __device__ __forceinline__ void run_critics(const MlpCriticState &cs, const float *Wc, const DevDesc &d,
                                             const typename P::W &w, float *tile, int lane, int rows, float ln_eps,
                                             uint32_t net_flags, float *rec, int row, int64_t w0, int64_t n) {
+    if constexpr (LOCAL) {
+        // one agent per iteration: unrolled, the A independent evaluations overlap and spill (spread N=6 at 255
+        // registers)
+#pragma unroll 1
+        for (int k = 0; k < P::A; ++k)
+            static_for<P::A>([&](auto kc) {
+                constexpr int K = decltype(kc)::value;
+                if (K == k)
+                    mlp_critic<P, K>(Wc + (cs.count == 1 ? 0 : LocalCriticShape<P>::critic_off(K)), d, w, tile, lane,
+                                     rows, ln_eps, net_flags, rec + (static_cast<int64_t>(row) * P::A + K) * n + w0, 1, n);
+            });
+    } else {
     const int slots = cs.count == 1 ? P::A : 1;
 #pragma unroll 1
     for (int k = 0; k < cs.count; ++k)
         mlp_critic<P>(Wc + k * CriticShape<P>::kFloats, d, w, tile, lane, rows, ln_eps, net_flags,
                       rec + (static_cast<int64_t>(row) * P::A + k) * n + w0, slots, n);
+    }
 }
 
 // Agent I's turn in the separated recurrent actor (SEPARATED): the whole block waits until every warp is done with the
@@ -1951,21 +2043,24 @@ __device__ __forceinline__ void gru_restage(float *slot, const float *images, ui
 // the body of both forms; ea is null in the single-episode form (EPISODES = false), cr unless CATEGORICAL; ln_eps and
 // net_flags are MAPPO's (MlpMappoArgs), gs the recurrent actor's (GRU, MlpGruArgs), cs the critic's (CRITIC,
 // MlpCriticArgs).  SEPARATED (with GRU) gives every agent its own weight set, restaged into one slot from the fragment
-// images at `images` (GruSeparatedShape) at every agent's turn (gru_restage).
+// images at `images` (GruSeparatedShape) at every agent's turn (gru_restage).  LOCAL (with CRITIC) makes cs IPPO's local
+// critics (LocalCriticShape).
 template <class P, int H, bool EPISODES, bool CATEGORICAL = false, bool MAPPO = false, bool GRU = false,
-          bool CRITIC = false, bool SEPARATED = false>
+          bool CRITIC = false, bool SEPARATED = false, bool LOCAL = false>
 __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEpisodeArgs *ea,
                                             const MlpCategoricalRecords *cr = nullptr, float ln_eps = 0.0f,
                                             uint32_t net_flags = 0, const MlpGruState *gs = nullptr,
                                             const MlpCriticState *cs = nullptr, const float *images = nullptr) {
     static_assert(!CRITIC || (MAPPO && !GRU), "the critic runs next to MAPPO's MLP actor");
     static_assert(!SEPARATED || GRU, "per-agent weight sets are the recurrent actor's");
+    static_assert(!LOCAL || CRITIC, "the local critics are a critic form");
     static_assert(H == 32 || H == 64, "MLP policy rollout: hidden width 32 or 64");
     constexpr int A = P::A, L = P::L, NC = Shape<P>::kNC;
     using S = MlpShape<P, H>;
     constexpr int kWarps = [] {
         if constexpr (SEPARATED) return gru_separated_block_warps<P>();
         else if constexpr (GRU) return gru_block_warps<P>();
+        else if constexpr (CRITIC && LOCAL) return local_critic_block_warps<P, EPISODES>();
         else if constexpr (CRITIC) return critic_block_warps<P, EPISODES>();
         else return mlp_block_warps<P, H, EPISODES | (MAPPO ? 2 : CATEGORICAL) << 1>();
     }();
@@ -1975,8 +2070,8 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
         else if constexpr (GRU) return GruShape<P>::kWeightFloats;
         else return S::kWeightFloats;
     }();
-    static_assert(kWarps >= 1 && (kWeightFloats + (CRITIC ? CriticShape<P>::kFloats : 0) + kWarps * S::kWarpFloats) * 4 <=
-                  kMlpSmemBytes, "one block fits an SM");
+    static_assert(kWarps >= 1 && (kWeightFloats + (CRITIC ? (LOCAL ? LocalCriticShape<P>::kMinFloats : CriticShape<P>::kFloats) : 0) +
+                                  kWarps * S::kWarpFloats) * 4 <= kMlpSmemBytes, "one block fits an SM");
     const StepArgs &a = pa.s;
     extern __shared__ __align__(16) float smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -2018,7 +2113,26 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
     });
     }
     int crit_floats = 0;   // the critics' weights after the actor's (CriticShape), cs->count sets
-    if constexpr (CRITIC) {
+    if constexpr (CRITIC && LOCAL) {   // set k (critic_off(k)) has agent k's W1; the shared set agent 0's
+        using LC = LocalCriticShape<P>;
+        crit_floats = LC::weight_floats(cs->count);
+        static_for<A>([&](auto kc) {
+            constexpr int k = decltype(kc)::value;
+            using C = CriticShape<P, k>;
+            static_assert(C::kFloats == LC::floats(k), "one local critic layout");
+            if (k < cs->count) {
+                float *base = smem + kWeightFloats + LC::critic_off(k);
+                stage_critic_w1<P, k, k>(base, cs->w1[k]);
+                stage_fragments<C::NT, C::NT, true>(base + C::w2_off, cs->w2[k], 64, 64);
+                stage_fragments<C::NT, 1, true>(base + C::w3_off, cs->w3[k], 1, 64);
+                for (int q = threadIdx.x; q < 64; q += blockDim.x) {
+                    base[C::b1_off + q] = cs->b1[k][q];
+                    base[C::b2_off + q] = cs->b2[k][q];
+                }
+                for (int q = threadIdx.x; q < 8; q += blockDim.x) base[C::b3_off + q] = q == 0 ? cs->b3[k][0] : 0.0f;
+            }
+        });
+    } else if constexpr (CRITIC) {
         using C = CriticShape<P>;
         crit_floats = cs->count * C::kFloats;
 #pragma unroll 1
@@ -2090,7 +2204,7 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
             float ux[A], uy[A];
             float cact[NC > 0 ? NC : 1];
             P::prepare(d, w);
-            if constexpr (CRITIC) run_critics<P>(*cs, Wc, d, w, s_warp, lane, rows, ln_eps, net_flags, cs->values, tg, w0, n);   // V of the state the actors act on
+            if constexpr (CRITIC) run_critics<P, LOCAL>(*cs,Wc, d, w, s_warp, lane, rows, ln_eps, net_flags, cs->values, tg, w0, n);   // V of the state the actors act on
             static_for<A>([&](auto ic) {
                 constexpr int i = decltype(ic)::value;
                 if constexpr (SEPARATED) gru_restage<P, i>(smem + kSlotOff, images, bar, phase);
@@ -2127,7 +2241,7 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
             if constexpr (CRITIC) {                            // V of the final state, before the reset
                 P::prepare(d, w);
                 __syncwarp();                                  // every lane has read its logits before the tile is reused
-                run_critics<P>(*cs, Wc, d, w, s_warp, lane, rows, ln_eps, net_flags, cs->final_values, e, w0, n);
+                run_critics<P, LOCAL>(*cs,Wc, d, w, s_warp, lane, rows, ln_eps, net_flags, cs->final_values, e, w0, n);
             }
             if (ea->final_obs[0] != nullptr) {                 // all agents or none (checked by the launcher)
                 P::prepare(d, w);
@@ -2171,7 +2285,7 @@ __device__ __forceinline__ void mlp_rollout(const MlpPolicyArgs &pa, const MlpEp
     P::prepare(d, w);
     __syncwarp();                  // every lane has read its logits before the tile is reused
     if constexpr (CRITIC && !EPISODES)
-        run_critics<P>(*cs, Wc, d, w, s_warp, lane, rows, ln_eps, net_flags, cs->final_values, 0, w0, n);   // V after the last step
+        run_critics<P, LOCAL>(*cs,Wc, d, w, s_warp, lane, rows, ln_eps, net_flags, cs->final_values, 0, w0, n);   // V after the last step
     write_observations<P>(a, d, w, s_warp, lane, rows, active, w0, wi);   // the slot is this warp's observation tile
     if (active) {
 #pragma unroll
@@ -2304,6 +2418,13 @@ const void *critic_kernel(int episodes);
 // instantiates it for the programs of GruBuilt
 template <class P>
 const void *critic_gru_kernel();
+// IPPO's local critics: MAPPO's actor with them (MlpCriticArgs, episodes = 0, 1) for the programs of
+// local_critic_built, and the recurrent local critic (RCriticArgs) for those of GruBuilt.  mpe_critic_local.cu
+// defines and instantiates both.
+template <class P>
+const void *local_critic_kernel(int episodes);
+template <class P>
+const void *critic_gru_local_kernel();
 // The per-agent recurrent actors' kernels of program P: 0 the fragment images, 1 the rollout, 2 its episode form, 3
 // rMAPPO's per-agent recurrent critics (RCriticSeparatedArgs).  mpe_gru_separated.cu defines and instantiates it for the
 // programs of GruSeparatedBuilt.
@@ -2523,11 +2644,16 @@ struct Program {
     // the same with the two-hidden-layer actor on the tensor cores, by form (episodes | kind << 1) and H = 32 / 64: the
     // kernel and its warps per block at most (mlp_block_warps); null for MAPPO's forms at H = 32.  Forms 6 and 7 are
     // the recurrent actor's (gru_block_warps, H = 64 only), whose one shared weight set takes gru_weight_floats; forms
-    // 8 and 9 MAPPO's actor with its critic (critic_block_warps, H = 64 only), each critic taking critic_floats more.
-    struct { const void *fn; int warps; } mlp[kMlpForms + 4][2];
-    int mlp_weight_floats[2], mlp_warp_floats[2], gru_weight_floats, critic_floats;
+    // 8 and 9 MAPPO's actor with its critic (critic_block_warps, H = 64 only), each critic taking critic_floats more;
+    // 10 and 11 MAPPO's actor with IPPO's local critics (local_critic_block_warps), whose weights take
+    // local_critic_floats[0] for one shared critic (0: the agents observe differently, no shared critic) and
+    // local_critic_floats[1] for A.
+    struct { const void *fn; int warps; } mlp[kMlpForms + 6][2];
+    int mlp_weight_floats[2], mlp_warp_floats[2], gru_weight_floats, critic_floats, local_critic_floats[2];
     const void *critic_gru_fn;   // rMAPPO's recurrent critic (kRCriticWarps per block), its weights critic_gru_floats
     int critic_gru_floats;
+    const void *critic_gru_local_fn;   // rIPPO's recurrent local critic (kRCriticWarps per block, A blocks in y)
+    int critic_gru_local_floats;
     // per-agent recurrent actors and critics (GruSeparatedBuilt, gru_separated_kernel): the fragment images' kernel, the
     // rollout's two forms (kGruWarps per block, a 4-float mbarrier header and gru_sep_slot_floats of slot), the critics
     // (kRCriticWarps per block, critic_gru_floats each); null where not built
@@ -2592,9 +2718,17 @@ static Program make_program() {
         p.mlp[kMlpForms + 3][1] = {critic_kernel<P>(1), critic_block_warps<P, true>()};
         p.critic_floats = CriticShape<P>::kFloats;
     }
+    if constexpr (local_critic_built<P>()) {
+        p.mlp[kMlpForms + 4][1] = {local_critic_kernel<P>(0), local_critic_block_warps<P, false>()};
+        p.mlp[kMlpForms + 5][1] = {local_critic_kernel<P>(1), local_critic_block_warps<P, true>()};
+        p.local_critic_floats[0] = LocalCriticShape<P>::shared_ok() ? LocalCriticShape<P>::weight_floats(1) : 0;
+        p.local_critic_floats[1] = LocalCriticShape<P>::weight_floats(P::A);
+    }
     if constexpr (GruBuilt<P>::value) {
         p.critic_gru_fn = critic_gru_kernel<P>();
         p.critic_gru_floats = RCriticShape<P>::kFloats;
+        p.critic_gru_local_fn = critic_gru_local_kernel<P>();
+        p.critic_gru_local_floats = RCriticShape<P, 0>::kFloats;
     }
     if constexpr (GruSeparatedBuilt<P>::value) {
         for (int j = 0; j < 4; ++j) p.gru_sep_fn[j] = gru_separated_kernel<P>(j);
@@ -2738,13 +2872,16 @@ extern "C" int mpe_create(const mpe_desc *desc, int64_t n_env, int device, mpe_h
                     CUDA_TRY(cudaFuncSetAttribute(prog->mlp[f][k].fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                   ((f < kMlpForms ? prog->mlp_weight_floats[k] : prog->gru_weight_floats) +
                                                    prog->mlp_warp_floats[k] * prog->mlp[f][k].warps) * 4));
-        for (int f = kMlpForms + 2; f < kMlpForms + 4; ++f)   // the critic's two: their size depends on the critics'
+        for (int f = kMlpForms + 2; f < kMlpForms + 6; ++f)   // the critics' four: their size depends on the critics'
             if (prog->mlp[f][1].fn)                            // count, so they may take the whole opt-in
                 CUDA_TRY(cudaFuncSetAttribute(prog->mlp[f][1].fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               kMlpSmemBytes));
         if (prog->critic_gru_fn)
             CUDA_TRY(cudaFuncSetAttribute(prog->critic_gru_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           prog->critic_gru_floats * 4));
+        if (prog->critic_gru_local_fn)
+            CUDA_TRY(cudaFuncSetAttribute(prog->critic_gru_local_fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          prog->critic_gru_local_floats * 4));
         for (int j = 1; j < 3; ++j)
             if (prog->gru_sep_fn[j])
                 CUDA_TRY(cudaFuncSetAttribute(prog->gru_sep_fn[j], cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -3109,7 +3246,8 @@ extern "C" int mpe_rollout_policy(mpe_handle h, void *pv, const void *lm, float 
 // form: episodes | kind << 1 (kMlpForms).  T is the episode length (n_steps in the single-episode forms); a record the
 // form does not have is null.  net_flags and ln_eps are MAPPO's (MlpMappoArgs); forms 6 and 7 (kMlpForms + episodes)
 // are the recurrent actor's, whose w[j] hold the shared set's pointer for every agent and gru its MlpGruState; forms 8
-// and 9 (kMlpForms + 2 + episodes) MAPPO's actor with critic, the critics' count, weights and value records.
+// and 9 (kMlpForms + 2 + episodes) MAPPO's actor with critic, the critics' count, weights and value records; forms 10
+// and 11 (kMlpForms + 4 + episodes) the same with IPPO's local critics.
 struct MlpCall {
     int form;
     MlpGruState gru;
@@ -3140,7 +3278,7 @@ struct MlpCall {
 };
 
 static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
-    static const char *const kName[kMlpForms + 4][2] = {   // the NVTX range, the launch's error context
+    static const char *const kName[kMlpForms + 6][2] = {   // the NVTX range, the launch's error context
         {"mpe_rollout_policy_mlp", "cudaLaunchKernelExC(rollout_policy_mlp)"},
         {"mpe_rollout_policy_mlp_episodes", "cudaLaunchKernelExC(rollout_policy_mlp_episodes)"},
         {"mpe_rollout_policy_mlp_categorical", "cudaLaunchKernelExC(rollout_policy_mlp_categorical)"},
@@ -3150,9 +3288,13 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
         {"mpe_rollout_policy_gru", "cudaLaunchKernelExC(rollout_policy_gru)"},
         {"mpe_rollout_policy_gru_episodes", "cudaLaunchKernelExC(rollout_policy_gru_episodes)"},
         {"mpe_rollout_policy_mappo_critic", "cudaLaunchKernelExC(rollout_policy_mappo_critic)"},
-        {"mpe_rollout_policy_mappo_critic_episodes", "cudaLaunchKernelExC(rollout_policy_mappo_critic_episodes)"}};
+        {"mpe_rollout_policy_mappo_critic_episodes", "cudaLaunchKernelExC(rollout_policy_mappo_critic_episodes)"},
+        {"mpe_rollout_policy_mappo_local_critic", "cudaLaunchKernelExC(rollout_policy_mappo_local_critic)"},
+        {"mpe_rollout_policy_mappo_local_critic_episodes",
+         "cudaLaunchKernelExC(rollout_policy_mappo_local_critic_episodes)"}};
     const bool episodes = c.form & 1, categorical = c.form >= 2, mappo = c.form >= 4;
     const bool gru = c.form == kMlpForms || c.form == kMlpForms + 1, critic = c.form >= kMlpForms + 2;
+    const bool local = c.form >= kMlpForms + 4;
     const bool no_weights = !c.w[0] || !c.w[1] || !c.w[2] || !c.w[3] || !c.w[4] || !c.w[5] ||
                             (c.separated && (!c.gru_w[0] || !c.gru_w[1] || !c.gru_w[2] || !c.gru_w[3]));
     // the single-episode forms refuse a negative n_steps and null weight arrays before anything else, the episode forms
@@ -3164,12 +3306,15 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     const void *const fn = k < 0 ? nullptr
                          : c.separated ? (k == 1 ? h->prog->gru_sep_fn[1 + episodes] : nullptr) : h->prog->mlp[c.form][k].fn;
     if (k < 0 || h->prog->scenario == MPE_SCN_CUSTOM || fn == nullptr) return MPE_ERR_UNSUPPORTED;
-    // 1 (shared) or A critics, whose weights must leave room for a warp's tiles next to the actor's
-    int critic_cap = 0;
+    // 1 (shared) or A critics, whose weights must leave room for a warp's tiles next to the actor's.  One shared local
+    // critic needs agents that observe alike.
+    int critic_cap = 0, critic_floats = 0;
     if (critic) {
         if (c.critic.count != 1 && c.critic.count != h->prog->A) return MPE_ERR_BAD_ARG;
-        critic_cap = (kMlpSmemBytes / 4 - h->prog->mlp_weight_floats[k] - c.critic.count * h->prog->critic_floats) /
-                     h->prog->mlp_warp_floats[k];
+        critic_floats = local ? h->prog->local_critic_floats[c.critic.count == 1 ? 0 : 1]
+                              : c.critic.count * h->prog->critic_floats;
+        if (local && critic_floats == 0) return MPE_ERR_BAD_ARG;
+        critic_cap = (kMlpSmemBytes / 4 - h->prog->mlp_weight_floats[k] - critic_floats) / h->prog->mlp_warp_floats[k];
         if (critic_cap < 1) return MPE_ERR_UNSUPPORTED;
     }
     if (c.flags & (MPE_FLAG_DISCRETE_ACTION_INPUT | MPE_FLAG_FORCE_DISCRETE_ACTION)) return MPE_ERR_UNSUPPORTED;
@@ -3243,7 +3388,7 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
     MlpGruEpisodeArgs gea{mea, c.gru};
     MlpCriticArgs va{ma, c.critic};
     MlpCriticEpisodeArgs vea{mea, c.critic};
-    void *const form_args[kMlpForms + 4] = {&pa, &ea, &ca, &cea, &ma, &mea, &ga, &gea, &va, &vea};
+    void *const form_args[kMlpForms + 6] = {&pa, &ea, &ca, &cea, &ma, &mea, &ga, &gea, &va, &vea, &va, &vea};
     const float *const images = static_cast<const float *>(c.workspace);
     MlpGruSeparatedArgs sga{ga, images};
     MlpGruSeparatedEpisodeArgs sgea{gea, images};
@@ -3272,8 +3417,7 @@ static int rollout_policy_mlp(mpe_handle h, const MlpCall &c) {
                                  episodes ? "cudaLaunchKernelExC(rollout_policy_gru_separated_episodes)"
                                           : "cudaLaunchKernelExC(rollout_policy_gru_separated)");
     }
-    const int weight_floats = gru ? h->prog->gru_weight_floats
-                                  : h->prog->mlp_weight_floats[k] + (critic ? c.critic.count * h->prog->critic_floats : 0);
+    const int weight_floats = gru ? h->prog->gru_weight_floats : h->prog->mlp_weight_floats[k] + critic_floats;
     return launch_persistent(h, fn, warps, wpb, static_cast<size_t>(weight_floats) * 4,
                              static_cast<size_t>(h->prog->mlp_warp_floats[k]) * 4, form_args[c.form], c.stream,
                              kName[c.form][1]);
@@ -3567,6 +3711,49 @@ extern "C" int mpe_rollout_policy_mappo_critic_episodes(
     return rollout_policy_critic(h, c, critic_count, {cw1, cb1, cw2, cb2, cw3, cb3}, values, final_values);
 }
 
+extern "C" int mpe_rollout_policy_mappo_local_critic(
+    mpe_handle h, void *pv, const void *lm, float *comm, const int32_t *goal, const float *const *w1_n,
+    const float *const *b1_n, const float *const *w2_n, const float *const *b2_n, const float *const *w3_n,
+    const float *const *b3_n, int32_t hidden, int32_t n_steps, int32_t explore, uint64_t explore_seed,
+    uint64_t explore_epoch, uint64_t world_offset, float *const *obs_n, float *rew_sum, float *rew_steps, float *logp_steps,
+    int32_t *const *act_index_record_n, float *const *obs_record_n, uint32_t net_flags, float ln_eps, int32_t critic_count,
+    const float *const *cw1, const float *const *cb1, const float *const *cw2, const float *const *cb2,
+    const float *const *cw3, const float *const *cb3, float *values, float *final_values, uint8_t *done, uint32_t flags,
+    void *stream) {
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.w[0] = w1_n; c.w[1] = b1_n; c.w[2] = w2_n; c.w[3] = b2_n; c.w[4] = w3_n; c.w[5] = b3_n;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = kMlpForms + 4; c.T = n_steps; c.episodes = 1; c.rew = rew_sum;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    c.net_flags = net_flags; c.ln_eps = ln_eps;
+    return rollout_policy_critic(h, c, critic_count, {cw1, cb1, cw2, cb2, cw3, cb3}, values, final_values);
+}
+
+extern "C" int mpe_rollout_policy_mappo_local_critic_episodes(
+    mpe_handle h, void *pv, void *lm, float *comm, int32_t *goal, const float *const *w1_n, const float *const *b1_n,
+    const float *const *w2_n, const float *const *b2_n, const float *const *w3_n, const float *const *b3_n, int32_t hidden,
+    int32_t episode_length, int32_t n_episodes, int32_t explore, uint64_t explore_seed, uint64_t explore_epoch,
+    uint64_t reset_seed, uint64_t reset_epoch, uint64_t world_offset, float *const *obs_n, float *ep_rew, float *rew_steps,
+    float *logp_steps, int32_t *const *act_index_record_n, float *const *obs_record_n, float *const *final_obs_record_n,
+    uint32_t net_flags, float ln_eps, int32_t critic_count, const float *const *cw1, const float *const *cb1,
+    const float *const *cw2, const float *const *cb2, const float *const *cw3, const float *const *cb3, float *values,
+    float *final_values, uint8_t *done, uint32_t flags, void *stream) {
+    MlpCall c{};
+    c.pv = pv; c.lm = lm; c.comm = comm; c.goal = goal;
+    c.w[0] = w1_n; c.w[1] = b1_n; c.w[2] = w2_n; c.w[3] = b2_n; c.w[4] = w3_n; c.w[5] = b3_n;
+    c.hidden = hidden; c.explore = explore; c.explore_seed = explore_seed; c.explore_epoch = explore_epoch;
+    c.world_offset = world_offset; c.obs_n = obs_n; c.rew_steps = rew_steps; c.obs_record_n = obs_record_n;
+    c.done = done; c.flags = flags; c.stream = stream;
+    c.form = kMlpForms + 5; c.T = episode_length; c.episodes = n_episodes; c.rew = ep_rew;
+    c.logp_steps = logp_steps; c.act_index_record_n = act_index_record_n;
+    c.reset_seed = reset_seed; c.reset_epoch = reset_epoch; c.final_obs_record_n = final_obs_record_n;
+    c.net_flags = net_flags; c.ln_eps = ln_eps;
+    return rollout_policy_critic(h, c, critic_count, {cw1, cb1, cw2, cb2, cw3, cb3}, values, final_values);
+}
+
 // The checks of the recurrent critics' entry points, in their documented order, and RCriticArgs but for the weights.
 // fn: the program's kernel; weights_ok: every weight pointer non-null and 4-byte aligned.
 static int rcritic_args(mpe_handle h, const void *fn, const float *const *obs_record_n, const float *const *final_obs_n,
@@ -3596,15 +3783,16 @@ static int rcritic_args(mpe_handle h, const void *fn, const float *const *obs_re
     return MPE_OK;
 }
 
-// one warp per 16 worlds, blocks_y critics
-static int launch_rcritic(mpe_handle h, const void *fn, void *args, unsigned blocks_y, void *stream, const char *what) {
+// one warp per 16 worlds, blocks_y critics, weight_floats of weights in shared memory
+static int launch_rcritic(mpe_handle h, const void *fn, void *args, unsigned blocks_y, int weight_floats, void *stream,
+                          const char *what) {
     const int64_t warps = (h->n + 15) / 16;
     int64_t wpb = (warps + h->sms - 1) / (h->sms > 0 ? h->sms : 1);
     if (wpb < 1) wpb = 1;
     if (wpb > kRCriticWarps) wpb = kRCriticWarps;
     void *params[] = {args};
     return launch_kernel(h, fn, (warps + wpb - 1) / wpb, static_cast<int>(32 * wpb),
-                         static_cast<size_t>(h->prog->critic_gru_floats) * 4, stream, params, false, what, blocks_y);
+                         static_cast<size_t>(weight_floats) * 4, stream, params, false, what, blocks_y);
 }
 
 extern "C" int mpe_critic_gru(mpe_handle h, const float *const *obs_record_n, const float *const *final_obs_n,
@@ -3622,7 +3810,29 @@ extern "C" int mpe_critic_gru(mpe_handle h, const float *const *obs_record_n, co
     a.w1 = w1; a.b1 = b1; a.w2 = w2; a.b2 = b2; a.w_ih = w_ih; a.b_ih = b_ih; a.w_hh = w_hh; a.b_hh = b_hh;
     a.w3 = w3; a.b3 = b3;
     NvtxRange range("mpe_critic_gru");
-    return launch_rcritic(h, h->prog->critic_gru_fn, &a, 1, stream, "cudaLaunchKernelExC(critic_gru)");
+    return launch_rcritic(h, h->prog->critic_gru_fn, &a, 1, h->prog->critic_gru_floats, stream,
+                          "cudaLaunchKernelExC(critic_gru)");
+}
+
+extern "C" int mpe_critic_gru_local(mpe_handle h, const float *const *obs_record_n, const float *const *final_obs_n,
+                                    int32_t n_steps, int32_t episode_length, const float *w1, const float *b1,
+                                    const float *w2, const float *b2, const float *w_ih, const float *b_ih,
+                                    const float *w_hh, const float *b_hh, const float *w3, const float *b3,
+                                    float *rnn_state, float *rnn_state_record, float *values, float *final_values,
+                                    uint32_t net_flags, float ln_eps, void *stream) {
+    const float *const wt[10] = {w1, b1, w2, b2, w_ih, b_ih, w_hh, b_hh, w3, b3};
+    bool weights_ok = true;
+    for (int j = 0; j < 10; ++j) weights_ok = weights_ok && ok4(wt[j]);
+    RCriticArgs a{};
+    int r = rcritic_args(h, h ? h->prog->critic_gru_local_fn : nullptr, obs_record_n, final_obs_n, n_steps,
+                         episode_length, weights_ok, rnn_state, rnn_state_record, values, final_values, net_flags, ln_eps,
+                         a);
+    if (r) return r;
+    a.w1 = w1; a.b1 = b1; a.w2 = w2; a.b2 = b2; a.w_ih = w_ih; a.b_ih = b_ih; a.w_hh = w_hh; a.b_hh = b_hh;
+    a.w3 = w3; a.b3 = b3;
+    NvtxRange range("mpe_critic_gru_local");
+    return launch_rcritic(h, h->prog->critic_gru_local_fn, &a, static_cast<unsigned>(h->prog->A),
+                          h->prog->critic_gru_local_floats, stream, "cudaLaunchKernelExC(critic_gru_local)");
 }
 
 extern "C" int mpe_critic_gru_separated(mpe_handle h, const float *const *obs_record_n, const float *const *final_obs_n,
@@ -3647,8 +3857,8 @@ extern "C" int mpe_critic_gru_separated(mpe_handle h, const float *const *obs_re
                          weights_ok, rnn_state, rnn_state_record, values, final_values, net_flags, ln_eps, sa.c);
     if (r) return r;
     NvtxRange range("mpe_critic_gru_separated");
-    return launch_rcritic(h, h->prog->gru_sep_fn[3], &sa, static_cast<unsigned>(h->prog->A), stream,
-                          "cudaLaunchKernelExC(critic_gru_separated)");
+    return launch_rcritic(h, h->prog->gru_sep_fn[3], &sa, static_cast<unsigned>(h->prog->A), h->prog->critic_gru_floats,
+                          stream, "cudaLaunchKernelExC(critic_gru_separated)");
 }
 
 static int64_t gae_scan_blocks(const mpe_env *h) { return (h->prog->A * h->n + kGaeThreads - 1) / kGaeThreads; }

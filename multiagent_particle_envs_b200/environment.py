@@ -246,7 +246,7 @@ class MultiAgentEnv(_Env):
     def rollout_policy(self, policies, n_steps, record_actions=False, per_step_rewards=False, record_observations=False,
                        explore_seed=None, episode_length=None, action_mode="softmax", record_log_probs=False,
                        rnn_states=None, record_rnn_states=False, critic=None, critic_rnn_states=None,
-                       record_critic_rnn_states=False):
+                       record_critic_rnn_states=False, centralized_critic=True):
         """T closed-loop steps in ONE kernel launch with the actors inside the kernel.
 
         One hidden layer (mpe_rollout_policy, fp32): agent i acts with softmax(W2_i relu(W1_i obs_i + b1_i) + b2_i).
@@ -374,7 +374,28 @@ class MultiAgentEnv(_Env):
         tuples, one per agent (mpe_critic_gru_separated, the separated runner's R_Critic per agent on share_obs), each
         folded by rmappo_critic_params: agent k's values and final values come from critic k, critic_rnn_states and
         extras["final_critic_rnn_states"] are [n, N, 64] and extras["critic_rnn_states"] [T, n, N, 64] (MAPPO's
-        separated rnn_states_critic); a single tuple or a list of another length raises ValueError."""
+        separated rnn_states_critic); a single tuple or a list of another length raises ValueError.
+
+        centralized_critic=False selects IPPO's local critics (MAPPO with use_centralized_V=False, share_obs = obs): every
+        critic above reads agent k's own raw observation instead of share_obs, its input width is obs_dim_k, and
+        nothing else changes -- extras keep their names and shapes and compute_gae takes them as they are.
+          - With MAPPO's MLP actor (mpe_rollout_policy_mappo_local_critic[_episodes]): the critic is
+            nn.Sequential([LayerNorm(obs_dim_k)], Linear(obs_dim_k, 64), Act, LayerNorm(64), Linear(64, 64), Act,
+            LayerNorm(64), Linear(64, 1)), folded by mappo_actor_params on [obs_dim_k].  One module (or [critic] * n)
+            is one shared critic evaluated on every agent's observation, which needs every obs_dim_i equal (simple,
+            simple_spread, simple_reference); n distinct modules give agent k its own.  extras["values"][t, k] =
+            V_k(obs_k at step t).  simple_tag 4+2 and 6+2 have no kernel, and n per-agent critics do not fit next to
+            the actors on simple_spread N = 5 and 6: those raise MpeError before anything runs.
+          - With MAPPO's shared recurrent actor (mpe_critic_gru_local, rIPPO): ONE tuple (base, gru, norm, v_out) (or
+            [critic] * n) whose base reads obs_dim inputs, folded by rmappo_critic_params(critic, [obs_dim]) and run on
+            every agent's observation record with that agent's own hidden state: critic_rnn_states and
+            extras["final_critic_rnn_states"] are [n, N, 64], extras["critic_rnn_states"] [T, n, N, 64].
+        Distinct per-agent recurrent local critics, local critics with the per-agent recurrent actors and local
+        critics with any actor but MAPPO's raise NotImplementedError.  ValueError for centralized_critic=False without a
+        critic, a shared critic on a program whose agents' obs_dims differ, a critic whose input width is not the
+        agent's obs_dim, a critic whose activation, input LayerNorm or eps differ from the actors', or a
+        critic_rnn_states other than a float32 [n, N, 64] tensor on the env's device.  Every refusal but MpeError
+        happens before the world is bound; none changes the state or an epoch."""
         import torch
         world = self.world
         if action_mode not in ("softmax", "categorical"):
@@ -407,6 +428,12 @@ class MultiAgentEnv(_Env):
                                           "critic is recurrent")
             if action_mode != "categorical":
                 raise NotImplementedError("rollout_policy: critic needs action_mode='categorical'")
+        local = None   # IPPO's local critics, folded and checked before the world is bound
+        if not centralized_critic:
+            if critic is None:
+                raise ValueError("rollout_policy: centralized_critic=False selects IPPO's local critics and needs a "
+                                 "critic")
+            local = self._local_critic_fold(policies, critic, recurrent, critic_rnn_states)
         if (critic_rnn_states is not None or record_critic_rnn_states) and not recurrent_critic:
             raise ValueError("rollout_policy: critic_rnn_states and record_critic_rnn_states need rMAPPO's recurrent "
                              "critic (a critic tuple holding an nn.GRU)")
@@ -426,7 +453,7 @@ class MultiAgentEnv(_Env):
                                             explore_seed, episode_length, True, record_log_probs, mappo=True,
                                             gru=(rnn_states, record_rnn_states, sep),
                                             rcritic=(critic, critic_rnn_states, record_critic_rnn_states)
-                                            if critic is not None else None)
+                                            if critic is not None else None, local=local)
         if rnn_states is not None or record_rnn_states:
             raise ValueError("rollout_policy: rnn_states and record_rnn_states need MAPPO's recurrent actor "
                              "(a policy tuple with an nn.GRU)")
@@ -439,7 +466,7 @@ class MultiAgentEnv(_Env):
                                           % (MAPPO_HIDDEN, sorted(_mappo_hidden_widths(policies))))
             return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
                                             explore_seed, episode_length, True, record_log_probs, mappo=True,
-                                            critic=critic)
+                                            critic=critic, local=local)
         if any(_has_two_hidden_layers(p) for p in policies):
             return self._rollout_policy_mlp(policies, n_steps, record_actions, per_step_rewards, record_observations,
                                             explore_seed, episode_length, action_mode == "categorical", record_log_probs)
@@ -491,6 +518,57 @@ class MultiAgentEnv(_Env):
         except _lib.MpeError:
             return False
         return True
+
+    def _local_critic_fold(self, policies, critic, recurrent, critic_rnn_states):
+        """IPPO's local critics, checked before the world is bound: the critic folded on one agent's obs_dim
+        (mappo_actor_params on [obs_dim_k] per critic, or rmappo_critic_params(critic, [obs_dim]) for the recurrent
+        one), its activation, input LayerNorm and eps against the actors', and critic_rnn_states [n, N, 64].  Returns
+        (params, tanh, feature_norm, eps) as the centralized folds do."""
+        import torch
+        shapes = self.world.native_shapes()
+        n, N, obs_dims = self.n, shapes.n_env, list(shapes.obs_dims)
+        if recurrent:
+            if any(p is not policies[0] for p in policies) and self._has_gru_separated():
+                raise NotImplementedError("rollout_policy: local critics with per-agent recurrent actors (rMAPPO's "
+                                          "separated runner) are not supported")
+            if isinstance(critic, (tuple, list)) and len(critic) == n and all(_is_recurrent(c) for c in critic):
+                if any(c is not critic[0] for c in critic):
+                    raise NotImplementedError("rollout_policy: distinct per-agent recurrent local critics are not "
+                                              "supported; pass one tuple ([critic] * n)")
+                critic = critic[0]
+            if len(set(obs_dims)) != 1:
+                raise ValueError("rollout_policy: one shared local critic needs agents with equal obs_dims; got %s"
+                                 % obs_dims)
+            fold = rmappo_critic_params(critic, obs_dims[:1])
+            actor = rmappo_actor_params(policies, obs_dims, list(shapes.act_dims))
+        else:
+            if isinstance(critic, torch.nn.Module):
+                critics = [critic]
+            elif isinstance(critic, (list, tuple)) and len(critic) in (1, n):
+                critics = [critic[0]] if all(c is critic[0] for c in critic) else list(critic)
+            else:
+                raise ValueError("rollout_policy: the local critic must be one module, or a list of 1 or %d modules" % n)
+            if len(critics) == 1 and len(set(obs_dims)) != 1:
+                raise ValueError("rollout_policy: one shared local critic needs agents with equal obs_dims; got %s "
+                                 "(pass %d per-agent critics)" % (obs_dims, n))
+            dims = obs_dims[:1] if len(critics) == 1 else obs_dims
+            try:
+                fold = mappo_actor_params(critics, dims, [1] * len(critics))
+            except ValueError as e:
+                raise ValueError("rollout_policy: the local critic must be %s: %s" % (_LOCAL_CRITIC_SHAPE, e)) from None
+            actor = mappo_actor_params(policies, obs_dims, list(shapes.act_dims))
+        if fold[1:] != actor[1:]:
+            raise ValueError("rollout_policy: the critic must use the actors' activation, input LayerNorm and eps (%s, "
+                             "%s, %g); got (%s, %s, %g)" % ("Tanh" if actor[1] else "ReLU", actor[2], actor[3],
+                                                           "Tanh" if fold[1] else "ReLU", fold[2], fold[3]))
+        t = critic_rnn_states
+        device = self._device()
+        if t is not None and not (torch.is_tensor(t) and tuple(t.shape) == (n, N, MAPPO_HIDDEN)
+                                  and t.dtype == torch.float32 and t.device == device):
+            raise ValueError("rollout_policy: critic_rnn_states must be a float32 tensor %s on %s; got %s"
+                             % ([n, N, MAPPO_HIDDEN], device, (tuple(t.shape), t.dtype, t.device)
+                                if torch.is_tensor(t) else type(t).__name__))
+        return fold
 
     def _device(self):
         """the env's device as bind() resolves it, without binding"""
@@ -628,7 +706,7 @@ class MultiAgentEnv(_Env):
 
     def _rollout_policy_mlp(self, policies, n_steps, record_actions, per_step_rewards, record_observations, explore_seed,
                             episode_length=None, categorical=False, record_log_probs=False, mappo=False, gru=None,
-                            critic=None, rcritic=None):
+                            critic=None, rcritic=None, local=None):
         import torch
         world = self.world
         nw = world.bind()
@@ -662,7 +740,10 @@ class MultiAgentEnv(_Env):
                 rnn += (torch.empty(nw.gru_separated_workspace_bytes() // 4, dtype=torch.float32, device=nw.device),)
             if rcritic is not None:   # rMAPPO's recurrent critic: rcritic = (critic, critic_rnn_states, record)
                 rmodule, ch0, crecord = rcritic
-                if sep is None:
+                if local is not None:   # rIPPO: checked by _local_critic_fold
+                    rparams = local[0]
+                    nw.require_critic_gru_local()
+                elif sep is None:
                     rparams, ctanh, cfn, ceps = rmappo_critic_params(rmodule, nw.obs_dims)
                     if (ctanh, cfn, ceps) != (tanh, feature_norm, eps):
                         raise ValueError("rollout_policy: the critic must use the actor's activation, input LayerNorm "
@@ -670,7 +751,7 @@ class MultiAgentEnv(_Env):
                                          % ("Tanh" if tanh else "ReLU", feature_norm, eps, "Tanh" if ctanh else "ReLU",
                                             cfn, ceps))
                     nw.require_critic_gru()
-                cshape = (N, MAPPO_HIDDEN) if sep is None else (self.n, N, MAPPO_HIDDEN)
+                cshape = (N, MAPPO_HIDDEN) if sep is None and local is None else (self.n, N, MAPPO_HIDDEN)
                 if ch0 is not None:
                     if not (torch.is_tensor(ch0) and tuple(ch0.shape) == cshape and ch0.dtype == torch.float32
                             and ch0.device == torch.device(nw.device)):
@@ -692,7 +773,10 @@ class MultiAgentEnv(_Env):
             params, tanh, feature_norm, eps = mappo_actor_params(policies, nw.obs_dims, nw.act_dims)
             hidden = MAPPO_HIDDEN
             net = ((_lib.MAPPO_FEATURE_NORM if feature_norm else 0) | (_lib.MAPPO_TANH if tanh else 0), eps)
-            if critic is not None:
+            if local is not None:   # IPPO: checked by _local_critic_fold
+                cparams = local[0]
+                nw.require_local_critic(len(cparams))   # a program without the kernel, or critics that do not fit
+            elif critic is not None:
                 cparams, ctanh, cfn, ceps = mappo_critic_params(critic, nw.obs_dims)
                 if (ctanh, cfn, ceps) != (tanh, feature_norm, eps):
                     raise ValueError("rollout_policy: the critic must use the actors' activation, input LayerNorm and "
@@ -742,7 +826,7 @@ class MultiAgentEnv(_Env):
                               rew_steps=rew_steps, act_rec_ptrs=act_ptrs, obs_rec_ptrs=obs_ptrs,
                               final_obs_ptrs=_lib.ptr_array([o.data_ptr() for o in final]) if final is not None else None,
                               logp_steps=log_probs, ep_rew=ep_rew, explore_seed=seed, explore_epoch=self.explore_epoch,
-                              mappo=net, gru=rnn, critic=crit)
+                              mappo=net, gru=rnn, critic=crit, local_critic=local is not None)
         if rnn is not None:
             extras["final_rnn_states"], extras["rnn_states"] = rnn[:2]
         if rcritic is not None:   # on the same stream, after the rollout that wrote its input records
@@ -751,7 +835,7 @@ class MultiAgentEnv(_Env):
             final_ptrs = out.obs_ptrs if final is None else _lib.ptr_array([o.data_ptr() for o in final])
             if sep is None:
                 nw.critic_gru([t.data_ptr() for t in rkeep], obs_ptrs, final_ptrs, T, episode_length, rcrit[0],
-                              rcrit[1], values, final_values, net)
+                              rcrit[1], values, final_values, net, local=local is not None)
             else:
                 nw.critic_gru_separated(rkeep, obs_ptrs, final_ptrs, T, episode_length, rcrit[0], rcrit[1], values,
                                         final_values, net)
@@ -1178,6 +1262,9 @@ def mappo_actor_params(policies, obs_dims, act_dims=None):
 # ---- MAPPO's centralized critic (R_Critic with use_centralized_V, non-recurrent) -------------------------------------
 _CRITIC_SHAPE = ("nn.Sequential([LayerNorm(D)], Linear(D, 64), Act, LayerNorm(64), Linear(64, 64), Act, LayerNorm(64), "
                  "Linear(64, 1)) with Act = ReLU() or Tanh() and D the sum of the agents' observation sizes")
+
+_LOCAL_CRITIC_SHAPE = ("nn.Sequential([LayerNorm(D)], Linear(D, 64), Act, LayerNorm(64), Linear(64, 64), Act, "
+                       "LayerNorm(64), Linear(64, 1)) with Act = ReLU() or Tanh() and D the agent's observation size")
 
 
 def mappo_critic_params(critic, obs_dims):

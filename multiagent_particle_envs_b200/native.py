@@ -312,6 +312,25 @@ class NativeWorld(ShapeHandle):
         if rc == _lib.ERR_UNSUPPORTED:
             check(rc, "mpe_rollout_policy_mappo_critic")
 
+    def require_local_critic(self, count):
+        """MpeError unless the library has IPPO's local critics next to MAPPO's actor for this program and `count`
+        critics (1 or A) fit in shared memory.  As in require_critic, the probe stops at the null state."""
+        none = _lib.ptr_array([256] * self.n_agents)
+        rc = self.lib.mpe_rollout_policy_mappo_local_critic(self.handle, None, None, None, None, *([none] * 6), 64, 0, 0,
+                                                            0, 0, 0, None, None, None, None, None, None, 0, 0.0,
+                                                            int(count), *([none] * 6), None, None, None, 0,
+                                                            self._stream())
+        if rc == _lib.ERR_UNSUPPORTED:
+            check(rc, "mpe_rollout_policy_mappo_local_critic")
+
+    def require_critic_gru_local(self):
+        """MpeError unless the library has rIPPO's recurrent local critic for this program (probed as
+        require_critic_gru)."""
+        rc = self.lib.mpe_critic_gru_local(self.handle, None, None, 0, 0, *([256] * 10), None, None, None, None, 0, 0.0,
+                                           self._stream())
+        if rc == _lib.ERR_UNSUPPORTED:
+            check(rc, "mpe_critic_gru_local")
+
     def require_critic_gru(self):
         """MpeError unless the library has rMAPPO's recurrent critic for this program.  mpe_critic_gru checks the program
         before any pointer, so the probe stops at the null state and runs nothing."""
@@ -321,18 +340,21 @@ class NativeWorld(ShapeHandle):
             check(rc, "mpe_critic_gru")
 
     def critic_gru(self, w_ptrs, obs_rec_ptrs, final_obs_ptrs, n_steps, episode_length, rnn_state, rnn_record, values,
-                   final_values, net):
+                   final_values, net, local=False):
         """rMAPPO's recurrent critic over a finished rollout's records (mpe_critic_gru), on the current stream: w_ptrs
         the ten device pointers of its folded weight set (environment.rmappo_critic_params), obs_rec_ptrs and
         final_obs_ptrs one [n_steps, N, obs_dim_i] and one [E, N, obs_dim_i] record per agent, episode_length None
         (one episode) or L.  rnn_state (float32 [N, 64]) holds the initial h (unless episode_length) and receives the
         final one, rnn_record (float32 [n_steps, N, 64] or None) the h each step consumed; values [n_steps, A, N] and
-        final_values [E, A, N] receive the values.  net = (net_flags, eps) as in rollout_policy_mlp."""
-        rc = self.lib.mpe_critic_gru(self.handle, obs_rec_ptrs, final_obs_ptrs, int(n_steps), int(episode_length or 0),
+        final_values [E, A, N] receive the values.  net = (net_flags, eps) as in rollout_policy_mlp.  local=True
+        (mpe_critic_gru_local): rIPPO's local critic, its W1 [64, obs_dim], run on every agent's own records with
+        rnn_state [A, N, 64] and rnn_record [n_steps, A, N, 64], agent k's values in row k."""
+        name = "mpe_critic_gru_local" if local else "mpe_critic_gru"
+        rc = getattr(self.lib, name)(self.handle, obs_rec_ptrs, final_obs_ptrs, int(n_steps), int(episode_length or 0),
                                      *w_ptrs, rnn_state.data_ptr(), rnn_record.data_ptr() if rnn_record is not None
                                      else None, values.data_ptr(), final_values.data_ptr(), int(net[0]), float(net[1]),
                                      self._stream())
-        check(rc, "mpe_critic_gru")
+        check(rc, name)
 
     def critic_gru_separated(self, w_ptrs, obs_rec_ptrs, final_obs_ptrs, n_steps, episode_length, rnn_state, rnn_record,
                              values, final_values, net):
@@ -366,7 +388,8 @@ class NativeWorld(ShapeHandle):
 
     def rollout_policy_mlp(self, w_ptrs, hidden, n_steps, out=None, flags=0, *, episode_length=None, categorical=False,
                            rew_steps=None, act_rec_ptrs=None, obs_rec_ptrs=None, final_obs_ptrs=None, logp_steps=None,
-                           ep_rew=None, explore_seed=None, explore_epoch=0, mappo=None, gru=None, critic=None):
+                           ep_rew=None, explore_seed=None, explore_epoch=0, mappo=None, gru=None, critic=None,
+                           local_critic=False):
         """n_steps fused steps in ONE launch with every agent's two-hidden-layer actor evaluated on the tensor cores
         (mpe_rollout_policy_mlp); w_ptrs: the six pointer arrays (W1, b1, W2, b2, W3, b3), one device pointer per
         agent each.  explore_seed (not None) switches the Gumbel-softmax sampling on.
@@ -395,7 +418,9 @@ class NativeWorld(ShapeHandle):
         critic=(count, cw_ptrs, values, final_values) with mappo (mpe_rollout_policy_mappo_critic[_episodes]): MAPPO's
         centralized critic next to the actor.  count is 1 (one shared critic) or A; cw_ptrs the six pointer arrays of
         the folded critics (environment.mappo_critic_params), count device pointers each; values a float32 [n_steps, A,
-        N] and final_values a float32 [A, N] ([episodes, A, N]) CUDA tensor."""
+        N] and final_values a float32 [A, N] ([episodes, A, N]) CUDA tensor.  local_critic=True
+        (mpe_rollout_policy_mappo_local_critic[_episodes]): the critics are IPPO's local ones, critic k's W1 [64,
+        obs_dim_k] (one shared critic: every agent's obs_dim)."""
         out = out or self.out
         episodes = episode_length is not None
         if gru is not None and mappo is None:
@@ -414,7 +439,8 @@ class NativeWorld(ShapeHandle):
         logp = (logp_steps.data_ptr() if logp_steps is not None else None,) if categorical else ()
         rnn = ()
         if critic is not None:
-            name = "mpe_rollout_policy_mappo_critic" + ("_episodes" if episodes else "")
+            name = "mpe_rollout_policy_mappo_" + ("local_critic" if local_critic else "critic") + \
+                ("_episodes" if episodes else "")
             net = (int(mappo[0]), float(mappo[1]), int(critic[0]), *critic[1], critic[2].data_ptr(),
                    critic[3].data_ptr())
         elif gru is not None:

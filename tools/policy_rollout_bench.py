@@ -27,6 +27,13 @@
       "kernel_then_torch_critic" (that rollout, then the torch critic under no_grad in its fastest form: base over
       [T N, D] in one call, one cuDNN nn.GRU call over the [T, N, 64] sequence, norm and v_out, plus the bootstrap step
       on the returned observations);
+      --critic local (with --actor mappo) / recurrent-local (with --actor rmappo): IPPO's local critics
+      (centralized_critic=False), each on its agent's own observation -- one shared critic where every agent observes
+      alike, else one per agent.  Arms: "in_kernel_local_critic", the same call without a critic
+      ("in_kernel_actor_only", recording observations for recurrent-local), that call then the same local critics in
+      torch over the records ("kernel_then_torch_local_critic"), and the centralized critic in-kernel on the same
+      program where it has a kernel ("in_kernel_centralized_critic"); with --critic local on a program whose agents
+      observe alike, also one critic per agent, local and centralized, where they fit ("..._per_agent");
       --separated (with --actor rmappo, simple_speaker_listener): rMAPPO's separated runner, a distinct tuple per agent
       (mpe_rollout_policy_gru_separated, which restages each agent's weights into shared memory at its turn), and with
       --critic recurrent a distinct critic per agent (mpe_critic_gru_separated; the torch arm runs each critic in turn).
@@ -176,6 +183,97 @@ def time_rcritic(args, env, mods, kw, res, e0, e1):
     return res
 
 
+def time_local_critic(args, env, mods, kw, res, e0, e1):
+    """IPPO's local critics (centralized_critic=False), each critic on its agent's own observation: (a) the call with
+    them in-kernel, (b) the same call without a critic (with --critic recurrent-local: recording observations, the
+    critic kernel's input), (c) (b), then the same local critics in torch over the records and the final observations,
+    and (d) the centralized critic in-kernel on the same program where it has a kernel; device time per step of each"""
+    import torch
+    from multiagent_particle_envs_b200._lib import MpeError
+    nn = torch.nn
+    nw = env.world.native
+    n, T, H, A = args.num_envs, args.steps, args.hidden, len(nw.obs_dims)
+    recurrent = args.critic == "recurrent-local"
+    dev = (mods[0][0][-1] if recurrent else mods[0][0]).weight.device
+    Act = nn.Tanh if args.tanh else nn.ReLU
+    shared = len(set(nw.obs_dims)) == 1     # one shared critic where the agents observe alike, else one per agent
+
+    def base(d):
+        return ([nn.LayerNorm(d)] if args.feature_norm else []) + [nn.Linear(d, H), Act(), nn.LayerNorm(H),
+                                                                  nn.Linear(H, H), Act(), nn.LayerNorm(H)]
+
+    def make(d):
+        if recurrent:
+            return tuple(m.to(dev) for m in (nn.Sequential(*base(d)), nn.GRU(H, H), nn.LayerNorm(H), nn.Linear(H, 1)))
+        return nn.Sequential(*base(d), nn.Linear(H, 1)).to(dev)
+
+    crits = [make(nw.obs_dims[0])] * A if shared else [make(od) for od in nw.obs_dims]
+    critic = crits[0] if shared else crits
+    central = make(sum(nw.obs_dims))
+    h0 = torch.zeros(1, n, H, device=dev)
+
+    def in_kernel():
+        env.rollout_policy(mods, T, critic=critic, centralized_critic=False, **kw)
+
+    def actor_only():
+        return env.rollout_policy(mods, T, record_observations=recurrent, **kw)
+
+    def kernel_then_torch():
+        obs_n, _, _, _, ex = env.rollout_policy(mods, T, record_observations=True, **kw)
+        with torch.no_grad():
+            for k, c in enumerate(crits):
+                x = ex["observations"][k].reshape(T * n, -1)
+                if recurrent:
+                    b, gru, norm, v_out = c
+                    out, hT = gru(b(x).reshape(T, n, H), h0)
+                    v_out(norm(out))
+                    _, hb = gru(b(obs_n[k])[None], hT)
+                    v_out(norm(hb[0]))
+                else:
+                    c(x)
+                    c(obs_n[k])
+
+    def centralized():
+        env.rollout_policy(mods, T, critic=central, **kw)
+
+    def timed(fn):
+        for _ in range(2):
+            fn()
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(args.reps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / 1e3 / (args.reps * T)
+
+    res["config"].update(torch_float32_matmul_precision=torch.get_float32_matmul_precision(),
+                         local_critics="shared" if shared else "per_agent")
+    sa, so, sb = timed(in_kernel), timed(actor_only), timed(kernel_then_torch)
+    res["in_kernel_local_critic"] = {"us_per_step": 1e6 * sa, "env_steps_per_sec": n / sa}
+    res["in_kernel_actor_only" + ("_recording_observations" if recurrent else "")] = \
+        {"us_per_step": 1e6 * so, "env_steps_per_sec": n / so}
+    res["kernel_then_torch_local_critic"] = {"us_per_step": 1e6 * sb, "env_steps_per_sec": n / sb}
+    res["local_critic_us_per_step"] = 1e6 * (sa - so)
+    res["speedup"] = sb / sa
+    try:
+        sc = timed(centralized)
+        res["in_kernel_centralized_critic"] = {"us_per_step": 1e6 * sc, "env_steps_per_sec": n / sc}
+    except MpeError as e:   # spread N=6: no centralized critic kernel
+        res["in_kernel_centralized_critic"] = {"error": str(e)}
+    if shared and not recurrent:   # one critic per agent, local and centralized, where they fit next to the actor
+        per_agent = {"in_kernel_local_critic_per_agent": ([make(od) for od in nw.obs_dims], False),
+                     "in_kernel_centralized_critic_per_agent": ([make(sum(nw.obs_dims)) for _ in range(A)], True)}
+        for name, (cs, cen) in per_agent.items():
+            try:
+                s = timed(lambda: env.rollout_policy(mods, T, critic=cs, centralized_critic=cen, **kw))
+                res[name] = {"us_per_step": 1e6 * s, "env_steps_per_sec": n / s}
+            except MpeError as e:
+                res[name] = {"error": str(e)}
+    res["card"] = card_info()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scenario", default="simple_spread")
@@ -196,14 +294,15 @@ def main():
     ap.add_argument("--feature-norm", action="store_true", help="MAPPO's actor with the input LayerNorm")
     ap.add_argument("--separated", action="store_true",
                     help="rMAPPO's separated runner: one recurrent actor (and critic) per agent (--actor rmappo)")
-    ap.add_argument("--critic", choices=("shared", "separated", "recurrent"),
+    ap.add_argument("--critic", choices=("shared", "separated", "recurrent", "local", "recurrent-local"),
                     help="time MAPPO's centralized critic in-kernel against the torch critic after the rollout "
-                         "(shared, separated: --actor mappo; recurrent: --actor rmappo)")
+                         "(shared, separated: --actor mappo; recurrent: --actor rmappo), or IPPO's local critics "
+                         "(local: --actor mappo; recurrent-local: --actor rmappo)")
     args = ap.parse_args()
-    if args.critic in ("shared", "separated") and args.actor != "mappo":
-        ap.error("--critic shared|separated needs --actor mappo")
-    if args.critic == "recurrent" and args.actor != "rmappo":
-        ap.error("--critic recurrent needs --actor rmappo")
+    if args.critic in ("shared", "separated", "local") and args.actor != "mappo":
+        ap.error("--critic shared|separated|local needs --actor mappo")
+    if args.critic in ("recurrent", "recurrent-local") and (args.actor != "rmappo" or args.separated):
+        ap.error("--critic recurrent|recurrent-local needs --actor rmappo (recurrent-local: without --separated)")
     if args.separated and args.actor != "rmappo":
         ap.error("--separated needs --actor rmappo")
     if args.actor in ("mappo", "rmappo"):
@@ -291,7 +390,8 @@ def main():
 
     if args.critic:
         res["config"].update(critic=args.critic)
-        timer = time_rcritic if args.critic == "recurrent" else time_critic
+        timer = {"recurrent": time_rcritic, "local": time_local_critic,
+                 "recurrent-local": time_local_critic}.get(args.critic, time_critic)
         res = timer(args, env, mods, kw, res, e0, e1)
         if not args.separated:   # the separated runner's critic arms go with its rollout arms, in the same run
             print(json.dumps(res))

@@ -130,12 +130,14 @@ def main():
     forms = {"mlp_rollout": "S", "mlp_episode": "E", "mlp_categorical": "C", "mlp_categorical_episode": "CE",
              "mappo": "M", "mappo_episode": "ME", "gru": "G", "gru_episode": "GE", "mappo_critic": "V",
              "mappo_critic_episode": "VE", "critic_gru": "R", "gru_separated": "GS", "gru_separated_episode": "GSE",
-             "critic_gru_separated": "RS", "gru_image": "I"}
+             "critic_gru_separated": "RS", "gru_image": "I", "mappo_local_critic": "L",
+             "mappo_local_critic_episode": "LE", "critic_gru_local": "RL"}
     mlp = []
     for mangled, (reg, stack) in usage.items():
         m = re.match(r"void mpe::mpe_(?:policy_)?(mlp_rollout|mlp_episode|mlp_categorical|mlp_categorical_episode|mappo|"
                      r"mappo_episode|gru|gru_episode|mappo_critic|mappo_critic_episode|critic_gru|gru_separated|"
-                     r"gru_separated_episode|critic_gru_separated|gru_image)_kernel<mpe::(.+?)"
+                     r"gru_separated_episode|critic_gru_separated|gru_image|mappo_local_critic|"
+                     r"mappo_local_critic_episode|critic_gru_local)_kernel<mpe::(.+?)"
                      r"(?:, (\d+))?\s*>\(", names[mangled])
         if m:
             c = mix.get(mangled, {})
@@ -148,7 +150,9 @@ def main():
               "recurrent actor `mpe_policy_gru[_episode]_kernel`, V and VE its LayerNorm actor with the centralized critic "
               "`mpe_policy_mappo_critic[_episode]_kernel`, R rMAPPO's recurrent critic `mpe_critic_gru_kernel`, GS and "
               "GSE per-agent recurrent actors `mpe_policy_gru_separated[_episode]_kernel`, RS per-agent recurrent critics "
-              "`mpe_critic_gru_separated_kernel`, I their fragment images `mpe_gru_image_kernel` (all H = 64)\n")
+              "`mpe_critic_gru_separated_kernel`, I their fragment images `mpe_gru_image_kernel`, L and LE the LayerNorm "
+              "actor with IPPO's local critics `mpe_policy_mappo_local_critic[_episode]_kernel`, RL rIPPO's recurrent "
+              "local critic `mpe_critic_gru_local_kernel` (all H = 64)\n")
         print("| program | H | form | regs | stack | instr | HMMA | LDS | MUFU |")
         print("|---|---|---|---|---|---|---|---|---|")
         for r in sorted(mlp):
